@@ -9,9 +9,8 @@
 //   * rays come from a compacted list (queue of path ids / SoA shadow segments) through a shared cursor: a warp refills its idle lanes with
 //     fresh rays (ballot + one atomic per refill) as soon as fewer than kRefillLanes of its 32 lanes are still traversing, instead of waiting
 //     for its longest ray (Aila & Laine's persistent while-while with dynamic fetch, adapted to a queue that stays on the device);
-//   * the per-ray traversal is the SAME near-first stack walk as bvh.h's traverse() — same nodes, same candidate order, same float operations
-//     — because the reference draws one sampler value per candidate hit (rt.cxx:436-457): the parity build runs these kernels too and stays
-//     bit-exact, whichever lane or warp a ray lands in.
+//   * the per-ray traversal is the SAME near-first stack walk as bvh.h's traverse() — same nodes, same candidate order, same float operations.
+// The product build's k_shadow_resolve runs these walks.
 #pragma once
 #include "dtrace.cuh"
 
