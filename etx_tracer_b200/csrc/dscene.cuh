@@ -153,18 +153,31 @@ DEV V2 lerp_uv(const DeviceScene& sc, const TriRec& tri, V3 b) {
 
 // scene.hxx:172-186 shading_pos
 DEV V3 shading_pos_project(V3 position, V3 origin, V3 normal) { return position - dot(position - origin, normal) * normal; }
-DEV V3 shading_pos(const DeviceScene& sc, const TriRec& tri, V3 bc, V3 w_o) {
-  V3 p0v = load_vertex_pos(sc, tri.i0), p1v = load_vertex_pos(sc, tri.i1), p2v = load_vertex_pos(sc, tri.i2);
-  V3 n0 = load_vertex_nrm(sc, tri.i0), n1 = load_vertex_nrm(sc, tri.i1), n2 = load_vertex_nrm(sc, tri.i2);
-  V3 geo_pos = p0v * bc.x + p1v * bc.y + p2v * bc.z;
-  V3 sh_normal = normalize(n0 * bc.x + n1 * bc.y + n2 * bc.z);
-  float direction = (dot(sh_normal, w_o) >= 0.0f) ? +1.0f : -1.0f;
-  V3 p0 = shading_pos_project(geo_pos, p0v, direction * n0);
-  V3 p1 = shading_pos_project(geo_pos, p1v, direction * n1);
-  V3 p2 = shading_pos_project(geo_pos, p2v, direction * n2);
+struct ShadingVerts {
+  V3 p0, p1, p2, n0, n1, n2;
+  V3 geo_pos, sh_normal;
+};
+DEV ShadingVerts load_shading_verts(const DeviceScene& sc, const TriRec& tri, V3 bc) {
+  ShadingVerts v;
+  v.p0 = load_vertex_pos(sc, tri.i0), v.p1 = load_vertex_pos(sc, tri.i1), v.p2 = load_vertex_pos(sc, tri.i2);
+  v.n0 = load_vertex_nrm(sc, tri.i0), v.n1 = load_vertex_nrm(sc, tri.i1), v.n2 = load_vertex_nrm(sc, tri.i2);
+  v.geo_pos = v.p0 * bc.x + v.p1 * bc.y + v.p2 * bc.z;
+  v.sh_normal = normalize(v.n0 * bc.x + v.n1 * bc.y + v.n2 * bc.z);
+  return v;
+}
+// the origin on one side of the surface: direction = +1 when w_o leaves on the side of the shading normal, -1 otherwise
+DEV V3 shading_pos_side(const ShadingVerts& v, const TriRec& tri, V3 bc, float direction) {
+  V3 p0 = shading_pos_project(v.geo_pos, v.p0, direction * v.n0);
+  V3 p1 = shading_pos_project(v.geo_pos, v.p1, direction * v.n1);
+  V3 p2 = shading_pos_project(v.geo_pos, v.p2, direction * v.n2);
   V3 sh_pos = p0 * bc.x + p1 * bc.y + p2 * bc.z;
-  bool convex = dot(sh_pos - geo_pos, sh_normal) * direction > 0.0f;
-  return offset_ray(convex ? sh_pos : geo_pos, tri.geo_n * direction);
+  bool convex = dot(sh_pos - v.geo_pos, v.sh_normal) * direction > 0.0f;
+  return offset_ray(convex ? sh_pos : v.geo_pos, tri.geo_n * direction);
+}
+DEV float shading_pos_direction(V3 sh_normal, V3 w_o) { return (dot(sh_normal, w_o) >= 0.0f) ? +1.0f : -1.0f; }
+DEV V3 shading_pos(const DeviceScene& sc, const TriRec& tri, V3 bc, V3 w_o) {
+  ShadingVerts v = load_shading_verts(sc, tri, bc);
+  return shading_pos_side(v, tri, bc, shading_pos_direction(v.sh_normal, w_o));
 }
 
 // scene.hxx:202-226 make_intersection (incl. normal mapping)

@@ -38,7 +38,7 @@ struct PathBuffers {
   float4* bs_wo_eta;      //         w_o, eta
   uint2* bs_props;        //         properties, medium index
   uint32_t* merge_key;    // camera: per queue slot, Morton code of the merge query's base grid cell (0xffffffff = no merge)
-  uint32_t* conn_seed;    // camera (product build): sampler state the vertex-connection stage derives its per-connection streams from
+  float4* conn_rec;       // camera (product build, connection stage): the ConnRec of the vertex shaded this bounce, kConnRecRows<SP> rows per path
   uint2* shadow_span;     // camera: (first deferred shadow ray, path connections | NEE << 16) of the vertex shaded this bounce
 };
 
@@ -612,9 +612,40 @@ DEV Isect stage_intersection(const LaunchParams& p, const PathState<SP>& state, 
 }
 
 // Scenes with stochastic BSDFs (product build): the camera-vertex x light-vertex connections (vcm_shared.hxx:765-803) become their
-// own wavefront stage, one thread per connection (k_camera_connect); the shade stage only emits the work list.
+// own wavefront stage, one thread per connection (k_camera_connect); the shade stage only emits the work list and the vertex's ConnRec.
+//
+// ConnRec: everything a connection needs from the camera side, prepared once per vertex by the shade stage, where the intersection and
+// the updated MIS state are in registers, and read by each of the vertex's connections (about three per vertex on C3) instead of every
+// connection rebuilding the vertex from the path state, the hit record, the triangle and its vertices.  One 16-B aligned record per path:
+// 224 B spectral, 288 B RGB.  Both kernels access it in place (a copy in registers would spill in either).
 template <bool SP>
-DEV void camera_emit_connections(const LaunchParams& p, uint32_t i, uint32_t camera_material, PathState<SP>& state, uint32_t& connections) {
+struct alignas(16) ConnRec {
+  Closure<SP> closure;  // the prepared camera vertex (make_closure): frame, w_i, wavelength, medium
+  V3 pos;
+  // the two origins shading_pos can return for a shadow ray from this vertex; it picks one by the sign of dot(sh_normal, w_o), and w_o
+  // enters through nothing else
+  V3 sh_normal, origin_front, origin_back;
+  Spec<SP> throughput;
+  float d_vcm, d_vc;
+  uint32_t seed;       // the path's sampler state the per-connection streams are derived from
+  uint32_t lp_offset;  // VCMLightPath::index of the paired light path
+};
+template <bool SP>
+constexpr uint32_t kConnRecRows = uint32_t(sizeof(ConnRec<SP>) / 16u);
+static_assert(sizeof(ConnRec<true>) == 224u && sizeof(ConnRec<false>) == 288u, "ConnRec layout");
+template <bool SP>
+DEV ConnRec<SP>* conn_rec_at(float4* recs, uint32_t i) {
+  return reinterpret_cast<ConnRec<SP>*>(recs + size_t(i) * kConnRecRows<SP>);
+}
+
+// shading_pos(tri, bc, w_o) of the vertex, from its record
+template <bool SP>
+DEV V3 conn_shadow_origin(const ConnRec<SP>& cam, V3 w_o) {
+  return (shading_pos_direction(cam.sh_normal, w_o) > 0.0f) ? cam.origin_front : cam.origin_back;
+}
+
+template <bool SP>
+DEV void camera_emit_connections(const LaunchParams& p, uint32_t i, const Isect& isect, PathState<SP>& state, uint32_t& connections) {
   const DeviceScene& sc = p.scene;
   if (p.vcm.connect_vertices() == false) return;
   uint32_t lp_count = p.paths.lv_count[i];
@@ -624,17 +655,35 @@ DEV void camera_emit_connections(const LaunchParams& p, uint32_t i, uint32_t cam
   if (k_end > k_begin) {
     uint32_t cnt = k_end - k_begin;
     uint32_t base = atomicAdd(p.conn_count, cnt);
+    const uint32_t lp_offset = p.lp_offset[i];
     if (base + cnt <= p.conn_capacity) {
       for (uint32_t k = 0; k < cnt; ++k) p.conn_list[base + k] = make_uint2(i, k_begin + k);
       if (p.conn_key != nullptr) {
-        uint32_t cam_mat = umin(camera_material, 0xffu) << 8;
-        const LightVertexRec* lvs = p.lv_final + p.lp_offset[i] + k_begin;
+        uint32_t cam_mat = umin(isect.material_index, 0xffu) << 8;
+        const LightVertexRec* lvs = p.lv_final + lp_offset + k_begin;
         for (uint32_t k = 0; k < cnt; ++k) p.conn_key[base + k] = cam_mat | umin(__float_as_uint(__ldg(&lvs[k].nrm_mat.w)), 0xffu);
       }
     } else {
       *p.overflow = 1u;
     }
-    p.paths.conn_seed[i] = state.sampler.seed;
+    ConnRec<SP>& rec = *conn_rec_at<SP>(p.paths.conn_rec, i);
+    Smp prep;  // the closure's own stream (RGB thin-film wavelength jitter), as in k_camera_merge_closure
+    prep.seed = state.sampler.seed ^ 0x85ebca6bu;
+    prep.fixed_u = prep.fixed_v = prep.fixed_w = 0.0f;
+    prep.next();
+    BData cam = make_bdata(isect, isect.w_i, state.wavelength, state.medium_index, kPathCamera);
+    rec.closure = make_closure<SP>(sc, cam, isect.material_index, prep);
+    rec.pos = isect.pos;
+    const TriRec tri = load_triangle(sc, isect.triangle_index);
+    const ShadingVerts sv = load_shading_verts(sc, tri, isect.barycentric);
+    rec.sh_normal = sv.sh_normal;
+    rec.origin_front = shading_pos_side(sv, tri, isect.barycentric, +1.0f);
+    rec.origin_back = shading_pos_side(sv, tri, isect.barycentric, -1.0f);
+    rec.throughput = state.throughput;
+    rec.d_vcm = state.d_vcm;
+    rec.d_vc = state.d_vc;
+    rec.seed = state.sampler.seed;
+    rec.lp_offset = lp_offset;
     state.sampler.next();  // the path's own stream moves on by one draw for the whole stage
     connections += cnt;
   }
@@ -759,7 +808,9 @@ __global__ void __launch_bounds__(128, kMinBlocksPerSm) k_camera_shade(const __g
             c = vcm_connect_to_light<SP, PLAIN>(sc, p.vcm, ep, state, stats, shadow_rays, deferred);
             state.sampler.pop_fixed();
           } else if (p.connect_stage && (ep_mode == kEpSurface)) {
-            camera_emit_connections<SP>(p, i, isect.material_index, state, connections);
+#if !(defined(ETXB_PARITY) && ETXB_PARITY)  // the parity build has no connection stage
+            camera_emit_connections<SP>(p, i, isect, state, connections);
+#endif
             continue;
           } else if (deferred && p.shadow_stage) {
             // one slot per connection of this vertex, in the reference's order (vcm_shared.hxx:765-803); k_camera_connect_deferred
@@ -854,10 +905,11 @@ __global__ void __launch_bounds__(128, kMinBlocksPerSm) k_camera_shade(const __g
 
 // vcm_connect_to_light_vertex (vcm_shared.hxx:673-763) on vertex closures: both end points are prepared once and each closure_evaluate returns
 // value, pdf and reverse pdf together (the generic routine re-derives IORs / thin film / tints from the Material record in each of its four
-// evaluate / reverse_pdf calls).  Surface camera vertices only; the light vertex may be a medium vertex.
+// evaluate / reverse_pdf calls).  Surface camera vertices only, prepared by the shade stage (ConnRec); the light vertex may be a medium vertex.
 template <bool SP>
-DEV bool vcm_connect_to_light_vertex_closure(const DeviceScene& sc, const VcmParams& it, PathState<SP>& state, const LightVertexRec& lv, const Isect& cam, V3& target_position,
+DEV bool vcm_connect_to_light_vertex_closure(const DeviceScene& sc, const VcmParams& it, const ConnRec<SP>& cam, const LightVertexRec& lv, Smp& smp, V3& target_position,
   Spec<SP>& value) {
+  const Closure<SP>& cc = cam.closure;
   const uint32_t lv_tri = __float_as_uint(lv.pos_tri.w);
   const bool lv_is_medium = lv_tri == kInvalidIndex;
   const V3 lv_wi = {lv.wi_dvc.x, lv.wi_dvc.y, lv.wi_dvc.z};
@@ -876,9 +928,7 @@ DEV bool vcm_connect_to_light_vertex_closure(const DeviceScene& sc, const VcmPar
   float w_dot_l = 1.0f;
   if (lv_is_medium == false) w_dot_l = -dot(light_v.nrm, w_o);
 
-  BData camera_data = make_bdata(cam, cam.w_i, state.wavelength, state.medium_index, kPathCamera);
-  Closure<SP> cc = make_closure<SP>(sc, camera_data, cam.material_index, state.sampler);
-  CEval<SP> ce = closure_evaluate<SP>(sc, cc, w_o, state.sampler);
+  CEval<SP> ce = closure_evaluate<SP>(sc, cc, w_o, smp);
   if (ce.valid() == false) return false;
   const float camera_area_pdf = ce.pdf * fabsf(w_dot_l) / distance_squared;
 
@@ -887,30 +937,32 @@ DEV bool vcm_connect_to_light_vertex_closure(const DeviceScene& sc, const VcmPar
   if (lv_is_medium) {
     float pf = medium_phase(sc, lv.ids.x, lv_wi, -w_o);
     if (pf <= 0.0f) return false;
-    light_area_pdf = pf * fabsf(dot(cam.nrm, w_o)) / distance_squared;
+    light_area_pdf = pf * fabsf(dot(cc.nrm, w_o)) / distance_squared;
     light_rev_pdf = medium_phase(sc, lv.ids.x, -w_o, lv_wi);
     light_scatter = Spec<SP>::make(pf);
   } else {
-    BData light_data = {light_v.pos, light_v.nrm, light_v.tan, light_v.btn, light_v.tex, lv_wi, state.wavelength, kPathLight, state.medium_index};
-    Closure<SP> lc = make_closure<SP>(sc, light_data, __float_as_uint(lv.nrm_mat.w), state.sampler);
-    CEval<SP> le = closure_evaluate<SP>(sc, lc, -w_o, state.sampler);
+    BData light_data = {light_v.pos, light_v.nrm, light_v.tan, light_v.btn, light_v.tex, lv_wi, cc.wavelength, kPathLight, cc.medium};
+    Closure<SP> lc = make_closure<SP>(sc, light_data, __float_as_uint(lv.nrm_mat.w), smp);
+    CEval<SP> le = closure_evaluate<SP>(sc, lc, -w_o, smp);
     if (le.valid() == false) return false;
-    light_area_pdf = le.pdf * fabsf(dot(cam.nrm, w_o)) / distance_squared;
+    light_area_pdf = le.pdf * fabsf(dot(cc.nrm, w_o)) / distance_squared;
     light_rev_pdf = le.rev_pdf;
     light_scatter = le.bsdf * fix_shading_normal(light_tri.geo_n, light_data.nrm, light_data.w_i, -w_o);
   }
   float vmW_pair = lv_is_medium ? 0.0f : it.vm_weight;
   float w_light = camera_area_pdf * (vmW_pair + lv.thr_dvcm.w + lv.wi_dvc.w * light_rev_pdf);
-  float w_camera = light_area_pdf * (vmW_pair + state.d_vcm + state.d_vc * ce.rev_pdf);
+  float w_camera = light_area_pdf * (vmW_pair + cam.d_vcm + cam.d_vc * ce.rev_pdf);
   float weight = it.enable_mis() ? 1.0f / (1.0f + w_light + w_camera) : 1.0f;
   Spec<SP> lv_throughput = Spec<SP>::make3({lv.thr_dvcm.x, lv.thr_dvcm.y, lv.thr_dvcm.z});
-  value = (ce.bsdf * state.throughput) * (light_scatter * lv_throughput) * (weight / distance_squared);
+  value = (ce.bsdf * cam.throughput) * (light_scatter * lv_throughput) * (weight / distance_squared);
   return true;
 }
 
+#if !(defined(ETXB_PARITY) && ETXB_PARITY)
 // Product build: one thread per (camera vertex, light vertex) connection — vcm_connect_to_light_vertex + the shadow ray of
-// vcm_connect_to_light_path (vcm_shared.hxx:673-803).  Each connection draws from its own stream derived from the path's sampler
-// (the reference shares one stream across the serial loop; the parity build keeps that order inside k_camera_shade).
+// vcm_connect_to_light_path (vcm_shared.hxx:673-803).  The camera side comes prepared from the vertex's ConnRec.  Each connection draws
+// from its own stream derived from the path's sampler (the reference shares one stream across the serial loop; the parity build keeps
+// that order inside k_camera_shade and has no connection stage).
 template <bool SP, bool PLAIN>
 __global__ void __launch_bounds__(128, kMinBlocksPerSm) k_camera_connect(const __grid_constant__ LaunchParams p, const uint2* conn_list) {
   uint32_t shadow_rays = 0;
@@ -922,28 +974,23 @@ __global__ void __launch_bounds__(128, kMinBlocksPerSm) k_camera_connect(const _
   for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < total; t += gridDim.x * blockDim.x) {
     uint2 entry = conn_list[t];
     uint32_t i = entry.x;
-    PathState<SP> state = load_state<SP>(p.paths, i);
-    float4 hit = p.paths.hit[i];
-    Isect isect = make_intersection(sc, state.ray_d, __float_as_uint(hit.w), hit.x, hit.y, hit.z);
-    state.sampler.seed = p.paths.conn_seed[i] ^ ((entry.y + 1u) * 0x9E3779B1u);
-    state.sampler.next();
-    LightVertexRec lv = load_light_vertex(p.lv_final + p.lp_offset[i] + entry.y);
-    Endpoint ep{false, &isect, {0.0f, 0.0f, 0.0f}};
+    const ConnRec<SP>& cam = *conn_rec_at<SP>(p.paths.conn_rec, i);
+    Smp smp;
+    smp.seed = cam.seed ^ ((entry.y + 1u) * 0x9E3779B1u);
+    smp.fixed_u = smp.fixed_v = smp.fixed_w = 0.0f;
+    smp.next();
+    LightVertexRec lv = load_light_vertex(p.lv_final + cam.lp_offset + entry.y);
     V3 target_position;
     Spec<SP> value;
-#if defined(ETXB_PARITY) && ETXB_PARITY
-    const bool connected = vcm_connect_to_light_vertex<SP>(sc, p.vcm, state, lv, ep, target_position, value);
-#else
-    const bool connected = vcm_connect_to_light_vertex_closure<SP>(sc, p.vcm, state, lv, isect, target_position, value);
-#endif
-    if (connected && PLAIN && p.shadow_atomic) {
-      shadow_rays += 1;
-      V3 p0 = shading_pos(sc, load_triangle(sc, isect.triangle_index), isect.barycentric, normalize(target_position - isect.pos));
+    if (vcm_connect_to_light_vertex_closure<SP>(sc, p.vcm, cam, lv, smp, target_position, value) == false) continue;
+    shadow_rays += 1;
+    const V3 p0 = conn_shadow_origin<SP>(cam, normalize(target_position - cam.pos));
+    if (PLAIN && p.shadow_atomic) {
       ShadowBatch batch = {p.shadow_p0, p.shadow_p1, p.shadow_value, 0u, 0u, p.shadow_count, p.shadow_capacity, i};
       batch.push<SP>(p0, target_position, value);
-    } else if (connected) {
-      shadow_rays += 1;
-      Spec<SP> tr = vcm_connection_transmittance<SP, PLAIN>(sc, ep, lv, target_position, state, stats);
+    } else {
+      // vcm_connection_transmittance from a surface vertex
+      Spec<SP> tr = trace_transmittance<SP, PLAIN>(sc, cam.closure.wavelength, p0, target_position, cam.closure.medium, smp, stats);
       if (tr.is_zero() == false) {
         V3 v = (tr * value).as_v3();
         float* dst = reinterpret_cast<float*>(p.paths.gathered + i);
@@ -959,6 +1006,7 @@ __global__ void __launch_bounds__(128, kMinBlocksPerSm) k_camera_connect(const _
   counter_add(&p.counters->nodes, STATS_NODES);
   counter_add(&p.counters->tris, STATS_TRIS);
 }
+#endif
 
 // Scenes with deferred shadow rays (no stochastic BSDF, no media): the connections of vcm_connect_to_light_path (vcm_shared.hxx:765-803)
 // one per thread.  Shadow slot `t` of the bounce was reserved by the shade stage; conn_list[t] names its (path, light vertex) pair.  A

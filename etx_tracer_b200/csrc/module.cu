@@ -137,7 +137,8 @@ struct etxb_ctx {
   DevBuf<float> wavelength;
   DevBuf<uint32_t> queue_sorted, queue_keys, queue_keys_sorted;  // path queue grouped by hit material (scenes with stochastic BSDFs)
   DevBuf<uint2> conn_list_sorted;
-  DevBuf<uint32_t> lv_count, lp_offset, queue_a, queue_b, queue_counts, sampler_end_light, sampler_end_camera, merge_key, conn_seed, conn_count;
+  DevBuf<uint32_t> lv_count, lp_offset, queue_a, queue_b, queue_counts, sampler_end_light, sampler_end_camera, merge_key, conn_count;
+  DevBuf<float4> conn_rec;  // product build, scenes with a connection stage: kConnRecRows rows per path (kernels.cuh)
   DevBuf<uint2> conn_list, shadow_span;
   DevBuf<float4> shadow_p0, shadow_p1, shadow_value;
   DevBuf<uint32_t> shadow_result, shadow_count, trace_cursor;  // trace_cursor: work cursor of k_shadow_resolve
@@ -336,7 +337,7 @@ LaunchParams make_params(etxb_ctx* ctx) {
   LaunchParams p = {};
   p.scene = ctx->dscene;
   p.paths = {ctx->ray_o.ptr, ctx->ray_d.ptr, ctx->thr.ptr, ctx->mis.ptr, ctx->misc.ptr, ctx->hit.ptr, ctx->gathered.ptr, ctx->merged.ptr, ctx->wavelength.ptr,
-    ctx->lv_count.ptr, ctx->bs_weight_pdf.ptr, ctx->bs_wo_eta.ptr, ctx->bs_props.ptr, ctx->merge_key.ptr, ctx->conn_seed.ptr};
+    ctx->lv_count.ptr, ctx->bs_weight_pdf.ptr, ctx->bs_wo_eta.ptr, ctx->bs_props.ptr, ctx->merge_key.ptr, ctx->conn_rec.ptr};
   p.film = {ctx->film_camera.ptr, ctx->film_light.ptr, ctx->film_light_iteration.ptr, ctx->width, ctx->height};
   p.grid = ctx->grid;
   p.lv_tmp = ctx->lv_tmp.ptr;
@@ -644,6 +645,7 @@ int run_camera_pass(etxb_ctx* ctx) {
       uint32_t blocks = std::min<uint32_t>(ctx->sm_count * 8u, blocks_for(std::min<uint64_t>(uint64_t(active) * 32ull, 0x7fffffffull), 256));
       k_shadow_trace<<<blocks, 256, 0, ctx->stream>>>(p);
     }
+#if !(defined(ETXB_PARITY) && ETXB_PARITY)  // make_params: the parity build has no connection stage
     if (p.connect_stage && (ctx->options.options & ETXB_VCM_CONNECT_VERTICES)) {
       if (active < kTailQueue) {
         // tail of the pass: the pair count stays on the device (k_camera_connect is grid-stride), no host round trip per bounce
@@ -677,6 +679,7 @@ int run_camera_pass(etxb_ctx* ctx) {
         }
       }
     }
+#endif
     if (p.shadow_atomic) {
       // emitter-sample and vertex-connection segments of this bounce: traced, the unoccluded ones added to their paths' gathered sums
       LaunchTimer t(ctx, K_SHADOW_TRACE);
@@ -1002,10 +1005,10 @@ void etxb_destroy(etxb_ctx* ctx) {
   cudaEventDestroy(ctx->ev_iter_start);
   cudaEventDestroy(ctx->ev_iter_stop);
   DevBuf<float4>* f4[] = {&ctx->ray_o, &ctx->ray_d, &ctx->thr, &ctx->mis, &ctx->hit, &ctx->gathered, &ctx->merged, &ctx->camera_value, &ctx->bvh_tris, &ctx->g_pos, &ctx->g_nrm,
-    &ctx->g_win, &ctx->g_thr, &ctx->film_camera, &ctx->film_light, &ctx->film_light_iteration, &ctx->film_out};
+    &ctx->g_win, &ctx->g_thr, &ctx->film_camera, &ctx->film_light, &ctx->film_light_iteration, &ctx->film_out, &ctx->conn_rec};
   for (auto* b : f4) b->release();
   DevBuf<uint32_t>* u32[] = {&ctx->tri_emitter, &ctx->lv_count, &ctx->lp_offset, &ctx->queue_a, &ctx->queue_b, &ctx->queue_counts, &ctx->sampler_end_light,
-    &ctx->sampler_end_camera, &ctx->merge_key, &ctx->conn_seed, &ctx->conn_count, &ctx->lv_tmp_count, &ctx->overflow, &ctx->grid_bbox, &ctx->keys_in, &ctx->keys_out, &ctx->vals_in, &ctx->vals_out};
+    &ctx->sampler_end_camera, &ctx->merge_key, &ctx->conn_count, &ctx->lv_tmp_count, &ctx->overflow, &ctx->grid_bbox, &ctx->keys_in, &ctx->keys_out, &ctx->vals_in, &ctx->vals_out};
   for (auto* b : u32) b->release();
   ctx->vertices.release();
   ctx->triangles.release();
@@ -1389,7 +1392,7 @@ int etxb_upload_scene(etxb_ctx* ctx, const void* scene_blob, uint64_t scene_byte
   CUDA_OK(ctx, ctx->bs_props.alloc(n));
   CUDA_OK(ctx, ctx->misc.alloc(n));
   CUDA_OK(ctx, ctx->wavelength.alloc(n));
-  DevBuf<uint32_t>* per_path_u32[] = {&ctx->lv_count, &ctx->lp_offset, &ctx->queue_a, &ctx->queue_b, &ctx->sampler_end_light, &ctx->sampler_end_camera, &ctx->merge_key, &ctx->conn_seed};
+  DevBuf<uint32_t>* per_path_u32[] = {&ctx->lv_count, &ctx->lp_offset, &ctx->queue_a, &ctx->queue_b, &ctx->sampler_end_light, &ctx->sampler_end_camera, &ctx->merge_key};
   for (auto* b : per_path_u32) CUDA_OK(ctx, b->alloc(n));
   CUDA_OK(ctx, ctx->conn_count.alloc(1));
   CUDA_OK(ctx, ctx->queue_counts.alloc(4));
@@ -1414,6 +1417,16 @@ int etxb_upload_scene(etxb_ctx* ctx, const void* scene_blob, uint64_t scene_byte
     ctx->queue_keys.release();
     ctx->queue_keys_sorted.release();
   }
+#if defined(ETXB_PARITY) && ETXB_PARITY
+  ctx->conn_rec.release();
+#else
+  // the connection stage's per-path camera vertex records (make_params: connect_stage = has_stochastic_merge)
+  if (ctx->has_stochastic_merge) {
+    CUDA_OK(ctx, ctx->conn_rec.alloc(n * (ctx->spectral ? kConnRecRows<true> : kConnRecRows<false>)));
+  } else {
+    ctx->conn_rec.release();
+  }
+#endif
   CUDA_OK(ctx, ctx->trace_cursor.alloc(1));
   const bool atomic_candidate = ctx->opaque_scene && ctx->plain_scene && ctx->has_stochastic_merge;
   if (ctx->dscene.deferred_shadow_rays || atomic_candidate) {
