@@ -122,6 +122,7 @@ def load_library(flavor="fast"):
     lib.etxb_stream.argtypes = [vp]
     lib.etxb_debug_trace.argtypes = [vp, vp, vp, u32, vp, vp]
     lib.etxb_debug_select_tree.argtypes = [vp, C.c_int]
+    lib.etxb_debug_occluded.argtypes = [vp, vp, u32, vp]
     lib.etxb_debug_sampler.argtypes = [vp, vp, vp, u32, u32, vp, vp]
     lib.etxb_debug_math.argtypes = [vp, u32, vp, vp, u32, vp]
     _libs[flavor] = lib
@@ -432,7 +433,8 @@ class GPUVCM:
 
     # -- unit entry points (parity tests) -----------------------------------------------------------------
     def debug_select_tree(self, wide):
-        """etxb_debug_trace walks the BVH2 (False) or the product build's 4-wide quantised tree (True); returns whether that tree exists."""
+        """etxb_debug_trace / etxb_debug_occluded walk the BVH2 (False) or the product build's 4-wide quantised tree (True); returns whether that
+        tree exists."""
         return self.lib.etxb_debug_select_tree(self.h, 1 if wide else 0) == 1
 
     def debug_trace(self, rays, seeds):
@@ -443,6 +445,14 @@ class GPUVCM:
         tri = np.zeros(n, dtype=np.uint32)
         self._check(self.lib.etxb_debug_trace(self.h, _p(rays), _p(seeds), n, _p(uvt), _p(tri)))
         return uvt, tri, seeds
+
+    def debug_occluded(self, segments):
+        """segments: float32 (n, 6) rows {p0, p1}; returns a bool per segment: is a non-Void surface between p0 and p1?"""
+        segments = np.ascontiguousarray(segments, dtype=np.float32)
+        n = segments.shape[0]
+        out = np.zeros(n, dtype=np.uint32)
+        self._check(self.lib.etxb_debug_occluded(self.h, _p(segments), n, _p(out)))
+        return out != 0
 
     def debug_sampler(self, a, b, draws):
         a = np.ascontiguousarray(a, dtype=np.uint32)

@@ -19,9 +19,14 @@
 
 namespace etxb {
 
-// resident blocks per SM the bounce / connection kernels and the closure gather are compiled for (128 threads each: 4 blocks = 128 registers
-// per thread).
+// resident blocks per SM the 128-thread bounce / connection kernels and the closure gather are compiled for (4 blocks = 128 registers per thread)
 constexpr int kMinBlocksPerSm = 4;
+// the PLAIN instantiations of the bounce / connection kernels (no media, boundaries or subsurface: C3) get 2 blocks = up to 255 registers.  At
+// 128 registers k_camera_shade and k_camera_connect spilled 0.5-2.7 KB per thread; with the registers they need they are faster on the H100
+// despite the lower occupancy (C3: k_camera_connect 14.1 -> 11.9 ms, k_camera_shade 24.1 -> 23.0 ms per iteration).  The general
+// instantiations (C4) are slower at 2 blocks (k_camera_shade 33.7 -> 40.1 ms) and keep 4, as does the closure gather (19.7 -> 26.4 ms at 2).
+template <bool PLAIN>
+constexpr int kBounceMinBlocksPerSm = PLAIN ? 2 : kMinBlocksPerSm;
 
 struct PathBuffers {
   float4* ray_o;     // o.xyz, min_t
@@ -286,7 +291,7 @@ enum : uint32_t { kEpNone = 0u, kEpMedium = 1u, kEpSurface = 2u, kEpSubsurface =
 // the segment (medium scattering, boundary crossing, surface hit incl. the subsurface walk), (B) camera connections from the
 // endpoint(s) it produced — one, or every gathered subsurface exit (:1207-1222), (C) the continuation.
 template <bool SP, bool PLAIN>
-__global__ void __launch_bounds__(128, kMinBlocksPerSm) k_light_bounce(const __grid_constant__ LaunchParams p, const uint32_t* queue_in, const uint32_t* count_in, uint32_t* queue_out, uint32_t* count_out) {
+__global__ void __launch_bounds__(128, kBounceMinBlocksPerSm<PLAIN>) k_light_bounce(const __grid_constant__ LaunchParams p, const uint32_t* queue_in, const uint32_t* count_in, uint32_t* queue_out, uint32_t* count_out) {
   uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
   bool alive = false;
   uint32_t i = 0;
@@ -693,7 +698,7 @@ DEV void camera_emit_connections(const LaunchParams& p, uint32_t i, const Isect&
 // the paired light path and to a sampled emitter from the endpoint(s) the event produced (one, or every gathered subsurface exit,
 // :1037-1053), (C) the MIS update / pending continuation sample handed to the merge and continue stages.
 template <bool SP, bool PLAIN>
-__global__ void __launch_bounds__(128, kMinBlocksPerSm) k_camera_shade(const __grid_constant__ LaunchParams p, const uint32_t* queue_in, const uint32_t* count_in) {
+__global__ void __launch_bounds__(128, kBounceMinBlocksPerSm<PLAIN>) k_camera_shade(const __grid_constant__ LaunchParams p, const uint32_t* queue_in, const uint32_t* count_in) {
   uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
   uint32_t shadow_rays = 0, connections = 0;
   uint32_t merge_key = 0xffffffffu;
@@ -964,7 +969,7 @@ DEV bool vcm_connect_to_light_vertex_closure(const DeviceScene& sc, const VcmPar
 // from its own stream derived from the path's sampler (the reference shares one stream across the serial loop; the parity build keeps
 // that order inside k_camera_shade and has no connection stage).
 template <bool SP, bool PLAIN>
-__global__ void __launch_bounds__(128, kMinBlocksPerSm) k_camera_connect(const __grid_constant__ LaunchParams p, const uint2* conn_list) {
+__global__ void __launch_bounds__(128, kBounceMinBlocksPerSm<PLAIN>) k_camera_connect(const __grid_constant__ LaunchParams p, const uint2* conn_list) {
   uint32_t shadow_rays = 0;
   STATS_DECL;
   const DeviceScene& sc = p.scene;
@@ -1743,7 +1748,7 @@ __global__ void k_debug_trace(const __grid_constant__ DeviceScene sc, const floa
   hits_uv_t[size_t(i) * 3 + 2] = hit ? h.t : 0.0f;
 }
 
-// the same query through the 4-wide quantised tree (product build, scenes that have one)
+// the same query through the 4-wide quantised tree (product build, scenes that have one): the walk k_trace_closest_wide runs (dwide.cuh)
 __global__ void k_debug_trace_wide(const __grid_constant__ DeviceScene sc, const float* rays, uint32_t* seeds, uint32_t count, float* hits_uv_t, uint32_t* hits_tri) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= count) return;
@@ -1766,6 +1771,37 @@ __global__ void k_debug_trace_wide(const __grid_constant__ DeviceScene sc, const
   hits_uv_t[size_t(i) * 3 + 0] = hit ? h.u : 0.0f;
   hits_uv_t[size_t(i) * 3 + 1] = hit ? h.v : 0.0f;
   hits_uv_t[size_t(i) * 3 + 2] = hit ? h.t : 0.0f;
+}
+
+// occlusion of segments (p0, p1: 6 floats each), as k_shadow_resolve tests them: any non-Void surface in between; through the 4-wide
+// quantised tree when `wide` (product build, scenes that have one), the BVH2 otherwise
+__global__ void k_debug_occluded(const __grid_constant__ DeviceScene sc, const float* segments, uint32_t count, uint32_t wide, uint32_t* occluded) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  const float* s = segments + size_t(i) * 6;
+  const V3 p0 = {s[0], s[1], s[2]}, p1 = {s[3], s[4], s[5]};
+  if (!wide) {
+    occluded[i] = trace_occluded(sc, p0, p1) ? 1u : 0u;
+    return;
+  }
+  V3 direction = p1 - p0;
+  float t_max = dot(direction, direction);
+  if (t_max <= kRayEpsilon) {
+    occluded[i] = 0u;  // a degenerate segment is unoccluded (rt.cxx:474-477)
+    return;
+  }
+  t_max = sqrtf(t_max);
+  direction /= t_max;
+  t_max -= fmaxf(kRayEpsilon, t_max * kRayEpsilon);
+  OcclusionVisitor visit{sc, false};
+  const WideNodes nodes{nullptr, sc.wide_nodes, 0u};
+  WideWalk walk;
+  WideHit stack[kWideStackSize];
+  uint32_t n_nodes = 0, n_tris = 0;
+  wide_begin(walk, p0, direction, kRayEpsilon, t_max);
+  while (!wide_step(walk, stack, nodes, sc.bvh_tris, visit, n_nodes, n_tris)) {
+  }
+  occluded[i] = visit.occluded ? 1u : 0u;
 }
 
 __global__ void k_debug_sampler(const uint32_t* a, const uint32_t* b, uint32_t count, uint32_t draws, uint32_t* out_seed, float* out_values) {

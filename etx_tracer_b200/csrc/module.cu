@@ -2047,7 +2047,27 @@ int etxb_debug_trace(etxb_ctx* ctx, const float* rays, uint32_t* seeds, uint32_t
   return ETXB_OK;
 }
 
-// Test hook: which tree etxb_debug_trace walks (0: the BVH2 shared with the oracle; 1: the 4-wide quantised tree of the product build).  Returns 1
+int etxb_debug_occluded(etxb_ctx* ctx, const float* segments, uint32_t count, uint32_t* occluded) {
+  if (!ctx || !segments || !occluded) return ETXB_ERR_INVALID_ARGUMENT;
+  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
+  if (count == 0) return ETXB_OK;
+  cudaSetDevice(ctx->device);
+  DevBuf<float> d_segments;
+  DevBuf<uint32_t> d_occluded;
+  CUDA_OK(ctx, d_segments.alloc(size_t(count) * 6));
+  CUDA_OK(ctx, d_occluded.alloc(count));
+  CUDA_OK(ctx, cudaMemcpy(d_segments.ptr, segments, d_segments.bytes(), cudaMemcpyHostToDevice));
+  const uint32_t wide = (ctx->debug_trace_wide && (ctx->dscene.wide_nodes != nullptr)) ? 1u : 0u;
+  k_debug_occluded<<<blocks_for(count, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_segments.ptr, count, wide, d_occluded.ptr);
+  ctx->kernel_launches += 1;
+  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+  CUDA_OK(ctx, cudaMemcpy(occluded, d_occluded.ptr, d_occluded.bytes(), cudaMemcpyDeviceToHost));
+  d_segments.release();
+  d_occluded.release();
+  return ETXB_OK;
+}
+
+// Test hook: which tree etxb_debug_trace and etxb_debug_occluded walk (0: the BVH2 shared with the oracle; 1: the 4-wide quantised tree of the product build).  Returns 1
 // when the requested tree exists for the uploaded scene.
 int etxb_debug_select_tree(etxb_ctx* ctx, int wide) {
   if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;

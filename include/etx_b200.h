@@ -454,7 +454,11 @@ void* etxb_stream(etxb_ctx* ctx); /* cudaStream_t the module launches on */
 /* Closest-hit query for `count` rays (rt.cxx:428 Raytracing::trace): rays = float[8]*count {o,min_t,d,max_t},
  * seeds in/out = sampler state per ray; hits out = {u, v, tri, t} (IntersectionBase, math.hxx:666). */
 int etxb_debug_trace(etxb_ctx* ctx, const float* rays, uint32_t* seeds, uint32_t count, float* hits_uv_t, uint32_t* hits_tri);
-/* Which tree etxb_debug_trace walks: 0 = the BVH2 shared with the oracle, 1 = the product build's 4-wide quantised tree (returns 1 if it exists). */
+/* Occlusion query for `count` segments (rt.cxx:468 Raytracing::trace_transmittance in an opaque scene): segments = float[6]*count {p0,p1};
+ * occluded out = 1 where a non-Void surface lies between p0 and p1, else 0. */
+int etxb_debug_occluded(etxb_ctx* ctx, const float* segments, uint32_t count, uint32_t* occluded);
+/* Which tree etxb_debug_trace and etxb_debug_occluded walk: 0 = the BVH2 shared with the oracle, 1 = the product build's 4-wide quantised tree
+ * (returns 1 if it exists). */
 int etxb_debug_select_tree(etxb_ctx* ctx, int wide);
 /* Sampler / spectral KATs evaluated on the device (sampler.hxx:54,66; spectrum.hxx:219,234). */
 int etxb_debug_sampler(etxb_ctx* ctx, const uint32_t* a, const uint32_t* b, uint32_t count, uint32_t draws, uint32_t* out_seed, float* out_values);
