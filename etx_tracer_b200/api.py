@@ -125,6 +125,7 @@ def load_library(flavor="fast"):
     lib.etxb_debug_occluded.argtypes = [vp, vp, u32, vp]
     lib.etxb_debug_sampler.argtypes = [vp, vp, vp, u32, u32, vp, vp]
     lib.etxb_debug_math.argtypes = [vp, u32, vp, vp, u32, vp]
+    lib.etxb_debug_closure_eval.argtypes = [vp, vp, u32, u32, vp]
     _libs[flavor] = lib
     return lib
 
@@ -468,6 +469,14 @@ class GPUVCM:
         out = np.zeros_like(x)
         yy = np.ascontiguousarray(y, dtype=np.float32) if y is not None else None
         self._check(self.lib.etxb_debug_math(self.h, fn, _p(x), _p(yy) if yy is not None else None, x.shape[0], _p(out)))
+        return out
+
+    def debug_closure(self, queries, repetitions):
+        """The vertex closures (make_closure + closure_evaluate) for S.CLOSURE_QUERY records on the uploaded scene, `repetitions` fresh
+        samplers per query; returns float64 (n, S.CLOSURE_STATS), laid out as etxb_debug_closure_eval documents (include/etx_b200.h)."""
+        queries = np.ascontiguousarray(queries, dtype=S.CLOSURE_QUERY)
+        out = np.zeros((queries.shape[0], S.CLOSURE_STATS), dtype=np.float64)
+        self._check(self.lib.etxb_debug_closure_eval(self.h, _p(queries), queries.shape[0], int(repetitions), _p(out)))
         return out
 
 

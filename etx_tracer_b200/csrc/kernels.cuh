@@ -1842,4 +1842,54 @@ __global__ void k_debug_math(const __grid_constant__ DeviceScene sc, uint32_t fn
   out[i] = r;
 }
 
+// one thread per etxb_closure_query: `reps` times make_closure + closure_evaluate on a fresh sampler Smp::init(seed, r), as the photon gather
+// and the vertex connections call them; float64 running moments (Welford: a constant output keeps a variance of exactly 0) of
+// {func.rgb, bsdf.rgb, pdf, rev_pdf}, repetition 0's raw values and the counters of include/etx_b200.h (ETXB_CLOSURE_STATS per query)
+template <bool SP>
+__global__ void k_debug_closure(const __grid_constant__ DeviceScene sc, const etxb_closure_query* queries, uint32_t count, uint32_t reps, double* out) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  const etxb_closure_query& q = queries[i];
+  const V3 nrm = {q.nrm[0], q.nrm[1], q.nrm[2]}, tan = {q.tan[0], q.tan[1], q.tan[2]}, btn = {q.btn[0], q.btn[1], q.btn[2]};
+  const V3 w_i = {q.w_i[0], q.w_i[1], q.w_i[2]}, w_o = {q.w_o[0], q.w_o[1], q.w_o[2]};
+  const BData d = {{0.0f, 0.0f, 0.0f}, nrm, tan, btn, {q.uv[0], q.uv[1]}, w_i, SP ? q.wavelength : -1.0f, q.path_source, kInvalidIndex};
+  double mean[8], m2[8];
+  double* o = out + size_t(i) * ETXB_CLOSURE_STATS;
+  for (uint32_t k = 0; k < 8; ++k) mean[k] = m2[k] = 0.0;
+  uint32_t finite = 0, nonfinite = 0, negative = 0, unsupported = 0;
+  for (uint32_t r = 0; r < reps; ++r) {
+    Smp smp;
+    smp.init(q.seed, r);
+    const Closure<SP> c = make_closure<SP>(sc, d, q.material, smp);
+    const CEval<SP> e = closure_evaluate<SP>(sc, c, w_o, smp);
+    const V3 f = e.func.as_v3(), b = e.bsdf.as_v3();
+    const float v[8] = {f.x, f.y, f.z, b.x, b.y, b.z, e.pdf, e.rev_pdf};
+    if (r == 0) {
+      for (uint32_t k = 0; k < 8; ++k) o[16 + k] = v[k];
+    }
+    bool ok = true;
+    for (uint32_t k = 0; k < 8; ++k) ok = ok && isfinite(v[k]);
+    negative += ((e.pdf < 0.0f) || (e.rev_pdf < 0.0f)) ? 1u : 0u;
+    unsupported += ((e.pdf == 0.0f) && ((f.x != 0.0f) || (f.y != 0.0f) || (f.z != 0.0f) || (b.x != 0.0f) || (b.y != 0.0f) || (b.z != 0.0f))) ? 1u : 0u;
+    if (!ok) {
+      nonfinite += 1u;
+      continue;
+    }
+    finite += 1u;
+    for (uint32_t k = 0; k < 8; ++k) {
+      const double delta = double(v[k]) - mean[k];
+      mean[k] += delta / double(finite);
+      m2[k] += delta * (double(v[k]) - mean[k]);
+    }
+  }
+  for (uint32_t k = 0; k < 8; ++k) {
+    o[k] = mean[k];
+    o[8 + k] = (finite > 0) ? m2[k] / double(finite) : 0.0;
+  }
+  o[24] = double(nonfinite);
+  o[25] = double(negative);
+  o[26] = double(unsupported);
+  for (uint32_t k = 27; k < ETXB_CLOSURE_STATS; ++k) o[k] = 0.0;
+}
+
 }  // namespace etxb

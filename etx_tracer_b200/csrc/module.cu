@@ -2119,6 +2119,34 @@ int etxb_debug_math(etxb_ctx* ctx, uint32_t fn, const float* x, const float* y, 
   return ETXB_OK;
 }
 
+// Test hook: the vertex closures of dclosure.cuh, query by query (layout and outputs in include/etx_b200.h)
+int etxb_debug_closure_eval(etxb_ctx* ctx, const etxb_closure_query* queries, uint32_t count, uint32_t repetitions, double* out) {
+  if (!ctx || !queries || !out || (repetitions == 0)) return ETXB_ERR_INVALID_ARGUMENT;
+  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
+  if (count == 0) return ETXB_OK;
+  for (uint32_t i = 0; i < count; ++i) {
+    if (queries[i].material >= ctx->materials.count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "closure query material index out of range");
+  }
+  cudaSetDevice(ctx->device);
+  DevBuf<etxb_closure_query> d_queries;
+  DevBuf<double> d_out;
+  CUDA_OK(ctx, d_queries.alloc(count));
+  CUDA_OK(ctx, d_out.alloc(size_t(count) * ETXB_CLOSURE_STATS));
+  CUDA_OK(ctx, cudaMemcpy(d_queries.ptr, queries, d_queries.bytes(), cudaMemcpyHostToDevice));
+  if (ctx->spectral) {
+    k_debug_closure<true><<<blocks_for(count, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
+  } else {
+    k_debug_closure<false><<<blocks_for(count, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
+  }
+  ctx->kernel_launches += 1;
+  CUDA_OK(ctx, cudaGetLastError());
+  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+  CUDA_OK(ctx, cudaMemcpy(out, d_out.ptr, d_out.bytes(), cudaMemcpyDeviceToHost));
+  d_queries.release();
+  d_out.release();
+  return ETXB_OK;
+}
+
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Iterations in flight (etxb_group): L contexts on one device, one host thread each, pulling iteration indices from a shared

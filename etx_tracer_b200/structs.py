@@ -101,11 +101,19 @@ COUNTERS = np.dtype([(n, u8) for n in (
     "rays_closest", "rays_shadow", "nodes_visited", "tris_tested", "bounces_light", "bounces_camera", "light_vertices",
     "connections", "merge_queries", "merge_candidates", "merge_accepts", "splats", "kernel_launches", "nodes_closest", "tris_closest")])
 DEVICE_CONFIG = np.dtype([("device_index", np.int32), ("max_light_vertices", u4), ("flags", u4), ("pad", u4)])
+# etxb_closure_query (96 B) and the per-query statistics etxb_debug_closure_eval / oracle_bsdf_eval return (include/etx_b200.h)
+CLOSURE_QUERY = np.dtype([
+    ("nrm", f4, 3), ("tan", f4, 3), ("btn", f4, 3), ("w_i", f4, 3), ("w_o", f4, 3), ("uv", f4, 2), ("wavelength", f4),
+    ("material", u4), ("path_source", u4), ("seed", u4), ("reserved", u4, 3),
+])
+CLOSURE_STATS = 32
+CLOSURE_OUTPUTS = ("func_r", "func_g", "func_b", "bsdf_r", "bsdf_g", "bsdf_b", "pdf", "rev_pdf")
+PATH_CAMERA, PATH_LIGHT = 1, 2
 
 EXPECTED_SIZES = {
     "VERTEX": (VERTEX, 56), "TRIANGLE": (TRIANGLE, 32), "MATERIAL": (MATERIAL, 200), "EMITTER_PROFILE": (EMITTER_PROFILE, 48),
     "EMITTER": (EMITTER, 32), "SPECTRUM": (SPECTRUM, 3552), "DISTRIBUTION": (DISTRIBUTION, 32), "IMAGE": (IMAGE, 112),
-    "MEDIUM": (MEDIUM, 80), "CAMERA": (CAMERA, 176), "SCENE": (SCENE, 528),
+    "MEDIUM": (MEDIUM, 80), "CAMERA": (CAMERA, 176), "SCENE": (SCENE, 528), "CLOSURE_QUERY": (CLOSURE_QUERY, 96),
 }
 for _name, (_dt, _size) in EXPECTED_SIZES.items():
     assert _dt.itemsize == _size, f"{_name}: {_dt.itemsize} != {_size}"

@@ -463,6 +463,24 @@ int etxb_debug_select_tree(etxb_ctx* ctx, int wide);
 /* Sampler / spectral KATs evaluated on the device (sampler.hxx:54,66; spectrum.hxx:219,234). */
 int etxb_debug_sampler(etxb_ctx* ctx, const uint32_t* a, const uint32_t* b, uint32_t count, uint32_t draws, uint32_t* out_seed, float* out_values);
 int etxb_debug_math(etxb_ctx* ctx, uint32_t fn, const float* x, const float* y, uint32_t count, float* out);
+/* Vertex-closure query (dclosure.cuh: make_closure + closure_evaluate, as the photon gather and the vertex connections run them) on the
+ * uploaded scene.  One query is 96 bytes: the shading frame as interpolated, w_i pointing AT the surface (BSDFData::w_i), w_o pointing away,
+ * uv, the wavelength (ignored in RGB scenes, which use the undefined wavelength -1), the material index, the path source (1 = camera,
+ * 2 = light) and a sampler seed. */
+typedef struct etxb_closure_query {
+  float nrm[3], tan[3], btn[3];
+  float w_i[3], w_o[3];
+  float uv[2];
+  float wavelength;
+  uint32_t material, path_source, seed;
+  uint32_t reserved[3];
+} etxb_closure_query;
+/* Per query, `repetitions` evaluations; repetition r starts from the sampler Smp::init(seed, r) (= the reference's Sampler(seed, r)).
+ * out = double[ETXB_CLOSURE_STATS] per query: the outputs are ordered {func.rgb, bsdf.rgb, pdf, rev_pdf} (a spectral value fills all three
+ * components); [0..8) their means, [8..16) their variances (population, over the finite repetitions), [16..24) repetition 0's raw values,
+ * [24] the number of repetitions with a non-finite output, [25] with pdf < 0 or rev_pdf < 0, [26] with pdf == 0 but a non-zero func or bsdf. */
+#define ETXB_CLOSURE_STATS 32
+int etxb_debug_closure_eval(etxb_ctx* ctx, const etxb_closure_query* queries, uint32_t count, uint32_t repetitions, double* out);
 
 /* ---- several iterations in flight on one device -----------------------------------------------------------------------
  * The reference runs ONE iteration at a time and spreads its paths over the CPU's threads (vcm_cpu.cxx:115-171, TaskScheduler).

@@ -44,6 +44,8 @@ def load(flavor="parity"):
     lib.oracle_get_counters.argtypes = [vp, vp]
     lib.oracle_trace.argtypes = [vp, vp, vp, u32, vp, vp]
     lib.oracle_bvh_info.argtypes = [vp, C.POINTER(u32), C.POINTER(u32)]
+    if hasattr(lib, "oracle_bsdf_eval"):  # an oracle/_ref built before this export still serves every other test
+        lib.oracle_bsdf_eval.argtypes = [vp, vp, u32, u32, u32, vp]
     lib.oracle_sampler.argtypes = [vp, vp, u32, u32, vp, vp]
     lib.oracle_math.argtypes = [u32, vp, vp, u32, vp]
     lib.oracle_offset_ray.argtypes = [vp, vp, vp]
@@ -63,6 +65,11 @@ def load(flavor="parity"):
     lib.oracle_sizeof.argtypes = [u32]
     _libs[flavor] = lib
     return lib
+
+
+def has_bsdf_eval(flavor="parity"):
+    """Whether the built oracle exports oracle_bsdf_eval (oracle/_ref is older than the export where the reference could not rebuild it)."""
+    return hasattr(load(flavor), "oracle_bsdf_eval")
 
 
 def _p(a):
@@ -228,6 +235,14 @@ class Oracle:
         tri = np.zeros(n, dtype=np.uint32)
         self.lib.oracle_trace(self.h, _p(rays), _p(seeds), n, _p(uvt), _p(tri))
         return uvt, tri, seeds
+
+    def bsdf_eval(self, queries, repetitions, threads=None):
+        """The reference's bsdf::evaluate + bsdf::reverse_pdf for S.CLOSURE_QUERY records, `repetitions` samplers Sampler(seed, r) per query;
+        float64 (n, S.CLOSURE_STATS) in the layout of GPUVCM.debug_closure."""
+        queries = np.ascontiguousarray(queries, dtype=self.S.CLOSURE_QUERY)
+        out = np.zeros((queries.shape[0], self.S.CLOSURE_STATS), dtype=np.float64)
+        self.lib.oracle_bsdf_eval(self.h, _p(queries), queries.shape[0], int(repetitions), int(threads or os.cpu_count() or 1), _p(out))
+        return out
 
     def bvh_info(self):
         a, b = C.c_uint32(0), C.c_uint32(0)

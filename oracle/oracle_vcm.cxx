@@ -1048,6 +1048,68 @@ void oracle_bvh_info(void* h, uint32_t* node_count, uint32_t* slot_count) {
   *slot_count = uint32_t(o->bvh.tri_index.size());
 }
 
+// The reference's own BSDF evaluation for etxb_closure_query records (include/etx_b200.h), as the VCM consumers call it
+// (vcm_shared.hxx:708-713,738-748,852-857): bsdf::evaluate, then bsdf::reverse_pdf on the same sampler where the evaluation is valid.
+// Repetition r runs on Sampler(seed, r); the statistics are those etxb_debug_closure_eval returns.  Queries are spread over `threads`.
+static_assert(sizeof(etxb_closure_query) == 96);
+void oracle_bsdf_eval(void* h, const etxb_closure_query* queries, uint32_t count, uint32_t repetitions, uint32_t threads, double* out) {
+  auto* o = static_cast<Oracle*>(h);
+  const Scene& scene = o->scene;
+  parallel_ranges(count, threads, [&](uint32_t begin, uint32_t end, uint32_t, uint32_t) {
+    for (uint32_t i = begin; i < end; ++i) {
+      const etxb_closure_query& q = queries[i];
+      Vertex v = {};
+      v.nrm = {q.nrm[0], q.nrm[1], q.nrm[2]};
+      v.tan = {q.tan[0], q.tan[1], q.tan[2]};
+      v.btn = {q.btn[0], q.btn[1], q.btn[2]};
+      v.tex = {q.uv[0], q.uv[1]};
+      const float3 w_i = {q.w_i[0], q.w_i[1], q.w_i[2]}, w_o = {q.w_o[0], q.w_o[1], q.w_o[2]};
+      const SpectralQuery spect = scene.spectral() ? SpectralQuery{q.wavelength, SpectralQuery::Spectral} : SpectralQuery::sample();
+      const BSDFData data(spect, kInvalidIndex, static_cast<PathSource>(q.path_source), v, w_i);
+      const Material& mat = scene.materials[q.material];
+      double mean[8] = {}, m2[8] = {};
+      double* dst = out + size_t(i) * ETXB_CLOSURE_STATS;
+      uint32_t finite = 0, nonfinite = 0, negative = 0, unsupported = 0;
+      for (uint32_t r = 0; r < repetitions; ++r) {
+        Sampler smp(q.seed, r);
+        BSDFEval e = bsdf::evaluate(data, w_o, mat, scene, smp);
+        float rev = e.valid() ? bsdf::reverse_pdf(data, w_o, mat, scene, smp) : 0.0f;
+        const float3 f = e.func.spectral() ? float3{e.func.value, e.func.value, e.func.value} : e.func.integrated;
+        const float3 b = e.bsdf.spectral() ? float3{e.bsdf.value, e.bsdf.value, e.bsdf.value} : e.bsdf.integrated;
+        const float val[8] = {f.x, f.y, f.z, b.x, b.y, b.z, e.pdf, rev};
+        if (r == 0) {
+          for (uint32_t k = 0; k < 8; ++k)
+            dst[16 + k] = val[k];
+        }
+        bool ok = true;
+        for (uint32_t k = 0; k < 8; ++k)
+          ok = ok && std::isfinite(val[k]);
+        negative += ((e.pdf < 0.0f) || (rev < 0.0f)) ? 1u : 0u;
+        unsupported += ((e.pdf == 0.0f) && ((f.x != 0.0f) || (f.y != 0.0f) || (f.z != 0.0f) || (b.x != 0.0f) || (b.y != 0.0f) || (b.z != 0.0f))) ? 1u : 0u;
+        if (!ok) {
+          nonfinite += 1u;
+          continue;
+        }
+        finite += 1u;
+        for (uint32_t k = 0; k < 8; ++k) {
+          const double delta = double(val[k]) - mean[k];
+          mean[k] += delta / double(finite);
+          m2[k] += delta * (double(val[k]) - mean[k]);
+        }
+      }
+      for (uint32_t k = 0; k < 8; ++k) {
+        dst[k] = mean[k];
+        dst[8 + k] = (finite > 0) ? m2[k] / double(finite) : 0.0;
+      }
+      dst[24] = double(nonfinite);
+      dst[25] = double(negative);
+      dst[26] = double(unsupported);
+      for (uint32_t k = 27; k < ETXB_CLOSURE_STATS; ++k)
+        dst[k] = 0.0;
+    }
+  });
+}
+
 // ---- known-answer helpers straight from the reference headers ----------------------------------------
 void oracle_sampler(const uint32_t* a, const uint32_t* b, uint32_t count, uint32_t draws, uint32_t* out_seed, float* out_values) {
   for (uint32_t i = 0; i < count; ++i) {

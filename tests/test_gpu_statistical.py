@@ -40,6 +40,11 @@ CONFIGS = {
     "C3": (lambda: scenes.procedural_room(64, 36, env_size=(256, 128)), False),  # the 1M-triangle room, stochastic BSDFs
     "C4": (lambda: scenes.sss_dragon(40, 40), False),
     "C5": (lambda: scenes.cloud_box(40, 40, grid=64), True),
+    # the vertex-closure classes inside the kernels that use them (the connection record, the gather's shared-memory closures, the
+    # per-pair streams); no BASELINE scene has a dielectric
+    "dielectric_rough/spectral": (lambda: scenes.material_box("dielectric_rough", 40, 40, spectral=True), False),
+    "plastic_thinfilm/rgb": (lambda: scenes.material_box("plastic_thinfilm", 40, 40, spectral=False), False),
+    "conductor_thinfilm/rgb": (lambda: scenes.material_box("conductor_thinfilm", 40, 40, spectral=False), False),
 }
 
 
