@@ -37,6 +37,8 @@ def load_library(flavor="fast"):
     lib.etxb_destroy.argtypes = [vp]
     lib.etxb_destroy.restype = None
     lib.etxb_upload_scene.argtypes = [vp, vp, u64, vp, u64]
+    lib.etxb_update_scene.argtypes = [vp, vp, u64, vp, u64, vp]
+    lib.etxb_group_update_scene.argtypes = [vp, vp, u64, vp, u64, vp]
     lib.etxb_upload_blue_noise.argtypes = [vp, vp, vp, vp]
     lib.etxb_upload_color_tables.argtypes = [vp, vp, vp]
     lib.etxb_scene_file_load.argtypes = [C.c_char_p, C.c_char_p, C.POINTER(vp), C.c_char_p, u64]
@@ -227,6 +229,14 @@ def load_scene_file(file_name, flavor="fast"):
 COMM_ID_BYTES = 128
 
 
+def _bn_variant(samples):
+    """BNSampler variant = next_power(min(samples, 256)) (thirdparty/bluenoise/bluenoise.cxx:73-95)"""
+    spp = 1
+    while spp < min(max(samples, 1), 256):
+        spp *= 2
+    return spp
+
+
 def comm_unique_ids(count, flavor="fast"):
     """`count` NCCL unique ids (ETXB_COMM_ID_BYTES each) from the module, for rank 0 to hand to the other ranks by any transport."""
     lib = load_library(flavor)
@@ -290,21 +300,41 @@ class GPUVCM:
     def name():
         return "VCM (B200)"
 
-    def set_scene(self, scene_data):
-        """Raytracing::link_scene/link_camera + commit_changes."""
-        self.scene_data = scene_data
-        samples = int(scene_data.scene["samples"][0])
-        # BNSampler variant = next_power(min(samples, 256)) (thirdparty/bluenoise/bluenoise.cxx:73-95)
-        spp = 1
-        while spp < min(max(samples, 1), 256):
-            spp *= 2
+    def _upload_blue_noise(self, samples):
+        spp = _bn_variant(samples)
         bn = _scenes.tables("bluenoise")
         self._bn = [np.ascontiguousarray(bn[k], dtype=np.uint8) for k in ("sobol", f"scrambling_{spp}", f"ranking_{spp}")]
         self._check(self.lib.etxb_upload_blue_noise(self.h, _p(self._bn[0]), _p(self._bn[1]), _p(self._bn[2])))
-        self._check(self.lib.etxb_upload_scene(self.h, _p(scene_data.scene), scene_data.scene.nbytes, _p(scene_data.camera), scene_data.camera.nbytes))
+        self._bn_spp = spp
+
+    def _read_film_size(self):
         w, h = C.c_uint32(0), C.c_uint32(0)
         self._check(self.lib.etxb_film_size(self.h, C.byref(w), C.byref(h)))
         self.width, self.height = w.value, h.value
+
+    def set_scene(self, scene_data):
+        """Raytracing::link_scene/link_camera + commit_changes."""
+        self.scene_data = scene_data
+        self._upload_blue_noise(int(scene_data.scene["samples"][0]))
+        self._check(self.lib.etxb_upload_scene(self.h, _p(scene_data.scene), scene_data.scene.nbytes, _p(scene_data.camera), scene_data.camera.nbytes))
+        self._read_film_size()
+
+    def update_scene(self, scene_data):
+        """The restart after an edit of the scene or camera (etxb_update_scene): renders what set_scene(scene_data) would, keeping on the device
+        what the edit did not change.  The film is cleared and armed at iteration 0; a render that was running goes on with the new scene.
+        Returns the etxb_update_info fields as a dict."""
+        info = np.zeros(1, dtype=S.UPDATE_INFO)
+        self._check(self.lib.etxb_update_scene(self.h, _p(scene_data.scene), scene_data.scene.nbytes, _p(scene_data.camera), scene_data.camera.nbytes, _p(info)))
+        self._after_update(scene_data)
+        return {k: info[k][0].item() for k in info.dtype.names}
+
+    def _after_update(self, scene_data):
+        self.scene_data = scene_data
+        samples = int(scene_data.scene["samples"][0])
+        if _bn_variant(samples) != getattr(self, "_bn_spp", None):
+            self._upload_blue_noise(samples)
+        self._read_film_size()
+        self._target_iterations = samples
 
     def set_option(self, key, value):
         """Integrator::options() keys: vcm-initial_radius, vcm-radius_decay, vcm-blue_noise, vcm-kernel, vcm-direct_hit, ..."""
@@ -587,6 +617,18 @@ class GPUVCMGroup:
     def run(self, first_iteration=0):
         self.set_options()
         self._check(self.lib.etxb_group_begin(self.h, first_iteration))
+
+    def update_scene(self, scene_data):
+        """GPUVCM.update_scene for every lane (etxb_group_update_scene): hashed once, then the group is idle and armed at iteration 0.  Returns
+        lane 0's etxb_update_info fields, `kept` being what every lane kept."""
+        info = np.zeros(1, dtype=S.UPDATE_INFO)
+        self._check(self.lib.etxb_group_update_scene(self.h, _p(scene_data.scene), scene_data.scene.nbytes, _p(scene_data.camera), scene_data.camera.nbytes,
+                                                     _p(info)))
+        for g in self.lanes:
+            g._after_update(scene_data)
+        self.scene_data = scene_data
+        self.width, self.height = self.lanes[0].width, self.lanes[0].height
+        return {k: info[k][0].item() for k in info.dtype.names}
 
     def comm_init(self, world, rank, comm_ids):
         """Pixel tiles over `world` processes with len(self.lanes) iterations in flight on each: collective; comm_ids = the (lanes + 1) x 128

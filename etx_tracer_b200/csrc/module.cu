@@ -79,6 +79,12 @@ struct DevBuf {
     if (n == 0) return cudaSuccess;
     return cudaMalloc(&ptr, n * sizeof(T));
   }
+  // alloc that keeps the allocation when it already holds n elements; counts the allocations it makes
+  cudaError_t ensure(size_t n, uint32_t& allocations) {
+    if (ptr && (count == n)) return cudaSuccess;
+    allocations += 1;
+    return alloc(n);
+  }
   void release() {
     if (ptr) cudaFree(ptr);
     ptr = nullptr;
@@ -90,6 +96,47 @@ struct DevBuf {
 struct TimedLaunch {
   uint32_t kernel;
   cudaEvent_t start, stop;
+};
+
+// 128-bit content hash of a byte range, chained through `seed`: four independent 64-bit multiply-rotate lanes over 32-byte stripes (the
+// round of xxHash64), a zero-padded tail, and two differently mixed 64-bit digests of the lanes and the length.  It detects edits, not
+// adversaries.
+struct Hash128 {
+  uint64_t lo = 0, hi = 0;
+  bool operator==(const Hash128& o) const { return (lo == o.lo) && (hi == o.hi); }
+};
+constexpr uint64_t kHashP1 = 0x9E3779B185EBCA87ull, kHashP2 = 0xC2B2AE3D27D4EB4Full, kHashP3 = 0x165667B19E3779F9ull, kHashP4 = 0x85EBCA77C2B2AE63ull;
+inline uint64_t rotl64(uint64_t x, int r) { return (x << r) | (x >> (64 - r)); }
+inline uint64_t hash_round(uint64_t acc, uint64_t w) { return rotl64(acc + w * kHashP2, 31) * kHashP1; }
+inline uint64_t hash_mix(uint64_t h) {
+  h ^= h >> 33;
+  h *= kHashP2;
+  h ^= h >> 29;
+  h *= kHashP3;
+  return h ^ (h >> 32);
+}
+Hash128 hash128(const void* data, size_t bytes, Hash128 seed) {
+  const uint8_t* p = static_cast<const uint8_t*>(data);
+  uint64_t v[4] = {seed.lo + kHashP1 + kHashP2, seed.hi + kHashP2, seed.lo ^ kHashP3, seed.hi - kHashP1};
+  size_t i = 0;
+  for (; i + 32 <= bytes; i += 32) {
+    uint64_t w[4];
+    memcpy(w, p + i, 32);
+    for (int k = 0; k < 4; ++k) v[k] = hash_round(v[k], w[k]);
+  }
+  uint64_t tail[4] = {0, 0, 0, 0};
+  if (bytes > i) memcpy(tail, p + i, bytes - i);
+  for (int k = 0; k < 4; ++k) v[k] = hash_round(v[k], tail[k]);
+  const uint64_t a = rotl64(v[0], 1) + rotl64(v[1], 7) + rotl64(v[2], 12) + rotl64(v[3], 18);
+  const uint64_t b = (v[0] * kHashP4) ^ rotl64(v[1], 29) ^ (v[2] * kHashP3) ^ rotl64(v[3], 43);
+  return {hash_mix(a ^ (uint64_t(bytes) * kHashP4)), hash_mix(b + uint64_t(bytes) * kHashP1)};
+}
+
+// what the last upload / update of a context copied, by content (etxb_update_scene keeps what did not change)
+struct SceneHashes {
+  bool valid = false;  // set once the whole scene is on the device
+  Hash128 geometry;    // vertex array + triangle array: device vertices, triangles, BVH2 (+ the 4-wide tree)
+  std::vector<Hash128> images, grids;  // per image; per medium (zero for media without a density grid)
 };
 
 }  // namespace
@@ -121,6 +168,7 @@ struct etxb_ctx {
   DevBuf<etxb_distribution_entry> emitter_dist;
   DevBuf<BvhNode> bvh_nodes;
   DevBuf<WideNode> wide_nodes;
+  bool wide_rejected = false;         // the committed geometry's 4-wide tree exceeds kWideStackSize (the scene walks the BVH2)
   bool debug_trace_wide = false;      // etxb_debug_select_tree: etxb_debug_trace walks the 4-wide tree when the scene has one
   DevBuf<float4> bvh_tris;
   DevBuf<float> xyz_table, rgb_response_table;
@@ -128,6 +176,7 @@ struct etxb_ctx {
   float y_integral = 0.0f;
   DeviceScene dscene = {};
   double bvh_build_seconds = 0.0;
+  SceneHashes hashes;
 
   // per-path state + queues
   uint32_t width = 0, height = 0, path_count = 0;
@@ -1094,19 +1143,48 @@ int etxb_upload_blue_noise(etxb_ctx* ctx, const uint8_t* sobol_256x256, const ui
   return ETXB_OK;
 }
 
-int etxb_upload_scene(etxb_ctx* ctx, const void* scene_blob, uint64_t scene_bytes, const void* camera_blob, uint64_t camera_bytes) {
-  if (!ctx || !scene_blob || !camera_blob) return ETXB_ERR_INVALID_ARGUMENT;
+// ---- scene upload / update ------------------------------------------------------------------------------------------------------------------
+// etxb_upload_scene and etxb_update_scene run the same stages: validate_scene makes every check and touches nothing on the device,
+// prepare_scene hashes the bulk arrays (prepare_bvh builds the host BVH when the geometry is new), commit_scene copies to the device.  An
+// update keeps the device copies whose content hashes did not change; everything small is derived from the PODs again on every call.
+extern "C++" {
+namespace {
+
+struct SceneClass {
+  bool stochastic = false;  // has_stochastic_merge
+  bool boundaries = false, subsurface = false, deferred = false, opaque = false, plain = false;
+};
+
+struct ScenePrep {
+  SceneClass cls;
+  SceneHashes hashes;
+  double fingerprint_seconds = 0.0, bvh_seconds = 0.0;
+  uint64_t bytes_hashed = 0;
+  Bvh bvh;                  // built by prepare_bvh (have_bvh), or only its nodes downloaded for a new 4-wide tree
+  bool have_bvh = false;
+  WideBvh wide;
+  bool have_wide = false;
+};
+
+double seconds_since(std::chrono::steady_clock::time_point t0) { return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(); }
+
+bool image_has_table(const etxb_image& im) {
+  return (im.y_distribution.values.a != nullptr) && distribution_covers(im.y_distribution.values.count, im.isize[1]) && (im.x_distributions.count == im.isize[1]);
+}
+size_t image_pixel_bytes(const etxb_image& im) { return size_t(im.isize[0]) * im.isize[1] * (im.format == 1u ? 16 : 4); }
+
+int check_scene_args(etxb_ctx* ctx, uint64_t scene_bytes, uint64_t camera_bytes) {
   if (scene_bytes != sizeof(etxb_scene) || camera_bytes != sizeof(etxb_camera))
     return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "scene/camera size mismatch: got %llu/%llu, expected %zu/%zu", (unsigned long long)scene_bytes,
       (unsigned long long)camera_bytes, sizeof(etxb_scene), sizeof(etxb_camera));
   if (!ctx->xyz_table.ptr) return fail(ctx, ETXB_ERR_NOT_READY, "etxb_upload_color_tables must be called before etxb_upload_scene");
-  ctx_drain_impl(ctx);
-  cudaSetDevice(ctx->device);
-  ctx->scene_ready = false;
-  const etxb_scene& s = *static_cast<const etxb_scene*>(scene_blob);
-  const etxb_camera& cam = *static_cast<const etxb_camera*>(camera_blob);
+  return ETXB_OK;
+}
 
-  // ---- what the device path does not cover yet fails loudly (no CPU fallback) --------------------------------------
+// Every check of the upload but the BVH depth (prepare_bvh), and the scene-class flags.  What the device path does not cover yet fails
+// loudly (no CPU fallback); every index the host builder and the kernels follow is checked: a malformed scene is an error, not an
+// out-of-bounds read.
+int validate_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, SceneClass& c) {
   if (cam.cls > 1u) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "unknown camera class %u", cam.cls);
   if (cam.lens_image != ETXB_INVALID_INDEX) {
     if (cam.lens_image >= s.images.count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "camera lens image index out of range");
@@ -1130,14 +1208,14 @@ int etxb_upload_scene(etxb_ctx* ctx, const void* scene_blob, uint64_t scene_byte
     if (((m.int_medium != ETXB_INVALID_INDEX) && (m.int_medium >= s.mediums.count)) || ((m.ext_medium != ETXB_INVALID_INDEX) && (m.ext_medium >= s.mediums.count)))
       return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "material %llu: medium index out of range", (unsigned long long)i);
   }
-  ctx->has_stochastic_merge = false;
+  c = {};
   for (uint64_t i = 0; i < s.materials.count; ++i) {
     const etxb_material& m = mats[i];
     bool lambert = (m.cls == ETXB_MAT_DIFFUSE) && (m.diffuse_variation == 0);
     bool smooth = (std::max(m.roughness.value[0], m.roughness.value[1]) <= 1.0e-4f) && (m.roughness.image_index == ETXB_INVALID_INDEX);
     bool always_delta = (((m.cls == ETXB_MAT_DIELECTRIC) || (m.cls == ETXB_MAT_CONDUCTOR)) && smooth) || (m.cls == ETXB_MAT_THINFILM) || (m.cls == ETXB_MAT_MIRROR) ||
                         (m.cls == ETXB_MAT_VOID);
-    if (!lambert && !always_delta) ctx->has_stochastic_merge = true;
+    if (!lambert && !always_delta) c.stochastic = true;
   }
   const auto* emitters = static_cast<const etxb_emitter*>(s.emitter_instances.a);
   for (uint64_t i = 0; i < s.emitter_instances.count; ++i) {
@@ -1149,185 +1227,287 @@ int etxb_upload_scene(etxb_ctx* ctx, const void* scene_blob, uint64_t scene_byte
       if (!distribution_covers(img.y_distribution.values.count, img.isize[1])) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "environment emitter %llu: image has no sampling table", (unsigned long long)i);
     }
   }
-  // ---- media (medium.hxx:8-47): dense density grids go to HBM as they are -------------------------------------------------------
+  // media (medium.hxx:8-47)
+  const auto* meds = static_cast<const etxb_medium*>(s.mediums.a);
+  for (uint64_t i = 0; i < s.mediums.count; ++i) {
+    const etxb_medium& md = meds[i];
+    if (md.cls == 1u) {
+      size_t n = size_t(md.dimensions[0]) * md.dimensions[1] * md.dimensions[2];
+      if ((n == 0) || (md.density.count != n)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium %llu: density grid does not match its dimensions", (unsigned long long)i);
+    } else if (md.cls != 0u) {
+      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium %llu: unknown class %u", (unsigned long long)i, md.cls);
+    }
+  }
+  for (uint64_t i = 0; i < s.materials.count; ++i) {
+    if (mats[i].cls == ETXB_MAT_BOUNDARY) c.boundaries = true;
+    if (mats[i].subsurface.cls != 0) c.subsurface = true;
+  }
+  if ((cam.medium_index != ETXB_INVALID_INDEX) && (cam.medium_index >= s.mediums.count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "camera medium index out of range");
+  // deferred shadow rays (ShadowBatch, dvcm.cuh) need: no alpha test that can reject, no Boundary surfaces / media (transmittance is 0 or 1),
+  // no BSDF whose evaluation draws from the sampler, no subsurface exits
+  c.plain = !c.boundaries && !c.subsurface && (s.mediums.count == 0) && (cam.medium_index == ETXB_INVALID_INDEX);
+  bool no_alpha = true;
+  const auto* all_images = static_cast<const etxb_image*>(s.images.a);
+  for (uint64_t i = 0; no_alpha && (i < s.materials.count); ++i) {
+    if (mats[i].opacity != 1.0f) no_alpha = false;
+    uint32_t im = mats[i].scattering.image_index;
+    if ((im != ETXB_INVALID_INDEX) && (all_images[im].options & kImageHasAlpha)) no_alpha = false;
+  }
+  c.opaque = c.plain && no_alpha;
+  c.deferred = c.opaque && !c.stochastic;
+  // images: pixels + flattened row/column CDFs (image.hxx:8-50)
+  for (uint64_t i = 0; i < s.images.count; ++i) {
+    const etxb_image& im = all_images[i];
+    if ((im.format != 1u) && (im.format != 2u)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "image %llu: unknown pixel format %u", (unsigned long long)i, im.format);
+    if (size_t(im.isize[0]) * im.isize[1] == 0) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "image %llu is empty", (unsigned long long)i);
+    if (image_has_table(im)) {
+      const auto* rows = static_cast<const etxb_distribution*>(im.x_distributions.a);
+      for (uint32_t y = 0; y < im.isize[1]; ++y)
+        if (!distribution_covers(rows[y].values.count, im.isize[0])) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "image %llu: row %u distribution has %llu entries", (unsigned long long)i, y, (unsigned long long)rows[y].values.count);
+    }
+  }
+  if (s.emitter_instances.count == 0) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "scene has no emitters");
+  const auto* spectra = static_cast<const etxb_spectrum*>(s.spectrums.a);
+  for (uint64_t i = 0; i < s.spectrums.count; ++i) {
+    const etxb_spectrum& sp = spectra[i];
+    if (sp.entry_count != 441) return fail(ctx, ETXB_ERR_UNSUPPORTED, "spectrum %llu has %u entries; the loader's 441-entry 390..830 nm grid is required", (unsigned long long)i, sp.entry_count);
+    for (uint32_t k = 0; k < 441; ++k)
+      if (sp.entries[k].wavelength != float(390 + k)) return fail(ctx, ETXB_ERR_UNSUPPORTED, "spectrum %llu is not on the integer 390..830 nm grid", (unsigned long long)i);
+  }
+  // geometry
+  const auto* tris = static_cast<const etxb_triangle*>(s.triangles.a);
+  for (uint64_t i = 0; i < s.triangles.count; ++i) {
+    const etxb_triangle& t = tris[i];
+    if ((t.i[0] >= s.vertices.count) || (t.i[1] >= s.vertices.count) || (t.i[2] >= s.vertices.count))
+      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "triangle %llu: vertex index out of range", (unsigned long long)i);
+    if (t.material_index >= s.materials.count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "triangle %llu: material index %u out of range", (unsigned long long)i, t.material_index);
+  }
+  if (s.triangle_to_emitter.count != s.triangles.count)
+    return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "triangle_to_emitter has %llu entries for %llu triangles", (unsigned long long)s.triangle_to_emitter.count, (unsigned long long)s.triangles.count);
+  const auto* t2e = static_cast<const uint32_t*>(s.triangle_to_emitter.a);
+  for (uint64_t i = 0; i < s.triangle_to_emitter.count; ++i)
+    if ((t2e[i] != ETXB_INVALID_INDEX) && (t2e[i] >= s.emitter_instances.count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "triangle %llu: emitter index out of range", (unsigned long long)i);
+  for (uint64_t i = 0; i < s.emitter_instances.count; ++i) {
+    if (emitters[i].profile >= s.emitter_profiles.count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "emitter %llu: profile index out of range", (unsigned long long)i);
+    if ((emitters[i].cls == 0u) && (emitters[i].triangle_index >= s.triangles.count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "area emitter %llu: triangle index out of range", (unsigned long long)i);
+  }
+  if (!distribution_covers(s.emitters_distribution.values.count, s.emitter_instances.count))
+    return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "emitter distribution has %llu entries for %llu emitters", (unsigned long long)s.emitters_distribution.values.count, (unsigned long long)s.emitter_instances.count);
+  if ((s.pixel_sampler_image != 0xffffffffu) && (s.pixel_sampler_image >= s.images.count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "pixel sampler image out of range");
+  if (size_t(cam.film_size[0]) * cam.film_size[1] == 0) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "empty film");
+  return ETXB_OK;
+}
+
+// validate_scene + the content hashes of the arrays commit_scene may keep on the device: the vertices and triangles (one geometry
+// hash), each image (pixels, sampling tables, scalar fields) and each density grid (values and dimensions)
+int prepare_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, ScenePrep& p) {
+  if (int rc = validate_scene(ctx, s, cam, p.cls)) return rc;
+  auto t0 = std::chrono::steady_clock::now();
+  SceneHashes& h = p.hashes;
+  auto hash = [&p](const void* data, size_t bytes, Hash128 seed) {
+    p.bytes_hashed += bytes;
+    return hash128(data, bytes, seed);
+  };
+  h.geometry = hash(s.vertices.a, s.vertices.count * sizeof(etxb_vertex), {});
+  h.geometry = hash(s.triangles.a, s.triangles.count * sizeof(etxb_triangle), h.geometry);
+  h.images.assign(s.images.count, {});
+  const auto* imgs = static_cast<const etxb_image*>(s.images.a);
+  for (uint64_t i = 0; i < s.images.count; ++i) {
+    const etxb_image& im = imgs[i];
+    const bool table = image_has_table(im);
+    const float fields[] = {im.fsize[0], im.fsize[1], im.offset[0], im.offset[1], im.scale[0], im.scale[1], im.normalization};
+    const uint32_t ifields[] = {im.isize[0], im.isize[1], im.options, im.format, table ? 1u : 0u};
+    Hash128 x = hash(fields, sizeof(fields), {});
+    x = hash(ifields, sizeof(ifields), x);
+    x = hash(im.pixels.a, image_pixel_bytes(im), x);
+    if (table) {
+      x = hash(im.y_distribution.values.a, (size_t(im.isize[1]) + 1u) * sizeof(etxb_distribution_entry), x);
+      const auto* rows = static_cast<const etxb_distribution*>(im.x_distributions.a);
+      for (uint32_t y = 0; y < im.isize[1]; ++y) x = hash(rows[y].values.a, (size_t(im.isize[0]) + 1u) * sizeof(etxb_distribution_entry), x);
+    }
+    h.images[i] = x;
+  }
+  h.grids.assign(s.mediums.count, {});
+  const auto* meds = static_cast<const etxb_medium*>(s.mediums.a);
+  for (uint64_t i = 0; i < s.mediums.count; ++i) {
+    if (meds[i].cls != 1u) continue;
+    h.grids[i] = hash(meds[i].dimensions, sizeof(meds[i].dimensions), {});
+    h.grids[i] = hash(meds[i].density.a, meds[i].density.count * sizeof(float), h.grids[i]);
+  }
+  h.valid = true;
+  p.fingerprint_seconds = seconds_since(t0);
+  return ETXB_OK;
+}
+
+// the host BVH of a new geometry, and the check of its depth against the traversal stack
+int prepare_bvh(etxb_ctx* ctx, const etxb_scene& s, ScenePrep& p) {
+  if (p.have_bvh) return ETXB_OK;
+  auto t0 = std::chrono::steady_clock::now();
+  auto c0 = std::clock();
+  build_bvh(reinterpret_cast<const float*>(s.vertices.a), sizeof(etxb_vertex), reinterpret_cast<const uint32_t*>(s.triangles.a), sizeof(etxb_triangle),
+    uint32_t(s.triangles.count), p.bvh);
+  ctx->bvh_build_seconds = double(std::clock() - c0) / CLOCKS_PER_SEC;
+  p.bvh_seconds += seconds_since(t0);
+  p.have_bvh = true;
+  if (p.bvh.max_depth >= uint32_t(kBvhStackSize)) return fail(ctx, ETXB_ERR_UNSUPPORTED, "BVH depth %u exceeds the traversal stack (%d)", p.bvh.max_depth, kBvhStackSize);
+  return ETXB_OK;
+}
+
+bool geometry_kept(const etxb_ctx* ctx, const ScenePrep& p, bool reuse) { return reuse && ctx->hashes.valid && (ctx->hashes.geometry == p.hashes.geometry); }
+
+// The device side of an upload (reuse = false: every buffer is allocated and copied again) or of an update (reuse = true: what the
+// hashes show unchanged stays, path-state buffers of the same size stay).  Runs after prepare_scene, so only CUDA errors remain: they
+// leave the scene not ready.  Ends with etxb_begin(ctx, 0).
+int commit_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, ScenePrep& p, bool reuse, etxb_update_info* info) {
+  const bool keep_geometry = geometry_kept(ctx, p, reuse);
+  if (!keep_geometry)
+    if (int rc = prepare_bvh(ctx, s, p)) return rc;
+  const SceneHashes old = std::move(ctx->hashes);
+  ctx->hashes = {};
+  ctx->scene_ready = false;
+  etxb_update_info st = {};
+  ctx->has_stochastic_merge = p.cls.stochastic;
+  ctx->plain_scene = p.cls.plain;
+  ctx->opaque_scene = p.cls.opaque;
+  DeviceScene& d = ctx->dscene;
+  const auto* mats = static_cast<const etxb_material*>(s.materials.a);
+
+  // ---- media: dense density grids go to HBM as they are ---------------------------------------------------------------------------------
   {
     const auto* meds = static_cast<const etxb_medium*>(s.mediums.a);
     std::vector<DMedium> dmeds(s.mediums.count);
-    for (auto& b : ctx->medium_density) b.release();
-    ctx->medium_density.assign(s.mediums.count, {});
+    for (size_t i = s.mediums.count; i < ctx->medium_density.size(); ++i) ctx->medium_density[i].release();
+    ctx->medium_density.resize(s.mediums.count);
     for (uint64_t i = 0; i < s.mediums.count; ++i) {
       const etxb_medium& md = meds[i];
-      DMedium& d = dmeds[i];
-      d = {};
-      d.bounds_min = {md.bounds_min[0], md.bounds_min[1], md.bounds_min[2]};
-      d.bounds_max = {md.bounds_max[0], md.bounds_max[1], md.bounds_max[2]};
-      d.cls = md.cls;
-      d.enable_explicit_connections = md.enable_explicit_connections;
-      d.absorption_index = md.absorption_index;
-      d.scattering_index = md.scattering_index;
-      d.phase_function_g = md.phase_function_g;
-      d.max_sigma = md.max_sigma;
-      d.dim_x = md.dimensions[0];
-      d.dim_y = md.dimensions[1];
-      d.dim_z = md.dimensions[2];
+      DMedium& dm = dmeds[i];
+      dm = {};
+      dm.bounds_min = {md.bounds_min[0], md.bounds_min[1], md.bounds_min[2]};
+      dm.bounds_max = {md.bounds_max[0], md.bounds_max[1], md.bounds_max[2]};
+      dm.cls = md.cls;
+      dm.enable_explicit_connections = md.enable_explicit_connections;
+      dm.absorption_index = md.absorption_index;
+      dm.scattering_index = md.scattering_index;
+      dm.phase_function_g = md.phase_function_g;
+      dm.max_sigma = md.max_sigma;
+      dm.dim_x = md.dimensions[0];
+      dm.dim_y = md.dimensions[1];
+      dm.dim_z = md.dimensions[2];
+      DevBuf<float>& grid = ctx->medium_density[i];
       if (md.cls == 1u) {
-        size_t n = size_t(d.dim_x) * d.dim_y * d.dim_z;
-        if ((n == 0) || (md.density.count != n)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium %llu: density grid does not match its dimensions", (unsigned long long)i);
-        CUDA_OK(ctx, ctx->medium_density[i].alloc(n));
-        CUDA_OK(ctx, cudaMemcpyAsync(ctx->medium_density[i].ptr, md.density.a, n * 4, cudaMemcpyHostToDevice, ctx->stream));
-        d.density = ctx->medium_density[i].ptr;
-      } else if (md.cls != 0u) {
-        return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium %llu: unknown class %u", (unsigned long long)i, md.cls);
+        size_t n = size_t(dm.dim_x) * dm.dim_y * dm.dim_z;
+        if (reuse && old.valid && (i < old.grids.size()) && (old.grids[i] == p.hashes.grids[i]) && (grid.count == n)) {
+          st.grids_kept += 1;
+        } else {
+          CUDA_OK(ctx, grid.alloc(n));
+          CUDA_OK(ctx, cudaMemcpyAsync(grid.ptr, md.density.a, n * 4, cudaMemcpyHostToDevice, ctx->stream));
+          st.grids_uploaded += 1;
+        }
+        dm.density = grid.ptr;
+      } else {
+        grid.release();
       }
     }
     if (int rc = upload(ctx, ctx->mediums, dmeds.data(), dmeds.size())) return rc;
-    ctx->dscene.mediums = ctx->mediums.ptr;
-    ctx->dscene.medium_count = uint32_t(dmeds.size());
-    ctx->dscene.has_boundaries = 0;
-    ctx->dscene.has_subsurface = 0;
-    ctx->dscene.subsurface_exit_material = s.subsurface_exit_material;
-    for (uint64_t i = 0; i < s.materials.count; ++i) {
-      if (mats[i].cls == ETXB_MAT_BOUNDARY) ctx->dscene.has_boundaries = 1;
-      if (mats[i].subsurface.cls != 0) ctx->dscene.has_subsurface = 1;
-    }
-    if ((cam.medium_index != ETXB_INVALID_INDEX) && (cam.medium_index >= s.mediums.count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "camera medium index out of range");
-    // deferred shadow rays (ShadowBatch, dvcm.cuh) need: no alpha test that can reject, no Boundary surfaces / media (transmittance is 0 or 1),
-    // no BSDF whose evaluation draws from the sampler, no subsurface exits
-    bool deferred = !ctx->has_stochastic_merge && !ctx->dscene.has_boundaries && !ctx->dscene.has_subsurface && (s.mediums.count == 0) && (cam.medium_index == ETXB_INVALID_INDEX);
-    const auto* all_images = static_cast<const etxb_image*>(s.images.a);
-    for (uint64_t i = 0; deferred && (i < s.materials.count); ++i) {
-      if (mats[i].opacity != 1.0f) deferred = false;
-      uint32_t im = mats[i].scattering.image_index;
-      if ((im != ETXB_INVALID_INDEX) && (all_images[im].options & kImageHasAlpha)) deferred = false;
-    }
-    ctx->dscene.deferred_shadow_rays = deferred ? 1u : 0u;
-    {
-      bool opaque = !ctx->dscene.has_boundaries && !ctx->dscene.has_subsurface && (s.mediums.count == 0) && (cam.medium_index == ETXB_INVALID_INDEX);
-      for (uint64_t i = 0; opaque && (i < s.materials.count); ++i) {
-        if (mats[i].opacity != 1.0f) opaque = false;
-        uint32_t im = mats[i].scattering.image_index;
-        if ((im != ETXB_INVALID_INDEX) && (all_images[im].options & kImageHasAlpha)) opaque = false;
-      }
-      ctx->opaque_scene = opaque;
-    }
-    ctx->plain_scene = !ctx->dscene.has_boundaries && !ctx->dscene.has_subsurface && (s.mediums.count == 0) && (cam.medium_index == ETXB_INVALID_INDEX);
+    d.mediums = ctx->mediums.ptr;
+    d.medium_count = uint32_t(dmeds.size());
+    d.has_boundaries = p.cls.boundaries ? 1 : 0;
+    d.has_subsurface = p.cls.subsurface ? 1 : 0;
+    d.subsurface_exit_material = s.subsurface_exit_material;
+    d.deferred_shadow_rays = p.cls.deferred ? 1u : 0u;
   }
   // ---- images: pixels + flattened row/column CDFs (image.hxx:8-50) ---------------------------------------------------------------
   {
     const auto* imgs = static_cast<const etxb_image*>(s.images.a);
     std::vector<DImage> dimgs(s.images.count);
-    for (auto& b : ctx->image_pixels) b.release();
-    for (auto& b : ctx->image_dists) b.release();
-    ctx->image_pixels.assign(s.images.count, {});
-    ctx->image_dists.assign(s.images.count * 2, {});
+    for (size_t i = s.images.count; i < ctx->image_pixels.size(); ++i) {
+      ctx->image_pixels[i].release();
+      ctx->image_dists[i * 2].release();
+      ctx->image_dists[i * 2 + 1].release();
+    }
+    ctx->image_pixels.resize(s.images.count);
+    ctx->image_dists.resize(s.images.count * 2);
     for (uint64_t i = 0; i < s.images.count; ++i) {
       const etxb_image& im = imgs[i];
-      DImage& d = dimgs[i];
-      d = {};
-      if ((im.format != 1u) && (im.format != 2u)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "image %llu: unknown pixel format %u", (unsigned long long)i, im.format);
-      size_t px = size_t(im.isize[0]) * im.isize[1];
-      if (px == 0) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "image %llu is empty", (unsigned long long)i);
-      size_t bytes = px * (im.format == 1u ? 16 : 4);
-      CUDA_OK(ctx, ctx->image_pixels[i].alloc(bytes));
-      CUDA_OK(ctx, cudaMemcpyAsync(ctx->image_pixels[i].ptr, im.pixels.a, bytes, cudaMemcpyHostToDevice, ctx->stream));
-      d.pixels_f32 = (im.format == 1u) ? reinterpret_cast<const float4*>(ctx->image_pixels[i].ptr) : nullptr;
-      d.pixels_u8 = (im.format == 2u) ? reinterpret_cast<const uchar4*>(ctx->image_pixels[i].ptr) : nullptr;
-      d.fsize_x = im.fsize[0]; d.fsize_y = im.fsize[1];
-      d.offset_x = im.offset[0]; d.offset_y = im.offset[1];
-      d.scale_x = im.scale[0]; d.scale_y = im.scale[1];
-      d.isize_x = im.isize[0]; d.isize_y = im.isize[1];
-      d.normalization = im.normalization;
-      d.options = im.options;
-      d.format = im.format;
-      if ((im.y_distribution.values.a != nullptr) && distribution_covers(im.y_distribution.values.count, im.isize[1]) && (im.x_distributions.count == im.isize[1])) {
-        size_t nx = size_t(im.isize[0]) + 1u, ny = size_t(im.isize[1]) + 1u;
-        std::vector<etxb_distribution_entry> flat(nx * im.isize[1]);
-        const auto* rows = static_cast<const etxb_distribution*>(im.x_distributions.a);
-        for (uint32_t y = 0; y < im.isize[1]; ++y) {
-          if (!distribution_covers(rows[y].values.count, im.isize[0])) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "image %llu: row %u distribution has %llu entries", (unsigned long long)i, y, (unsigned long long)rows[y].values.count);
-          memcpy(flat.data() + size_t(y) * nx, rows[y].values.a, nx * sizeof(etxb_distribution_entry));
+      DImage& di = dimgs[i];
+      di = {};
+      const size_t bytes = image_pixel_bytes(im);
+      const bool table = image_has_table(im);
+      DevBuf<uint8_t>& pixels = ctx->image_pixels[i];
+      DevBuf<uint8_t>& x_dist = ctx->image_dists[i * 2];
+      DevBuf<uint8_t>& y_dist = ctx->image_dists[i * 2 + 1];
+      if (reuse && old.valid && (i < old.images.size()) && (old.images[i] == p.hashes.images[i]) && (pixels.count == bytes)) {
+        st.images_kept += 1;
+      } else {
+        CUDA_OK(ctx, pixels.alloc(bytes));
+        CUDA_OK(ctx, cudaMemcpyAsync(pixels.ptr, im.pixels.a, bytes, cudaMemcpyHostToDevice, ctx->stream));
+        x_dist.release();
+        y_dist.release();
+        if (table) {
+          size_t nx = size_t(im.isize[0]) + 1u, ny = size_t(im.isize[1]) + 1u;
+          std::vector<etxb_distribution_entry> flat(nx * im.isize[1]);
+          const auto* rows = static_cast<const etxb_distribution*>(im.x_distributions.a);
+          for (uint32_t y = 0; y < im.isize[1]; ++y) memcpy(flat.data() + size_t(y) * nx, rows[y].values.a, nx * sizeof(etxb_distribution_entry));
+          CUDA_OK(ctx, x_dist.alloc(flat.size() * sizeof(etxb_distribution_entry)));
+          CUDA_OK(ctx, cudaMemcpy(x_dist.ptr, flat.data(), flat.size() * sizeof(etxb_distribution_entry), cudaMemcpyHostToDevice));
+          CUDA_OK(ctx, y_dist.alloc(ny * sizeof(etxb_distribution_entry)));
+          CUDA_OK(ctx, cudaMemcpy(y_dist.ptr, im.y_distribution.values.a, ny * sizeof(etxb_distribution_entry), cudaMemcpyHostToDevice));
         }
-        CUDA_OK(ctx, ctx->image_dists[i * 2].alloc(flat.size() * sizeof(etxb_distribution_entry)));
-        CUDA_OK(ctx, cudaMemcpy(ctx->image_dists[i * 2].ptr, flat.data(), flat.size() * sizeof(etxb_distribution_entry), cudaMemcpyHostToDevice));
-        CUDA_OK(ctx, ctx->image_dists[i * 2 + 1].alloc(ny * sizeof(etxb_distribution_entry)));
-        CUDA_OK(ctx, cudaMemcpy(ctx->image_dists[i * 2 + 1].ptr, im.y_distribution.values.a, ny * sizeof(etxb_distribution_entry), cudaMemcpyHostToDevice));
-        d.x_dist = reinterpret_cast<const etxb_distribution_entry*>(ctx->image_dists[i * 2].ptr);
-        d.y_dist = reinterpret_cast<const etxb_distribution_entry*>(ctx->image_dists[i * 2 + 1].ptr);
-        d.has_distribution = 1;
+        st.images_uploaded += 1;
+      }
+      di.pixels_f32 = (im.format == 1u) ? reinterpret_cast<const float4*>(pixels.ptr) : nullptr;
+      di.pixels_u8 = (im.format == 2u) ? reinterpret_cast<const uchar4*>(pixels.ptr) : nullptr;
+      di.fsize_x = im.fsize[0]; di.fsize_y = im.fsize[1];
+      di.offset_x = im.offset[0]; di.offset_y = im.offset[1];
+      di.scale_x = im.scale[0]; di.scale_y = im.scale[1];
+      di.isize_x = im.isize[0]; di.isize_y = im.isize[1];
+      di.normalization = im.normalization;
+      di.options = im.options;
+      di.format = im.format;
+      if (table) {
+        di.x_dist = reinterpret_cast<const etxb_distribution_entry*>(x_dist.ptr);
+        di.y_dist = reinterpret_cast<const etxb_distribution_entry*>(y_dist.ptr);
+        di.has_distribution = 1;
       }
     }
     if (int rc = upload(ctx, ctx->images, dimgs.data(), dimgs.size())) return rc;
-    ctx->dscene.images = ctx->images.ptr;
-    ctx->dscene.image_count = uint32_t(dimgs.size());
+    d.images = ctx->images.ptr;
+    d.image_count = uint32_t(dimgs.size());
   }
-  if (s.emitter_instances.count == 0) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "scene has no emitters");
   const auto* spectra = static_cast<const etxb_spectrum*>(s.spectrums.a);
   std::vector<DSpectrum> dspec(s.spectrums.count);
   for (uint64_t i = 0; i < s.spectrums.count; ++i) {
-    const etxb_spectrum& sp = spectra[i];
-    if (sp.entry_count != 441) return fail(ctx, ETXB_ERR_UNSUPPORTED, "spectrum %llu has %u entries; the loader's 441-entry 390..830 nm grid is required", (unsigned long long)i, sp.entry_count);
-    for (uint32_t k = 0; k < 441; ++k) {
-      if (sp.entries[k].wavelength != float(390 + k)) return fail(ctx, ETXB_ERR_UNSUPPORTED, "spectrum %llu is not on the integer 390..830 nm grid", (unsigned long long)i);
-      dspec[i].power[k] = sp.entries[k].power;
-    }
-    memcpy(dspec[i].rgb, sp.integrated, 12);
+    for (uint32_t k = 0; k < 441; ++k) dspec[i].power[k] = spectra[i].entries[k].power;
+    memcpy(dspec[i].rgb, spectra[i].integrated, 12);
   }
 
   // ---- geometry ------------------------------------------------------------------------------------------------------
-  // every index the host builder and the kernels follow is checked here: a malformed scene is an error, not an out-of-bounds read
-  {
-    const auto* tris = static_cast<const etxb_triangle*>(s.triangles.a);
-    for (uint64_t i = 0; i < s.triangles.count; ++i) {
-      const etxb_triangle& t = tris[i];
-      if ((t.i[0] >= s.vertices.count) || (t.i[1] >= s.vertices.count) || (t.i[2] >= s.vertices.count))
-        return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "triangle %llu: vertex index out of range", (unsigned long long)i);
-      if (t.material_index >= s.materials.count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "triangle %llu: material index %u out of range", (unsigned long long)i, t.material_index);
-    }
-    if (s.triangle_to_emitter.count != s.triangles.count)
-      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "triangle_to_emitter has %llu entries for %llu triangles", (unsigned long long)s.triangle_to_emitter.count, (unsigned long long)s.triangles.count);
-    const auto* t2e = static_cast<const uint32_t*>(s.triangle_to_emitter.a);
-    for (uint64_t i = 0; i < s.triangle_to_emitter.count; ++i)
-      if ((t2e[i] != ETXB_INVALID_INDEX) && (t2e[i] >= s.emitter_instances.count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "triangle %llu: emitter index out of range", (unsigned long long)i);
-    for (uint64_t i = 0; i < s.emitter_instances.count; ++i) {
-      if (emitters[i].profile >= s.emitter_profiles.count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "emitter %llu: profile index out of range", (unsigned long long)i);
-      if ((emitters[i].cls == 0u) && (emitters[i].triangle_index >= s.triangles.count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "area emitter %llu: triangle index out of range", (unsigned long long)i);
-    }
-    if (!distribution_covers(s.emitters_distribution.values.count, s.emitter_instances.count))
-      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "emitter distribution has %llu entries for %llu emitters", (unsigned long long)s.emitters_distribution.values.count, (unsigned long long)s.emitter_instances.count);
-  }
-  const auto* verts = static_cast<const etxb_vertex*>(s.vertices.a);
-  std::vector<DVertex> dverts(s.vertices.count);
-  for (uint64_t i = 0; i < s.vertices.count; ++i) {
-    const etxb_vertex& v = verts[i];
-    dverts[i].pos_u = make_float4(v.pos[0], v.pos[1], v.pos[2], v.tex[0]);
-    dverts[i].nrm_v = make_float4(v.nrm[0], v.nrm[1], v.nrm[2], v.tex[1]);
-    dverts[i].tan = make_float4(v.tan[0], v.tan[1], v.tan[2], 0.0f);
-    dverts[i].btn = make_float4(v.btn[0], v.btn[1], v.btn[2], 0.0f);
-  }
   static_assert(sizeof(DTriangle) == sizeof(etxb_triangle), "triangle layout");
-  Bvh bvh;
-  {
-    cudaEvent_t dummy;
-    (void)dummy;
-    auto t0 = std::clock();
-    build_bvh(reinterpret_cast<const float*>(s.vertices.a), sizeof(etxb_vertex), reinterpret_cast<const uint32_t*>(s.triangles.a), sizeof(etxb_triangle),
-      uint32_t(s.triangles.count), bvh);
-    ctx->bvh_build_seconds = double(std::clock() - t0) / CLOCKS_PER_SEC;
+  if (!keep_geometry) {
+    const auto* verts = static_cast<const etxb_vertex*>(s.vertices.a);
+    std::vector<DVertex> dverts(s.vertices.count);
+    for (uint64_t i = 0; i < s.vertices.count; ++i) {
+      const etxb_vertex& v = verts[i];
+      dverts[i].pos_u = make_float4(v.pos[0], v.pos[1], v.pos[2], v.tex[0]);
+      dverts[i].nrm_v = make_float4(v.nrm[0], v.nrm[1], v.nrm[2], v.tex[1]);
+      dverts[i].tan = make_float4(v.tan[0], v.tan[1], v.tan[2], 0.0f);
+      dverts[i].btn = make_float4(v.btn[0], v.btn[1], v.btn[2], 0.0f);
+    }
+    if (int rc = upload(ctx, ctx->vertices, dverts.data(), dverts.size())) return rc;
+    if (int rc = upload(ctx, ctx->triangles, reinterpret_cast<const DTriangle*>(s.triangles.a), size_t(s.triangles.count))) return rc;
   }
-  if (bvh.max_depth >= uint32_t(kBvhStackSize)) return fail(ctx, ETXB_ERR_UNSUPPORTED, "BVH depth %u exceeds the traversal stack (%d)", bvh.max_depth, kBvhStackSize);
-  if (int rc = upload(ctx, ctx->vertices, dverts.data(), dverts.size())) return rc;
-  if (int rc = upload(ctx, ctx->triangles, reinterpret_cast<const DTriangle*>(s.triangles.a), size_t(s.triangles.count))) return rc;
   if (int rc = upload(ctx, ctx->tri_emitter, static_cast<const uint32_t*>(s.triangle_to_emitter.a), size_t(s.triangle_to_emitter.count))) return rc;
   if (int rc = upload(ctx, ctx->materials, mats, size_t(s.materials.count))) return rc;
   if (int rc = upload(ctx, ctx->profiles, static_cast<const etxb_emitter_profile*>(s.emitter_profiles.a), size_t(s.emitter_profiles.count))) return rc;
-  if (int rc = upload(ctx, ctx->emitters, emitters, size_t(s.emitter_instances.count))) return rc;
+  if (int rc = upload(ctx, ctx->emitters, static_cast<const etxb_emitter*>(s.emitter_instances.a), size_t(s.emitter_instances.count))) return rc;
   if (int rc = upload(ctx, ctx->spectra, dspec.data(), dspec.size())) return rc;
   if (int rc = upload(ctx, ctx->emitter_dist, static_cast<const etxb_distribution_entry*>(s.emitters_distribution.values.a), size_t(s.emitter_instances.count) + 1u))
     return rc;
-  if (int rc = upload(ctx, ctx->bvh_nodes, bvh.nodes.data(), bvh.nodes.size())) return rc;
-  if (int rc = upload(ctx, ctx->bvh_tris, reinterpret_cast<const float4*>(bvh.tri_pos.data()), bvh.tri_pos.size())) return rc;
-
-  DeviceScene& d = ctx->dscene;
+  if (!keep_geometry) {
+    if (int rc = upload(ctx, ctx->bvh_nodes, p.bvh.nodes.data(), p.bvh.nodes.size())) return rc;
+    if (int rc = upload(ctx, ctx->bvh_tris, reinterpret_cast<const float4*>(p.bvh.tri_pos.data()), p.bvh.tri_pos.size())) return rc;
+    d.bvh_node_count = uint32_t(p.bvh.nodes.size());
+  }
   d.vertices = ctx->vertices.ptr;
   d.triangles = ctx->triangles.ptr;
   d.tri_emitter = ctx->tri_emitter.ptr;
@@ -1338,19 +1518,39 @@ int etxb_upload_scene(etxb_ctx* ctx, const void* scene_blob, uint64_t scene_byte
   d.emitter_dist = ctx->emitter_dist.ptr;
   d.bvh_nodes = ctx->bvh_nodes.ptr;
   d.bvh_tris = ctx->bvh_tris.ptr;
-  d.bvh_node_count = uint32_t(bvh.nodes.size());
-  d.wide_nodes = nullptr;
-  d.wide_node_count = 0;
+  bool keep_wide = false;
 #if !(defined(ETXB_PARITY) && ETXB_PARITY)
-  if (ctx->has_stochastic_merge) {
+  // a geometry whose 4-wide tree the traversal stack cannot hold keeps that verdict with it: an update that keeps the geometry does not
+  // collapse the tree again only to reject it
+  if (!keep_geometry) ctx->wide_rejected = false;
+  keep_wide = keep_geometry && ctx->has_stochastic_merge && ((d.wide_nodes != nullptr) || ctx->wide_rejected);
+#endif
+  if (!keep_wide) {
+    d.wide_nodes = nullptr;
+    d.wide_node_count = 0;
+    if (reuse) ctx->wide_nodes.release();
+  }
+#if !(defined(ETXB_PARITY) && ETXB_PARITY)
+  if (ctx->has_stochastic_merge && !keep_wide) {
     // the sampler streams of such a scene's stochastic stages are the product build's own already: its traversal kernels may meet candidates in
     // another order, so they walk the 4-wide quantised form of the tree (dwide.cuh); Lambert / delta scenes keep the oracle's candidate order
-    WideBvh wide;
-    build_wide_bvh(bvh, wide);
-    if (wide.max_stack < uint32_t(kWideStackSize)) {
-      if (int rc = upload(ctx, ctx->wide_nodes, wide.nodes.data(), wide.nodes.size())) return rc;
+    if (!p.have_wide) {
+      auto t0 = std::chrono::steady_clock::now();
+      if (!p.have_bvh) {
+        // kept geometry that now needs the 4-wide tree: it is collapsed from the device's BVH2 nodes (the builder reads nothing else)
+        p.bvh.nodes.resize(ctx->bvh_nodes.count);
+        CUDA_OK(ctx, cudaMemcpy(p.bvh.nodes.data(), ctx->bvh_nodes.ptr, ctx->bvh_nodes.bytes(), cudaMemcpyDeviceToHost));
+      }
+      build_wide_bvh(p.bvh, p.wide);
+      p.have_wide = true;
+      p.bvh_seconds += seconds_since(t0);
+    }
+    if (p.wide.max_stack < uint32_t(kWideStackSize)) {
+      if (int rc = upload(ctx, ctx->wide_nodes, p.wide.nodes.data(), p.wide.nodes.size())) return rc;
       d.wide_nodes = ctx->wide_nodes.ptr;
-      d.wide_node_count = uint32_t(wide.nodes.size());
+      d.wide_node_count = uint32_t(p.wide.nodes.size());
+    } else {
+      ctx->wide_rejected = true;
     }
   }
 #endif
@@ -1372,45 +1572,55 @@ int etxb_upload_scene(etxb_ctx* ctx, const void* scene_blob, uint64_t scene_byte
   d.default_conductor_k = s.default_conductor_k;
   d.camera = cam;
   ctx->spectral = d.spectral != 0;
-  if ((s.pixel_sampler_image != 0xffffffffu) && (s.pixel_sampler_image >= s.images.count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "pixel sampler image out of range");
   ctx->pixel_sampler_image = s.pixel_sampler_image;
   ctx->pixel_sampler_radius = s.pixel_sampler_radius;
   ctx->noise_threshold = s.noise_threshold;
   ctx->radiance_clamp = s.radiance_clamp;
   ctx->scene_samples = s.samples;
-  ctx->film_normals.release();  // sized by the film: re-allocated by the next path-tracer run
 
   // ---- film + queues (Film::allocate, film.cxx) ----------------------------------------------------------------------
+  // an update keeps every buffer whose size is what the upload would allocate (DevBuf::ensure)
+  uint32_t allocations = 0;
+  auto sized = [&](auto& b, size_t count) -> cudaError_t {
+    if (reuse) return b.ensure(count, allocations);
+    allocations += 1;
+    return b.alloc(count);
+  };
   ctx->width = cam.film_size[0];
   ctx->height = cam.film_size[1];
   ctx->path_count = ctx->width * ctx->height;
   size_t n = ctx->path_count;
-  if (n == 0) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "empty film");
+  if (!reuse) {
+    ctx->film_normals.release();  // sized by the film: re-allocated by the next path-tracer run
+  } else if (ctx->film_normals.ptr && (ctx->film_normals.count != n)) {
+    if (int rc = pt_ensure_film(ctx)) return rc;  // the path tracer's layers and per-pixel history at the new film size
+    allocations += 1;
+  }
   DevBuf<float4>* per_path_f4[] = {&ctx->ray_o, &ctx->ray_d, &ctx->thr, &ctx->mis, &ctx->hit, &ctx->gathered, &ctx->merged, &ctx->camera_value, &ctx->film_camera,
     &ctx->film_light, &ctx->film_light_iteration, &ctx->film_out, &ctx->bs_weight_pdf, &ctx->bs_wo_eta};
-  for (auto* b : per_path_f4) CUDA_OK(ctx, b->alloc(n));
-  CUDA_OK(ctx, ctx->bs_props.alloc(n));
-  CUDA_OK(ctx, ctx->misc.alloc(n));
-  CUDA_OK(ctx, ctx->wavelength.alloc(n));
+  for (auto* b : per_path_f4) CUDA_OK(ctx, sized(*b, n));
+  CUDA_OK(ctx, sized(ctx->bs_props, n));
+  CUDA_OK(ctx, sized(ctx->misc, n));
+  CUDA_OK(ctx, sized(ctx->wavelength, n));
   DevBuf<uint32_t>* per_path_u32[] = {&ctx->lv_count, &ctx->lp_offset, &ctx->queue_a, &ctx->queue_b, &ctx->sampler_end_light, &ctx->sampler_end_camera, &ctx->merge_key};
-  for (auto* b : per_path_u32) CUDA_OK(ctx, b->alloc(n));
-  CUDA_OK(ctx, ctx->conn_count.alloc(1));
-  CUDA_OK(ctx, ctx->queue_counts.alloc(4));
-  CUDA_OK(ctx, ctx->lv_tmp_count.alloc(1));
-  CUDA_OK(ctx, ctx->overflow.alloc(1));
-  CUDA_OK(ctx, ctx->grid_bbox.alloc(8));
-  CUDA_OK(ctx, ctx->counters.alloc(1));
+  for (auto* b : per_path_u32) CUDA_OK(ctx, sized(*b, n));
+  CUDA_OK(ctx, sized(ctx->conn_count, 1));
+  CUDA_OK(ctx, sized(ctx->queue_counts, 4));
+  CUDA_OK(ctx, sized(ctx->lv_tmp_count, 1));
+  CUDA_OK(ctx, sized(ctx->overflow, 1));
+  CUDA_OK(ctx, sized(ctx->grid_bbox, 8));
+  CUDA_OK(ctx, sized(ctx->counters, 1));
   uint64_t cap = ctx->max_light_vertices_cfg ? ctx->max_light_vertices_cfg : uint64_t(n) * 16ull;
   cap = std::min<uint64_t>(cap, 0x7fffffffull);
   ctx->lv_capacity = uint32_t(cap);
-  CUDA_OK(ctx, ctx->lv_tmp.alloc(cap));
-  CUDA_OK(ctx, ctx->lv_final.alloc(cap));
-  CUDA_OK(ctx, ctx->conn_list.alloc(cap));
+  CUDA_OK(ctx, sized(ctx->lv_tmp, cap));
+  CUDA_OK(ctx, sized(ctx->lv_final, cap));
+  CUDA_OK(ctx, sized(ctx->conn_list, cap));
   if (ctx->has_stochastic_merge) {
-    CUDA_OK(ctx, ctx->conn_list_sorted.alloc(cap));
-    CUDA_OK(ctx, ctx->queue_sorted.alloc(n));
-    CUDA_OK(ctx, ctx->queue_keys.alloc(n));
-    CUDA_OK(ctx, ctx->queue_keys_sorted.alloc(n));
+    CUDA_OK(ctx, sized(ctx->conn_list_sorted, cap));
+    CUDA_OK(ctx, sized(ctx->queue_sorted, n));
+    CUDA_OK(ctx, sized(ctx->queue_keys, n));
+    CUDA_OK(ctx, sized(ctx->queue_keys_sorted, n));
   } else {
     ctx->conn_list_sorted.release();
     ctx->queue_sorted.release();
@@ -1422,22 +1632,22 @@ int etxb_upload_scene(etxb_ctx* ctx, const void* scene_blob, uint64_t scene_byte
 #else
   // the connection stage's per-path camera vertex records (make_params: connect_stage = has_stochastic_merge)
   if (ctx->has_stochastic_merge) {
-    CUDA_OK(ctx, ctx->conn_rec.alloc(n * (ctx->spectral ? kConnRecRows<true> : kConnRecRows<false>)));
+    CUDA_OK(ctx, sized(ctx->conn_rec, n * (ctx->spectral ? kConnRecRows<true> : kConnRecRows<false>)));
   } else {
     ctx->conn_rec.release();
   }
 #endif
-  CUDA_OK(ctx, ctx->trace_cursor.alloc(1));
+  CUDA_OK(ctx, sized(ctx->trace_cursor, 1));
   const bool atomic_candidate = ctx->opaque_scene && ctx->plain_scene && ctx->has_stochastic_merge;
   if (ctx->dscene.deferred_shadow_rays || atomic_candidate) {
     // atomic mode: a camera bounce queues its vertex connections (<= cap, the pair list's capacity) plus one emitter segment per path
     const uint64_t shadow_cap = std::min<uint64_t>(cap + (atomic_candidate ? n : 0), 0x7fffffffull);
-    CUDA_OK(ctx, ctx->shadow_span.alloc(n));
-    CUDA_OK(ctx, ctx->shadow_p0.alloc(shadow_cap));
-    CUDA_OK(ctx, ctx->shadow_p1.alloc(shadow_cap));
-    CUDA_OK(ctx, ctx->shadow_value.alloc(shadow_cap));
-    CUDA_OK(ctx, ctx->shadow_result.alloc(shadow_cap));
-    CUDA_OK(ctx, ctx->shadow_count.alloc(2));
+    CUDA_OK(ctx, sized(ctx->shadow_span, n));
+    CUDA_OK(ctx, sized(ctx->shadow_p0, shadow_cap));
+    CUDA_OK(ctx, sized(ctx->shadow_p1, shadow_cap));
+    CUDA_OK(ctx, sized(ctx->shadow_value, shadow_cap));
+    CUDA_OK(ctx, sized(ctx->shadow_result, shadow_cap));
+    CUDA_OK(ctx, sized(ctx->shadow_count, 2));
   } else {
     ctx->shadow_span.release();
     ctx->shadow_p0.release();
@@ -1448,17 +1658,17 @@ int etxb_upload_scene(etxb_ctx* ctx, const void* scene_blob, uint64_t scene_byte
   // the sort buffers also hold the gather queue and the path queues (up to one entry per path), whatever the configured pool capacity
   const uint64_t sort_cap = std::max<uint64_t>(cap, n);
   DevBuf<uint32_t>* per_vertex_u32[] = {&ctx->keys_in, &ctx->keys_out, &ctx->vals_in, &ctx->vals_out};
-  for (auto* b : per_vertex_u32) CUDA_OK(ctx, b->alloc(sort_cap));
+  for (auto* b : per_vertex_u32) CUDA_OK(ctx, sized(*b, sort_cap));
   DevBuf<float4>* per_vertex_f4[] = {&ctx->g_pos, &ctx->g_nrm, &ctx->g_win, &ctx->g_thr};
-  for (auto* b : per_vertex_f4) CUDA_OK(ctx, b->alloc(cap));
-  CUDA_OK(ctx, ctx->cell_range.alloc(next_pow2(cap)));
+  for (auto* b : per_vertex_f4) CUDA_OK(ctx, sized(*b, cap));
+  CUDA_OK(ctx, sized(ctx->cell_range, next_pow2(cap)));
   // one scratch buffer for every CUB call of an iteration: the 32-bit pair sorts (photon grid, gather queue, path queues), the pair-list
   // sort with its 64-bit (path, light vertex) values, and the scan over the per-path vertex counts
   size_t temp_sort = 0, temp_sort64 = 0, temp_scan = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, temp_sort, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, int(sort_cap));
   cub::DeviceRadixSort::SortPairs(nullptr, temp_sort64, (uint32_t*)nullptr, (uint32_t*)nullptr, (unsigned long long*)nullptr, (unsigned long long*)nullptr, int(sort_cap), 0, 16);
   cub::DeviceScan::ExclusiveSum(nullptr, temp_scan, (uint32_t*)nullptr, (uint32_t*)nullptr, int(n));
-  CUDA_OK(ctx, ctx->cub_temp.alloc(std::max(std::max(temp_sort, temp_sort64), temp_scan) + 256));
+  CUDA_OK(ctx, sized(ctx->cub_temp, std::max(std::max(temp_sort, temp_sort64), temp_scan) + 256));
   CUDA_OK(ctx, cudaMemsetAsync(ctx->overflow.ptr, 0, 4, ctx->stream));
   CUDA_OK(ctx, cudaMemsetAsync(ctx->counters.ptr, 0, sizeof(DeviceCounters), ctx->stream));
   CUDA_OK(ctx, cudaMemsetAsync(ctx->sampler_end_light.ptr, 0, n * 4, ctx->stream));
@@ -1466,8 +1676,49 @@ int etxb_upload_scene(etxb_ctx* ctx, const void* scene_blob, uint64_t scene_byte
   CUDA_OK(ctx, cudaMemsetAsync(ctx->lv_count.ptr, 0, n * 4, ctx->stream));
   CUDA_OK(ctx, cudaMemsetAsync(ctx->lp_offset.ptr, 0, n * 4, ctx->stream));
   CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+  ctx->hashes = p.hashes;
   ctx->scene_ready = true;
+  if (info) {
+    st.kept = (keep_geometry ? ETXB_KEPT_GEOMETRY : 0u) | ((keep_wide && (d.wide_nodes != nullptr)) ? ETXB_KEPT_WIDE_TREE : 0u) | (allocations == 0 ? ETXB_KEPT_PATH_STATE : 0u);
+    st.fingerprint_seconds = p.fingerprint_seconds;
+    st.bytes_hashed = p.bytes_hashed;
+    st.bvh_seconds = p.bvh_seconds;
+    *info = st;
+  }
   return etxb_begin(ctx, 0);
+}
+
+}  // namespace
+}  // extern "C++"
+
+int etxb_upload_scene(etxb_ctx* ctx, const void* scene_blob, uint64_t scene_bytes, const void* camera_blob, uint64_t camera_bytes) {
+  if (!ctx || !scene_blob || !camera_blob) return ETXB_ERR_INVALID_ARGUMENT;
+  if (int rc = check_scene_args(ctx, scene_bytes, camera_bytes)) return rc;
+  ctx_drain_impl(ctx);
+  cudaSetDevice(ctx->device);
+  ctx->scene_ready = false;
+  const etxb_scene& s = *static_cast<const etxb_scene*>(scene_blob);
+  const etxb_camera& cam = *static_cast<const etxb_camera*>(camera_blob);
+  ScenePrep p;
+  if (int rc = prepare_scene(ctx, s, cam, p)) return rc;
+  return commit_scene(ctx, s, cam, p, false, nullptr);
+}
+
+int etxb_update_scene(etxb_ctx* ctx, const void* scene_blob, uint64_t scene_bytes, const void* camera_blob, uint64_t camera_bytes, etxb_update_info* info) {
+  const auto t0 = std::chrono::steady_clock::now();
+  if (info) memset(info, 0, sizeof(*info));
+  if (!ctx || !scene_blob || !camera_blob) return ETXB_ERR_INVALID_ARGUMENT;
+  if (int rc = check_scene_args(ctx, scene_bytes, camera_bytes)) return rc;
+  if (ctx->comm != nullptr) return fail(ctx, ETXB_ERR_UNSUPPORTED, "etxb_update_scene: a context with a communicator takes a new scene through etxb_upload_scene");
+  ctx_drain_impl(ctx);
+  cudaSetDevice(ctx->device);
+  const etxb_scene& s = *static_cast<const etxb_scene*>(scene_blob);
+  const etxb_camera& cam = *static_cast<const etxb_camera*>(camera_blob);
+  ScenePrep p;
+  if (int rc = prepare_scene(ctx, s, cam, p)) return rc;
+  int rc = commit_scene(ctx, s, cam, p, ctx->scene_ready, info);
+  if (info) info->total_seconds = seconds_since(t0);
+  return rc;
 }
 
 void etxb_options_default(etxb_vcm_options* opt) {
@@ -2412,6 +2663,50 @@ int etxb_group_begin(etxb_group* grp, uint32_t first_iteration) {
   grp->error = ETXB_OK;
   grp->error_text.clear();
   return ETXB_OK;
+}
+
+int etxb_group_update_scene(etxb_group* grp, const void* scene_blob, uint64_t scene_bytes, const void* camera_blob, uint64_t camera_bytes, etxb_update_info* info) {
+  const auto t0 = std::chrono::steady_clock::now();
+  if (info) memset(info, 0, sizeof(*info));
+  if (!grp || !scene_blob || !camera_blob) return ETXB_ERR_INVALID_ARGUMENT;
+  etxb_ctx* first = grp->lanes[0];
+  auto refuse = [&](int rc) {
+    std::lock_guard<std::mutex> lock(grp->m);
+    grp->error_text = etxb_last_error(first);
+    return rc;
+  };
+  bool comm = grp->sharded || grp->replicas;
+  for (auto* c : grp->lanes) comm = comm || (c->comm != nullptr);
+  if (comm) return refuse(fail(first, ETXB_ERR_UNSUPPORTED, "etxb_group_update_scene: a group with communicators takes a new scene through etxb_upload_scene on each lane"));
+  if (int rc = check_scene_args(first, scene_bytes, camera_bytes)) return refuse(rc);
+  if (int rc = etxb_group_wait(grp)) return rc;
+  const etxb_scene& s = *static_cast<const etxb_scene*>(scene_blob);
+  const etxb_camera& cam = *static_cast<const etxb_camera*>(camera_blob);
+  cudaSetDevice(grp->device);
+  // hashed and validated once; a new geometry's BVH is built once, and its depth checked, before any lane changes
+  ScenePrep p;
+  if (int rc = prepare_scene(first, s, cam, p)) return refuse(rc);
+  for (auto* c : grp->lanes)
+    if (!geometry_kept(c, p, c->scene_ready))
+      if (int rc = prepare_bvh(first, s, p)) return refuse(rc);
+  uint32_t kept = ~0u;
+  for (size_t l = 0; l < grp->lanes.size(); ++l) {
+    etxb_ctx* c = grp->lanes[l];
+    etxb_update_info lane = {};
+    ctx_drain_impl(c);
+    if (int rc = commit_scene(c, s, cam, p, c->scene_ready, &lane)) {
+      std::lock_guard<std::mutex> lock(grp->m);
+      grp->error_text = etxb_last_error(c);
+      return rc;
+    }
+    kept &= lane.kept;
+    if (info && (l == 0)) *info = lane;
+  }
+  if (info) {
+    info->kept = kept;  // what every lane kept; the image and grid counts are lane 0's
+    info->total_seconds = seconds_since(t0);
+  }
+  return etxb_group_begin(grp, 0);
 }
 
 int etxb_group_set_stride(etxb_group* grp, uint32_t stride) {

@@ -73,6 +73,21 @@ class GPUVCM {
     if (_scene_committed) _samples = etxb_scene_file_scene(file)->samples;
     return rc;
   }
+  // The application's restart after it edited the committed PODs (camera moves, material / medium / emitter / settings edits,
+  // app.cxx:131-141, 368-403): etxb_update_scene keeps on the device what the edit did not change.  A render that was running starts again
+  // from iteration 0; a refused edit leaves the previous scene committed (and restarts it).
+  int update_scene(const void* scene, uint64_t scene_bytes, const void* camera, uint64_t camera_bytes, uint32_t samples, etxb_update_info* info = nullptr) {
+    const bool was_running = (_state.load() != State::Stopped);
+    stop(Stop::Immediate);
+    if (!enabled()) return _create_result;
+    int rc = etxb_update_scene(_ctx, scene, scene_bytes, camera, camera_bytes, info);
+    if (rc == ETXB_OK) {
+      _scene_committed = true;
+      _samples = samples;
+    }
+    if (was_running) run();
+    return rc;
+  }
   int upload_tables(const float* xyz_441x3, const float* rgb_response_391x3, const uint8_t* sobol, const uint8_t* scrambling, const uint8_t* ranking) {
     if (!enabled()) return _create_result;
     int rc = etxb_upload_color_tables(_ctx, xyz_441x3, rgb_response_391x3);

@@ -101,6 +101,11 @@ COUNTERS = np.dtype([(n, u8) for n in (
     "rays_closest", "rays_shadow", "nodes_visited", "tris_tested", "bounces_light", "bounces_camera", "light_vertices",
     "connections", "merge_queries", "merge_candidates", "merge_accepts", "splats", "kernel_launches", "nodes_closest", "tris_closest")])
 DEVICE_CONFIG = np.dtype([("device_index", np.int32), ("max_light_vertices", u4), ("flags", u4), ("pad", u4)])
+# etxb_update_info (etxb_update_scene / etxb_group_update_scene), 56 B with the C padding before the doubles
+UPDATE_INFO = np.dtype({"names": ["kept", "images_kept", "images_uploaded", "grids_kept", "grids_uploaded", "fingerprint_seconds", "bvh_seconds", "total_seconds",
+                                  "bytes_hashed"],
+                        "formats": [u4, u4, u4, u4, u4, np.float64, np.float64, np.float64, u8], "offsets": [0, 4, 8, 12, 16, 24, 32, 40, 48], "itemsize": 56})
+KEPT_GEOMETRY, KEPT_WIDE_TREE, KEPT_PATH_STATE = 1, 2, 4
 # etxb_closure_query (96 B) and the per-query statistics etxb_debug_closure_eval / oracle_bsdf_eval return (include/etx_b200.h)
 CLOSURE_QUERY = np.dtype([
     ("nrm", f4, 3), ("tan", f4, 3), ("btn", f4, 3), ("w_i", f4, 3), ("w_o", f4, 3), ("uv", f4, 2), ("wavelength", f4),

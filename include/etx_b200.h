@@ -309,6 +309,35 @@ const char* etxb_last_error(const etxb_ctx* ctx);
  * allocates film + queues for camera->film_size.  `scene`/`camera` use the reference layouts. */
 int etxb_upload_scene(etxb_ctx* ctx, const void* scene, uint64_t scene_bytes, const void* camera, uint64_t camera_bytes);
 
+/* The restart after an edit of the committed Scene / Camera (the application restarts its integrator after every camera move and every
+ * material, medium, emitter or scene-settings edit, app.cxx:131-141, 368-403).  The context then renders exactly what a fresh context
+ * renders after etxb_upload_scene with the same PODs: the film is cleared and etxb_begin(ctx, 0) applied; options and the selected
+ * integrator stay.  What is reused is decided by content, never by pointer (the application edits the PODs in place and
+ * rebuild_area_emitters reallocates its arrays): upload and update record a 128-bit hash of the vertex + triangle arrays, of each image
+ * (pixels, sampling tables, scalar fields) and of each density grid (values, dimensions).
+ *  - same geometry hash: the device vertices, triangles and BVH2 stay (no BVH build), and the 4-wide tree of a product-build scene with
+ *    stochastic BSDFs stays; an edit that newly needs that tree collapses it from the device's BVH2;
+ *  - images and density grids: each kept or copied on its own hash;
+ *  - per-path / per-vertex / shadow / connection-record / sort / film buffers: kept where the upload would allocate the same size;
+ *  - everything else (materials, spectra, emitters, their distribution, media records, scene scalars, camera, scene-class flags) is
+ *    derived again as the upload derives it.
+ * Every check of the upload runs before any device buffer changes: a refused update returns the error and the previous scene stays
+ * committed and renderable.  A CUDA failure part-way leaves the scene not ready, like a failed upload.  Iterations in flight are drained
+ * first.  Without a committed scene it is an upload.  ETXB_ERR_UNSUPPORTED on a context with a communicator (etxb_comm_init).
+ * `info` (may be NULL) reports what was kept, the bytes hashed and the host time spent hashing, building trees (BVH2 and 4-wide) and in
+ * the whole call. */
+typedef struct etxb_update_info {
+  uint32_t kept; /* ETXB_KEPT_* bits */
+  uint32_t images_kept, images_uploaded;
+  uint32_t grids_kept, grids_uploaded;
+  double fingerprint_seconds, bvh_seconds, total_seconds;
+  uint64_t bytes_hashed; /* what the content hashes read: geometry, images with their sampling tables, density grids */
+} etxb_update_info;
+#define ETXB_KEPT_GEOMETRY (1u << 0)   /* device vertices + triangles + BVH2 */
+#define ETXB_KEPT_WIDE_TREE (1u << 1)  /* the 4-wide tree (product build, scenes with stochastic BSDFs; set only where one exists) */
+#define ETXB_KEPT_PATH_STATE (1u << 2) /* per-path / per-vertex / film buffers not re-allocated */
+int etxb_update_scene(etxb_ctx* ctx, const void* scene, uint64_t scene_bytes, const void* camera, uint64_t camera_bytes, etxb_update_info* info);
+
 /* Blue-noise tables (thirdparty/bluenoise): sobol[256*256], and for the variant selected by
  * next_power(min(scene.samples,256)) (bluenoise.cxx:73-95) scrambling[128*128*8], ranking[128*128*8], as uint8. */
 int etxb_upload_blue_noise(etxb_ctx* ctx, const uint8_t* sobol_256x256, const uint8_t* scrambling, const uint8_t* ranking);
@@ -496,6 +525,10 @@ uint32_t etxb_group_lanes(const etxb_group* group);
 etxb_ctx* etxb_group_lane(etxb_group* group, uint32_t lane);
 const char* etxb_group_last_error(const etxb_group* group);
 int etxb_group_begin(etxb_group* group, uint32_t first_iteration);   /* Integrator::run: clears every lane's film */
+/* etxb_update_scene for every lane: waits for the group to go idle, validates and hashes once (and builds a new geometry's BVH once),
+ * updates each lane, then etxb_group_begin(group, 0).  `info` is lane 0's, with `kept` the bits every lane kept.  ETXB_ERR_UNSUPPORTED on
+ * a group with communicators (etxb_group_comm_init, etxb_group_comm_init_replicas). */
+int etxb_group_update_scene(etxb_group* group, const void* scene, uint64_t scene_bytes, const void* camera, uint64_t camera_bytes, etxb_update_info* info);
 int etxb_group_set_stride(etxb_group* group, uint32_t stride);       /* the k-th iteration handed out renders index first + k * stride
                                                                         (iteration-interleaved multi-GPU runs: first = rank, stride = ranks) */
 int etxb_group_enqueue(etxb_group* group, uint32_t iterations);      /* asynchronous: queues `iterations` more iterations */
