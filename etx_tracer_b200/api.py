@@ -128,6 +128,9 @@ def load_library(flavor="fast"):
     lib.etxb_debug_sampler.argtypes = [vp, vp, vp, u32, u32, vp, vp]
     lib.etxb_debug_math.argtypes = [vp, u32, vp, vp, u32, vp]
     lib.etxb_debug_closure_eval.argtypes = [vp, vp, u32, u32, vp]
+    lib.etxb_debug_set_thresholds.argtypes = [vp, vp]
+    lib.etxb_debug_get_branch_counts.argtypes = [vp, vp]
+    lib.etxb_debug_merge.argtypes = [vp, vp, u32, vp, vp, u32, vp, vp]
     _libs[flavor] = lib
     return lib
 
@@ -508,6 +511,37 @@ class GPUVCM:
         out = np.zeros((queries.shape[0], S.CLOSURE_STATS), dtype=np.float64)
         self._check(self.lib.etxb_debug_closure_eval(self.h, _p(queries), queries.shape[0], int(repetitions), _p(out)))
         return out
+
+    def debug_thresholds(self, **fields):
+        """The queue sizes from which the passes take their large-queue branches (etxb_debug_set_thresholds): keyword fields of
+        S.DEBUG_THRESHOLDS, the others at their defaults; 0 = always, S.NEVER = never.  No argument restores the defaults."""
+        unknown = set(fields) - set(S.DEFAULT_THRESHOLDS)
+        if unknown:
+            raise ValueError(f"unknown thresholds {sorted(unknown)}")
+        t = np.zeros(1, dtype=S.DEBUG_THRESHOLDS)
+        for k, v in dict(S.DEFAULT_THRESHOLDS, **fields).items():
+            t[k] = v
+        self._check(self.lib.etxb_debug_set_thresholds(self.h, _p(t)))
+
+    def debug_branch_counts(self):
+        """etxb_debug_get_branch_counts as a dict; `merge_qpw` maps queries per warp (1 .. 32) to gather launches."""
+        c = np.zeros(1, dtype=S.DEBUG_BRANCH_COUNTS)
+        self._check(self.lib.etxb_debug_get_branch_counts(self.h, _p(c)))
+        out = {k: int(c[k][0]) for k in ("merge_sorts", "connect_launches", "pair_sorts", "queue_sorts")}
+        out["merge_qpw"] = {q: int(n) for q, n in zip(S.MERGE_QPW, c["merge_launches"][0])}
+        return out
+
+    def debug_merge(self, records, light_wavelengths, queries):
+        """The photon gather query by query (etxb_debug_merge): S.LIGHT_VERTEX_REC records, one wavelength per light path index (path_count of
+        them), S.MERGE_QUERY records; returns (S.MERGE_RESULT per query, S.MERGE_GRID as a dict).  Leaves the context to etxb_begin."""
+        records = np.ascontiguousarray(records, dtype=S.LIGHT_VERTEX_REC)
+        wl = np.zeros(self.width * self.height, dtype=np.float32)
+        wl[:len(light_wavelengths)] = light_wavelengths
+        queries = np.ascontiguousarray(queries, dtype=S.MERGE_QUERY)
+        out = np.zeros(queries.shape[0], dtype=S.MERGE_RESULT)
+        grid = np.zeros(1, dtype=S.MERGE_GRID)
+        self._check(self.lib.etxb_debug_merge(self.h, _p(records), records.shape[0], _p(wl), _p(queries), queries.shape[0], _p(out), _p(grid)))
+        return out, {k: (grid[k][0].copy() if grid[k][0].ndim else grid[k][0].item()) for k in grid.dtype.names}
 
 
 class GPUPathTracing(GPUVCM):

@@ -1892,4 +1892,32 @@ __global__ void k_debug_closure(const __grid_constant__ DeviceScene sc, const et
   for (uint32_t k = 27; k < ETXB_CLOSURE_STATS; ++k) o[k] = 0.0;
 }
 
+// etxb_debug_merge: query i becomes path i of a one-bounce queue, staged in the columns the gather kernels read (hit record, ray
+// direction, throughput, MIS terms, sampler, depth, medium, wavelength), with the merge key k_camera_shade would give it.  Writes the
+// staged camera vertex's position and normal to pos_nrm[2 i], [2 i + 1], and i to queue slot i.
+template <bool SP>
+__global__ void k_debug_merge_stage(const __grid_constant__ LaunchParams p, const etxb_merge_query* queries, uint32_t count, uint32_t* queue, float4* pos_nrm) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  queue[i] = i;
+  const etxb_merge_query& q = queries[i];
+  const float4 hit = make_float4(q.u, q.v, 0.0f, __uint_as_float(q.tri));
+  p.paths.hit[i] = hit;
+  p.paths.ray_o[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+  p.paths.ray_d[i] = make_float4(q.w_i[0], q.w_i[1], q.w_i[2], kMaxFloat);
+  p.paths.thr[i] = make_float4(q.throughput[0], q.throughput[1], q.throughput[2], 0.0f);
+  p.paths.mis[i] = make_float4(q.d_vcm, 0.0f, q.d_vm, 1.0f);
+  p.paths.misc[i] = make_uint4(q.seed, q.total_path_depth, q.medium, 0u);
+  p.paths.wavelength[i] = SP ? q.wavelength : -1.0f;
+  p.paths.bs_props[i] = make_uint2(0u, q.medium);
+  p.paths.merged[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+  const PathState<SP> state = load_state<SP>(p.paths, i);
+  const Isect isect = stage_intersection<SP>(p, state, i, hit);
+  uint32_t key = merge_query_key(p.grid, isect.pos);
+  if (p.merge_material_major && (key != 0xffffffffu)) key = (umin(isect.material_index, 0x7eu) << 24) | (key >> 6);
+  p.paths.merge_key[i] = key;
+  pos_nrm[2u * i] = make_float4(isect.pos.x, isect.pos.y, isect.pos.z, 0.0f);
+  pos_nrm[2u * i + 1u] = make_float4(isect.nrm.x, isect.nrm.y, isect.nrm.z, 0.0f);
+}
+
 }  // namespace etxb

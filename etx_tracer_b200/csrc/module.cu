@@ -69,6 +69,13 @@ const char* kKernelNames[K_COUNT] = {"light_begin", "trace_closest(light)", "lig
   "camera_begin", "trace_closest(camera)", "camera_shade", "camera_connect", "shadow_trace", "queue_sort", "camera_merge_sort", "camera_merge", "camera_merge_generic", "camera_continue", "film_commit_light", "nccl_allreduce_light_image", "nccl_allgather_photons",
   "pt_begin", "pt_shade", "pt_accumulate", "film_noise_levels"};
 
+// Queue sizes from which a pass takes its large-queue branches (the context's `thresholds`; etxb_debug_set_thresholds overrides them):
+//   merge_sort_min_queries  the gather queue is sorted by its merge keys (below it, a latency-bound tail, the sort launches cost more than they save)
+//   merge_min_warps_per_sm  the gather gives each warp up to 32 queries while the queue still fills this many warps per SM
+//   tail_queue              vertex connections go through the host-sized, material-pair-sorted list, and the queue count is read every bounce
+//   sort_queue_min          path queues and connection lists are grouped by material (scenes with stochastic BSDFs)
+constexpr etxb_debug_thresholds kDefaultThresholds = {16384u, 32u, 8192u, 1024u, 0u};
+
 template <class T>
 struct DevBuf {
   T* ptr = nullptr;
@@ -227,6 +234,9 @@ struct etxb_ctx {
   uint64_t kernel_launches = 0;
   GridData grid = {};
   bool light_pass_done = false, grid_done = false;
+  // queue sizes from which a pass takes its large-queue branches (etxb_debug_set_thresholds; 0 = always, 0xffffffff = never), and what ran
+  etxb_debug_thresholds thresholds = kDefaultThresholds;
+  etxb_debug_branch_counts branch_counts = {};
 
   // pixel-tile sharding across processes (one per GPU): NCCL communicator over NVLink, created by etxb_comm_init
   ncclComm_t comm = nullptr;
@@ -448,8 +458,6 @@ LaunchParams make_params(etxb_ctx* ctx) {
 }
 
 uint32_t blocks_for(uint32_t n, uint32_t block) { return (n + block - 1u) / block; }
-constexpr uint32_t kMergeSortMinQueries = 16384u;  // below this the merge queries are not sorted
-constexpr uint32_t kMergeMinWarpsPerSm = 32u;      // the merge wants at least this many warps in flight per SM
 
 int read_u32(etxb_ctx* ctx, const uint32_t* dptr, uint32_t& out) {
   CUDA_OK(ctx, cudaMemcpyAsync(&out, dptr, 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -459,11 +467,11 @@ int read_u32(etxb_ctx* ctx, const uint32_t* dptr, uint32_t& out) {
 
 // Size of the next bounce's queue.  A long queue is read back every bounce (the grids are sized by it).  In the tail of a pass the
 // queue only shrinks and every kernel guards on the device-side count, so the previous size stays a valid upper bound for the launch
-// grids: the host then enqueues several bounces back to back and reads the count only every kTailBatch bounces.
-constexpr uint32_t kTailQueue = 8192u;
+// grids: the host then enqueues several bounces back to back and reads the count only every kTailBatch bounces.  A tail starts below
+// thresholds.tail_queue.
 constexpr uint32_t kTailBatch = 4u;
 int next_queue_size(etxb_ctx* ctx, const uint32_t* dptr, uint32_t& active, uint32_t& unsynced) {
-  if ((active < kTailQueue) && (unsynced + 1u < kTailBatch)) {
+  if ((active < ctx->thresholds.tail_queue) && (unsynced + 1u < kTailBatch)) {
     unsynced += 1u;
     return ETXB_OK;
   }
@@ -474,10 +482,10 @@ int next_queue_size(etxb_ctx* ctx, const uint32_t* dptr, uint32_t& active, uint3
 // Scenes with stochastic BSDFs: the bounce kernels spend their time in the BSDF class of the surface that was hit, and a warp that holds
 // several classes runs them one after the other.  k_trace_closest leaves one key per queue slot (material index; 0xff = miss; 0x100 = slot
 // past the device-side count); a stable 9-bit radix sort groups the queue, slots past the count stay at the end.  Returns the queue the
-// rest of the bounce must use.  Short queues (the tail of a pass) are latency bound and skip it.
-constexpr uint32_t kSortQueueMin = 1024u;
-inline bool sorts_queue(const etxb_ctx* ctx, uint32_t active) { return ctx->has_stochastic_merge && (active >= kSortQueueMin) && ctx->queue_sorted.count; }
+// rest of the bounce must use.  Short queues (the tail of a pass, below thresholds.sort_queue_min) are latency bound and skip it.
+inline bool sorts_queue(const etxb_ctx* ctx, uint32_t active) { return ctx->has_stochastic_merge && (active >= ctx->thresholds.sort_queue_min) && ctx->queue_sorted.count; }
 int sort_queue_by_material(etxb_ctx* ctx, const uint32_t* queue, uint32_t active, const uint32_t** sorted) {
+  ctx->branch_counts.queue_sorts += 1;
   size_t temp_bytes = ctx->cub_temp.bytes();
   CUDA_OK(ctx, cub::DeviceRadixSort::SortPairs(ctx->cub_temp.ptr, temp_bytes, ctx->queue_keys.ptr, ctx->queue_keys_sorted.ptr, queue, ctx->queue_sorted.ptr, int(active), 0, 9,
                  ctx->stream));
@@ -645,6 +653,50 @@ int run_grid_build(etxb_ctx* ctx, const LightVertexRec* records, uint32_t count)
   return ETXB_OK;
 }
 
+// The photon gather of a bounce over queue `q` (`active` slots, device-side count at `count`); merge_key holds one key per slot.  The parity
+// build runs the serial, reference-ordered gather; the product build the warp-cooperative Lambert gather and, in scenes with stochastic
+// BSDFs, the closure gather.  `active` must be the exact count when the queue is sorted here: a stale slot past the count would be sorted in.
+template <bool SP>
+int launch_merge(etxb_ctx* ctx, const LaunchParams& p, const uint32_t* q, const uint32_t* count, uint32_t active) {
+#if defined(ETXB_PARITY) && ETXB_PARITY
+  LaunchTimer t(ctx, K_CAMERA_MERGE_SERIAL);
+  k_camera_merge_serial<SP><<<blocks_for(active, 128), 128, 0, ctx->stream>>>(p, q, count);
+  ctx->branch_counts.merge_launches[0] += 1;
+#else
+  if (!ctx->grid.photon_count) return ETXB_OK;
+  const etxb_debug_thresholds& th = ctx->thresholds;
+  const uint32_t* ids = q;
+  const uint32_t* keys = ctx->merge_key.ptr;
+  if (active >= th.merge_sort_min_queries) {
+    // queries sorted by the Morton code of their base cell: neighbours in the queue read the same photon cells.  A short queue
+    // (the tail of the pass) is latency bound, not bandwidth bound: it goes in queue order and saves the sort launches.
+    LaunchTimer t(ctx, K_CAMERA_MERGE_SORT);
+    size_t temp_bytes = ctx->cub_temp.bytes();
+    CUDA_OK(ctx, cub::DeviceRadixSort::SortPairs(ctx->cub_temp.ptr, temp_bytes, ctx->merge_key.ptr, ctx->keys_out.ptr, q, ctx->vals_out.ptr, int(active), 0, 32,
+                   ctx->stream));
+    ids = ctx->vals_out.ptr;
+    keys = ctx->keys_out.ptr;
+    ctx->branch_counts.merge_sorts += 1;
+  }
+  // queries per warp: 32 while that still fills the machine, fewer for short queues (a warp serialises its queries)
+  uint32_t qpw = 32u;
+  while ((qpw > 1u) && (uint64_t(active / qpw) < uint64_t(th.merge_min_warps_per_sm) * ctx->sm_count)) qpw >>= 1;
+  if (th.merge_qpw) qpw = th.merge_qpw;
+  const uint32_t merge_blocks = blocks_for(blocks_for(active, qpw), kMergeWarpsPerBlock);
+  {
+    LaunchTimer t(ctx, K_CAMERA_MERGE);
+    k_camera_merge_coop<SP><<<merge_blocks, kMergeWarpsPerBlock * 32, 0, ctx->stream>>>(p, ids, keys, count, qpw);
+  }
+  if (ctx->has_stochastic_merge) {
+    LaunchTimer t(ctx, K_CAMERA_MERGE_SERIAL);
+    const uint32_t closure_blocks = blocks_for(blocks_for(active, qpw), kClosureWarpsPerBlock);
+    k_camera_merge_closure<SP><<<closure_blocks, kClosureWarpsPerBlock * 32, 0, ctx->stream>>>(p, ids, keys, count, qpw);
+  }
+  ctx->branch_counts.merge_launches[__builtin_ctz(qpw)] += 1;
+#endif
+  return ETXB_OK;
+}
+
 template <bool SP>
 int run_camera_pass(etxb_ctx* ctx) {
   LaunchParams p = make_params(ctx);
@@ -696,7 +748,7 @@ int run_camera_pass(etxb_ctx* ctx) {
     }
 #if !(defined(ETXB_PARITY) && ETXB_PARITY)  // make_params: the parity build has no connection stage
     if (p.connect_stage && (ctx->options.options & ETXB_VCM_CONNECT_VERTICES)) {
-      if (active < kTailQueue) {
+      if (active < ctx->thresholds.tail_queue) {
         // tail of the pass: the pair count stays on the device (k_camera_connect is grid-stride), no host round trip per bounce
         LaunchTimer t(ctx, K_CAMERA_CONNECT);
         const uint32_t blocks = std::min<uint32_t>(ctx->sm_count * 4u, blocks_for(active * 4u, 128));
@@ -711,14 +763,16 @@ int run_camera_pass(etxb_ctx* ctx) {
         pending = std::min(pending, ctx->lv_capacity);
         if (pending) {
           const uint2* list = ctx->conn_list.ptr;
-          if (p.conn_key && (pending >= kSortQueueMin)) {
+          if (p.conn_key && (pending >= ctx->thresholds.sort_queue_min)) {
             // connections grouped by (camera vertex material, light vertex material): one pair of BSDF classes per warp
             LaunchTimer t(ctx, K_QUEUE_SORT);
             size_t temp_bytes = ctx->cub_temp.bytes();
             CUDA_OK(ctx, cub::DeviceRadixSort::SortPairs(ctx->cub_temp.ptr, temp_bytes, ctx->keys_in.ptr, ctx->vals_in.ptr, reinterpret_cast<const unsigned long long*>(ctx->conn_list.ptr),
                            reinterpret_cast<unsigned long long*>(ctx->conn_list_sorted.ptr), int(pending), 0, 16, ctx->stream));
             list = ctx->conn_list_sorted.ptr;
+            ctx->branch_counts.pair_sorts += 1;
           }
+          ctx->branch_counts.connect_launches += 1;
           LaunchTimer t(ctx, K_CAMERA_CONNECT);
           if (ctx->plain_scene) {
             k_camera_connect<SP, true><<<blocks_for(pending, 128), 128, 0, ctx->stream>>>(p, list);
@@ -734,40 +788,9 @@ int run_camera_pass(etxb_ctx* ctx) {
       LaunchTimer t(ctx, K_SHADOW_TRACE);
       if (int rc = launch_shadow_resolve(ctx, p, active)) return rc;
     }
-#if defined(ETXB_PARITY) && ETXB_PARITY
     if (merging) {
-      LaunchTimer t(ctx, K_CAMERA_MERGE_SERIAL);
-      k_camera_merge_serial<SP><<<blocks_for(active, 128), 128, 0, ctx->stream>>>(p, q, counts + cur);
+      if (int rc = launch_merge<SP>(ctx, p, q, counts + cur, active)) return rc;
     }
-#else
-    if (merging && ctx->grid.photon_count) {
-      const uint32_t* ids = q;
-      const uint32_t* keys = ctx->merge_key.ptr;
-      if (active >= kMergeSortMinQueries) {
-        // queries sorted by the Morton code of their base cell: neighbours in the queue read the same photon cells.  A short queue
-        // (the tail of the pass) is latency bound, not bandwidth bound: it goes in queue order and saves the sort launches.
-        LaunchTimer t(ctx, K_CAMERA_MERGE_SORT);
-        size_t temp_bytes = ctx->cub_temp.bytes();
-        CUDA_OK(ctx, cub::DeviceRadixSort::SortPairs(ctx->cub_temp.ptr, temp_bytes, ctx->merge_key.ptr, ctx->keys_out.ptr, q, ctx->vals_out.ptr, int(active), 0, 32,
-                       ctx->stream));
-        ids = ctx->vals_out.ptr;
-        keys = ctx->keys_out.ptr;
-      }
-      // queries per warp: 32 while that still fills the machine, fewer for short queues (a warp serialises its queries)
-      uint32_t qpw = 32u;
-      while ((qpw > 1u) && (active / qpw < kMergeMinWarpsPerSm * ctx->sm_count)) qpw >>= 1;
-      const uint32_t merge_blocks = blocks_for(blocks_for(active, qpw), kMergeWarpsPerBlock);
-      {
-        LaunchTimer t(ctx, K_CAMERA_MERGE);
-        k_camera_merge_coop<SP><<<merge_blocks, kMergeWarpsPerBlock * 32, 0, ctx->stream>>>(p, ids, keys, counts + cur, qpw);
-      }
-      if (ctx->has_stochastic_merge) {
-        LaunchTimer t(ctx, K_CAMERA_MERGE_SERIAL);
-        const uint32_t closure_blocks = blocks_for(blocks_for(active, qpw), kClosureWarpsPerBlock);
-        k_camera_merge_closure<SP><<<closure_blocks, kClosureWarpsPerBlock * 32, 0, ctx->stream>>>(p, ids, keys, counts + cur, qpw);
-      }
-    }
-#endif
     {
       LaunchTimer t(ctx, K_CAMERA_CONTINUE);
       k_camera_continue<SP><<<blocks_for(active, 128), 128, 0, ctx->stream>>>(p, q, counts + cur, qout, counts + (cur ^ 1u));
@@ -1804,6 +1827,7 @@ int etxb_begin(etxb_ctx* ctx, uint32_t first_iteration) {
   ctx->last_iteration_time = 0.0;
   ctx->overflow_flag = 0;
   ctx->kernel_launches = 0;
+  ctx->branch_counts = {};
   ctx->light_pass_done = ctx->grid_done = false;
   memset(ctx->kernel_ms, 0, sizeof(ctx->kernel_ms));
   memset(ctx->kernel_count, 0, sizeof(ctx->kernel_count));
@@ -2395,6 +2419,102 @@ int etxb_debug_closure_eval(etxb_ctx* ctx, const etxb_closure_query* queries, ui
   CUDA_OK(ctx, cudaMemcpy(out, d_out.ptr, d_out.bytes(), cudaMemcpyDeviceToHost));
   d_queries.release();
   d_out.release();
+  return ETXB_OK;
+}
+
+// Test hook: the queue sizes from which the passes take their large-queue branches (NULL = the defaults), and what ran since etxb_begin
+int etxb_debug_set_thresholds(etxb_ctx* ctx, const etxb_debug_thresholds* thresholds) {
+  if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;
+  const etxb_debug_thresholds t = thresholds ? *thresholds : kDefaultThresholds;
+  if ((t.merge_qpw > 32u) || (t.merge_qpw & (t.merge_qpw - 1u))) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "merge_qpw must be 0, 1, 2, 4, 8, 16 or 32");
+  if (t.merge_sort_min_queries < t.tail_queue) {
+    // below tail_queue the host enqueues bounces on a stale queue size, and the gather's sort would take in slots past the count
+    return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "merge_sort_min_queries (%u) must not be below tail_queue (%u)", t.merge_sort_min_queries, t.tail_queue);
+  }
+  ctx_drain_impl(ctx);
+  ctx->thresholds = t;
+  return ETXB_OK;
+}
+
+int etxb_debug_get_branch_counts(etxb_ctx* ctx, etxb_debug_branch_counts* out) {
+  if (!ctx || !out) return ETXB_ERR_INVALID_ARGUMENT;
+  if (int rc = ctx_drain_impl(ctx)) return rc;
+  *out = ctx->branch_counts;
+  return ETXB_OK;
+}
+
+extern "C++" {
+namespace {
+template <bool SP>
+int debug_merge(etxb_ctx* ctx, uint32_t record_count, const etxb_merge_query* d_queries, uint32_t count, float4* d_pos_nrm) {
+  if (int rc = run_grid_build<SP>(ctx, ctx->lv_final.ptr, record_count)) return rc;
+  LaunchParams p = make_params(ctx);
+  if (count) k_debug_merge_stage<SP><<<blocks_for(count, 128), 128, 0, ctx->stream>>>(p, d_queries, count, ctx->queue_a.ptr, d_pos_nrm);
+  ctx->kernel_launches += 1;
+  CUDA_OK(ctx, cudaMemcpyAsync(ctx->queue_counts.ptr, &count, 4, cudaMemcpyHostToDevice, ctx->stream));
+  if (count == 0) return ETXB_OK;
+  return launch_merge<SP>(ctx, p, ctx->queue_a.ptr, ctx->queue_counts.ptr, count);
+}
+}  // namespace
+}  // extern "C++"
+
+// Test hook: the photon gather query by query (layout and outputs in include/etx_b200.h)
+int etxb_debug_merge(etxb_ctx* ctx, const void* records, uint32_t record_count, const float* light_wavelengths, const etxb_merge_query* queries, uint32_t count,
+                     etxb_merge_result* out, etxb_merge_grid* grid) {
+  if (!ctx || (record_count && !records) || !light_wavelengths || (count && (!queries || !out)) || !grid) return ETXB_ERR_INVALID_ARGUMENT;
+  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
+  if (count > ctx->path_count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "%u merge queries exceed the %u paths of the context", count, ctx->path_count);
+  if (record_count > ctx->lv_capacity) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "%u light vertices exceed the pool capacity %u", record_count, ctx->lv_capacity);
+  const LightVertexRec* recs = static_cast<const LightVertexRec*>(records);
+  for (uint32_t k = 0; k < record_count; ++k) {
+    if (recs[k].ids.z >= ctx->path_count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "light vertex %u: path index out of range", k);
+  }
+  for (uint32_t k = 0; k < count; ++k) {
+    if (queries[k].tri >= ctx->triangles.count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "merge query %u: triangle index out of range", k);
+    if ((queries[k].medium != ETXB_INVALID_INDEX) && (queries[k].medium >= ctx->dscene.medium_count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "merge query %u: medium index out of range", k);
+  }
+  if (int rc = ctx_drain_impl(ctx)) return rc;
+  cudaSetDevice(ctx->device);
+  if (record_count) CUDA_OK(ctx, cudaMemcpyAsync(ctx->lv_final.ptr, records, size_t(record_count) * sizeof(LightVertexRec), cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_OK(ctx, cudaMemcpyAsync(ctx->wavelength.ptr, light_wavelengths, size_t(ctx->path_count) * 4u, cudaMemcpyHostToDevice, ctx->stream));
+  DeviceCounters before = {}, after = {};
+  CUDA_OK(ctx, cudaMemcpyAsync(&before, ctx->counters.ptr, sizeof(before), cudaMemcpyDeviceToHost, ctx->stream));
+  DevBuf<etxb_merge_query> d_queries;
+  DevBuf<float4> d_pos_nrm;
+  CUDA_OK(ctx, d_queries.alloc(std::max<uint32_t>(count, 1u)));
+  CUDA_OK(ctx, d_pos_nrm.alloc(2u * std::max<uint32_t>(count, 1u)));
+  if (count) CUDA_OK(ctx, cudaMemcpyAsync(d_queries.ptr, queries, size_t(count) * sizeof(etxb_merge_query), cudaMemcpyHostToDevice, ctx->stream));
+  int rc = ctx->spectral ? debug_merge<true>(ctx, record_count, d_queries.ptr, count, d_pos_nrm.ptr) : debug_merge<false>(ctx, record_count, d_queries.ptr, count, d_pos_nrm.ptr);
+  if (rc) return rc;
+  CUDA_OK(ctx, cudaGetLastError());
+  std::vector<float4> merged(count), pos_nrm(2u * size_t(count));
+  std::vector<uint4> misc(count);
+  if (count) {
+    CUDA_OK(ctx, cudaMemcpyAsync(merged.data(), ctx->merged.ptr, size_t(count) * 16u, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(misc.data(), ctx->misc.ptr, size_t(count) * 16u, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(pos_nrm.data(), d_pos_nrm.ptr, size_t(count) * 32u, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  CUDA_OK(ctx, cudaMemcpyAsync(&after, ctx->counters.ptr, sizeof(after), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+  for (uint32_t k = 0; k < count; ++k) {
+    etxb_merge_result& r = out[k];
+    r = {};
+    r.merged[0] = merged[k].x, r.merged[1] = merged[k].y, r.merged[2] = merged[k].z;
+    r.seed = misc[k].x;
+    r.pos[0] = pos_nrm[2 * k].x, r.pos[1] = pos_nrm[2 * k].y, r.pos[2] = pos_nrm[2 * k].z;
+    r.nrm[0] = pos_nrm[2 * k + 1].x, r.nrm[1] = pos_nrm[2 * k + 1].y, r.nrm[2] = pos_nrm[2 * k + 1].z;
+  }
+  const GridData& g = ctx->grid;
+  *grid = {};
+  grid->bbox_min[0] = g.bbox_min.x, grid->bbox_min[1] = g.bbox_min.y, grid->bbox_min[2] = g.bbox_min.z;
+  grid->bbox_max[0] = g.bbox_max.x, grid->bbox_max[1] = g.bbox_max.y, grid->bbox_max[2] = g.bbox_max.z;
+  grid->cell_size = g.cell_size;
+  grid->radius_squared = g.radius_squared;
+  grid->hash_table_mask = g.hash_table_mask;
+  grid->photon_count = g.photon_count;
+  grid->merge_queries = after.merge_queries - before.merge_queries;
+  grid->merge_candidates = after.merge_candidates - before.merge_candidates;
+  grid->merge_accepts = after.merge_accepts - before.merge_accepts;
   return ETXB_OK;
 }
 

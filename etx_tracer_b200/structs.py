@@ -112,6 +112,20 @@ CLOSURE_QUERY = np.dtype([
     ("material", u4), ("path_source", u4), ("seed", u4), ("reserved", u4, 3),
 ])
 CLOSURE_STATS = 32
+# etxb_debug_thresholds / etxb_debug_branch_counts (include/etx_b200.h): a threshold of 0 always takes the large-queue branch, NEVER never does
+DEBUG_THRESHOLDS = np.dtype([("merge_sort_min_queries", u4), ("merge_min_warps_per_sm", u4), ("tail_queue", u4), ("sort_queue_min", u4), ("merge_qpw", u4)])
+DEFAULT_THRESHOLDS = {"merge_sort_min_queries": 16384, "merge_min_warps_per_sm": 32, "tail_queue": 8192, "sort_queue_min": 1024, "merge_qpw": 0}
+NEVER = INVALID
+MERGE_QPW = (1, 2, 4, 8, 16, 32)
+DEBUG_BRANCH_COUNTS = np.dtype([("merge_sorts", u8), ("merge_launches", u8, 6), ("connect_launches", u8), ("pair_sorts", u8), ("queue_sorts", u8)])
+# the device's light-vertex record (dvcm.cuh LightVertexRec, BUF_PHOTON_RECORDS), etxb_merge_query / etxb_merge_result / etxb_merge_grid (etxb_debug_merge)
+LIGHT_VERTEX_REC = np.dtype([("throughput", f4, 3), ("d_vcm", f4), ("w_i", f4, 3), ("d_vc", f4), ("bc", f4, 3), ("d_vm", f4), ("pos", f4, 3), ("tri", u4),
+                             ("nrm", f4, 3), ("material", u4), ("medium", u4), ("path_length", u4), ("path_index", u4), ("ordinal", u4)])
+MERGE_QUERY = np.dtype([("tri", u4), ("u", f4), ("v", f4), ("w_i", f4, 3), ("throughput", f4, 3), ("wavelength", f4), ("d_vcm", f4), ("d_vm", f4),
+                        ("total_path_depth", u4), ("seed", u4), ("medium", u4), ("reserved", u4)])
+MERGE_RESULT = np.dtype([("merged", f4, 3), ("seed", u4), ("pos", f4, 3), ("nrm", f4, 3), ("reserved", u4, 2)])
+MERGE_GRID = np.dtype([("bbox_min", f4, 3), ("bbox_max", f4, 3), ("cell_size", f4), ("radius_squared", f4), ("hash_table_mask", u4), ("photon_count", u4),
+                       ("merge_queries", u8), ("merge_candidates", u8), ("merge_accepts", u8)])
 CLOSURE_OUTPUTS = ("func_r", "func_g", "func_b", "bsdf_r", "bsdf_g", "bsdf_b", "pdf", "rev_pdf")
 PATH_CAMERA, PATH_LIGHT = 1, 2
 
@@ -119,6 +133,7 @@ EXPECTED_SIZES = {
     "VERTEX": (VERTEX, 56), "TRIANGLE": (TRIANGLE, 32), "MATERIAL": (MATERIAL, 200), "EMITTER_PROFILE": (EMITTER_PROFILE, 48),
     "EMITTER": (EMITTER, 32), "SPECTRUM": (SPECTRUM, 3552), "DISTRIBUTION": (DISTRIBUTION, 32), "IMAGE": (IMAGE, 112),
     "MEDIUM": (MEDIUM, 80), "CAMERA": (CAMERA, 176), "SCENE": (SCENE, 528), "CLOSURE_QUERY": (CLOSURE_QUERY, 96),
+    "LIGHT_VERTEX_REC": (LIGHT_VERTEX_REC, 96), "MERGE_QUERY": (MERGE_QUERY, 64), "MERGE_RESULT": (MERGE_RESULT, 48), "MERGE_GRID": (MERGE_GRID, 64),
 }
 for _name, (_dt, _size) in EXPECTED_SIZES.items():
     assert _dt.itemsize == _size, f"{_name}: {_dt.itemsize} != {_size}"

@@ -510,6 +510,60 @@ typedef struct etxb_closure_query {
  * [24] the number of repetitions with a non-finite output, [25] with pdf < 0 or rev_pdf < 0, [26] with pdf == 0 but a non-zero func or bsdf. */
 #define ETXB_CLOSURE_STATS 32
 int etxb_debug_closure_eval(etxb_ctx* ctx, const etxb_closure_query* queries, uint32_t count, uint32_t repetitions, double* out);
+/* Queue sizes from which the light and camera passes take their large-queue branches.  A pass of a long queue runs the same paths as
+ * one of a short queue, in another order; these let a small film take either branch.  Each field is a queue size: 0 = always the
+ * large-queue branch, 0xffffffff = never.
+ *   merge_sort_min_queries  the gather queue is sorted by its merge keys (default 16384); must not be below tail_queue
+ *   merge_min_warps_per_sm  the gather gives a warp 32 queries, halved while the queue fills fewer than this many warps per SM (default 32)
+ *   tail_queue              from this size the vertex connections run over the host-sized pair list and the queue size is read back every
+ *                           bounce; below it, every 4 bounces (default 8192)
+ *   sort_queue_min          scenes with stochastic BSDFs: path queues and connection pair lists are sorted by material (default 1024)
+ *   merge_qpw               queries per warp of the gather, 1, 2, 4, ..., 32; 0 = chosen from merge_min_warps_per_sm (default 0)
+ * NULL restores the defaults; the setting stays until the next call. */
+typedef struct etxb_debug_thresholds {
+  uint32_t merge_sort_min_queries, merge_min_warps_per_sm, tail_queue, sort_queue_min, merge_qpw;
+} etxb_debug_thresholds;
+int etxb_debug_set_thresholds(etxb_ctx* ctx, const etxb_debug_thresholds* thresholds);
+/* Host-side counts since the last etxb_begin of the branches above: gather-queue sorts, gather launches by queries per warp
+ * (index k = 2^k queries; the parity build's serial gather counts as 1), vertex-connection launches over the host-sized pair list,
+ * pair-list sorts and path-queue sorts. */
+typedef struct etxb_debug_branch_counts {
+  uint64_t merge_sorts;
+  uint64_t merge_launches[6];
+  uint64_t connect_launches, pair_sorts, queue_sorts;
+} etxb_debug_branch_counts;
+int etxb_debug_get_branch_counts(etxb_ctx* ctx, etxb_debug_branch_counts* out);
+/* The photon gather (VCMSpatialGridData::gather, vcm_shared.hxx:805-925), query by query, through the launch code of the camera pass.
+ * `records` = `record_count` light-vertex records of the device layout (96 B each: {throughput.xyz, d_vcm}, {w_i, d_vc}, {barycentric, d_vm},
+ * {pos, triangle}, {nrm, material}, {medium, path_length, path_index, ordinal}); `light_wavelengths` = one wavelength per light path index
+ * (path_count of them; ignored in RGB scenes).  The photon grid is built from them at the context's current iteration and options, then
+ * each query becomes one camera vertex of a one-bounce queue (at most path_count queries) with the merge key the camera pass gives it, and the
+ * gather runs under the current etxb_debug_set_thresholds: the parity build's serial gather; the product build's Lambert and closure gathers.
+ * The context's path state, photon grid and light image change; call etxb_begin before rendering again. */
+typedef struct etxb_merge_query {
+  uint32_t tri;                       /* the hit: triangle and the barycentrics (u, v) etxb_debug_trace returns */
+  float u, v;
+  float w_i[3];                       /* the direction the camera path arrived along (pointing AT the surface) */
+  float throughput[3];
+  float wavelength;                   /* ignored in RGB scenes */
+  float d_vcm, d_vm;
+  uint32_t total_path_depth, seed, medium;
+  uint32_t reserved;
+} etxb_merge_query;
+typedef struct etxb_merge_result {
+  float merged[3];                    /* what the gather added to VCMPathState::merged */
+  uint32_t seed;                      /* the path's sampler state afterwards */
+  float pos[3], nrm[3];               /* the staged camera vertex */
+  uint32_t reserved[2];
+} etxb_merge_result;
+typedef struct etxb_merge_grid {
+  float bbox_min[3], bbox_max[3];     /* the photon grid the queries were gathered on */
+  float cell_size, radius_squared;
+  uint32_t hash_table_mask, photon_count;
+  uint64_t merge_queries, merge_candidates, merge_accepts;  /* the gather's counters for this call */
+} etxb_merge_grid;
+int etxb_debug_merge(etxb_ctx* ctx, const void* records, uint32_t record_count, const float* light_wavelengths, const etxb_merge_query* queries, uint32_t count,
+                     etxb_merge_result* out, etxb_merge_grid* grid);
 
 /* ---- several iterations in flight on one device -----------------------------------------------------------------------
  * The reference runs ONE iteration at a time and spreads its paths over the CPU's threads (vcm_cpu.cxx:115-171, TaskScheduler).

@@ -46,6 +46,8 @@ def load(flavor="parity"):
     lib.oracle_bvh_info.argtypes = [vp, C.POINTER(u32), C.POINTER(u32)]
     if hasattr(lib, "oracle_bsdf_eval"):  # an oracle/_ref built before this export still serves every other test
         lib.oracle_bsdf_eval.argtypes = [vp, vp, u32, u32, u32, vp]
+    if hasattr(lib, "oracle_merge"):
+        lib.oracle_merge.argtypes = [vp, vp, u32, vp, vp, u32, u32, u32, vp, vp]
     lib.oracle_sampler.argtypes = [vp, vp, u32, u32, vp, vp]
     lib.oracle_math.argtypes = [u32, vp, vp, u32, vp]
     lib.oracle_offset_ray.argtypes = [vp, vp, vp]
@@ -70,6 +72,11 @@ def load(flavor="parity"):
 def has_bsdf_eval(flavor="parity"):
     """Whether the built oracle exports oracle_bsdf_eval (oracle/_ref is older than the export where the reference could not rebuild it)."""
     return hasattr(load(flavor), "oracle_bsdf_eval")
+
+
+def has_merge(flavor="parity"):
+    """Whether the built oracle exports oracle_merge."""
+    return hasattr(load(flavor), "oracle_merge")
 
 
 def _p(a):
@@ -243,6 +250,22 @@ class Oracle:
         out = np.zeros((queries.shape[0], self.S.CLOSURE_STATS), dtype=np.float64)
         self.lib.oracle_bsdf_eval(self.h, _p(queries), queries.shape[0], int(repetitions), int(threads or os.cpu_count() or 1), _p(out))
         return out
+
+    def merge(self, records, light_wavelengths, queries, repetitions=1, threads=None):
+        """The reference's VCMSpatialGridData::gather for etxb_debug_merge's inputs (S.LIGHT_VERTEX_REC records, a wavelength per light path index,
+        S.MERGE_QUERY records) at the current options and iteration, `repetitions` samplers Sampler(seed, r) per query.  Returns float64 (n, 8):
+        mean rgb, variance rgb, the sampler state after repetition 0, 0; and the grid as a dict like GPUVCM.debug_merge's."""
+        records = np.ascontiguousarray(records, dtype=self.S.LIGHT_VERTEX_REC)
+        wl = np.zeros(self.width * self.height, dtype=np.float32)
+        wl[:len(light_wavelengths)] = light_wavelengths
+        queries = np.ascontiguousarray(queries, dtype=self.S.MERGE_QUERY)
+        out = np.zeros((queries.shape[0], 8), dtype=np.float64)
+        g = np.zeros(10, dtype=np.float64)
+        self.lib.oracle_merge(self.h, _p(records), records.shape[0], _p(wl), _p(queries), queries.shape[0], int(repetitions), int(threads or os.cpu_count() or 1),
+                              _p(out), _p(g))
+        grid = {"bbox_min": g[0:3].astype(np.float32), "bbox_max": g[3:6].astype(np.float32), "cell_size": float(g[6]), "radius_squared": float(g[7]),
+                "hash_table_mask": int(g[8]), "photon_count": int(g[9])}
+        return out, grid
 
     def bvh_info(self):
         a, b = C.c_uint32(0), C.c_uint32(0)

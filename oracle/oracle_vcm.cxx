@@ -541,6 +541,22 @@ void parallel_ranges(uint32_t count, uint32_t threads, F&& fn) {
     th.join();
 }
 
+// start_next_iteration (vcm_cpu.cxx:95-124): merge radius and MIS weights of the iteration
+void start_next_iteration(Oracle& o) {
+  auto& it = o.iteration;
+  float used_radius = o.options.initial_radius;
+  if (used_radius == 0.0f) {
+    uint32_t max_dim = max(o.width, o.height);
+    used_radius = 5.0f * o.scene.bounding_sphere_radius / float(max_dim);
+  }
+  float radius_scale = 1.0f / (1.0f + float(it.iteration) / float(o.options.radius_decay));
+  it.current_radius = used_radius * radius_scale;
+  float eta_vcm = kPi * sqr(it.current_radius) * float(o.pixel_count());
+  it.vc_weight = 1.0f / eta_vcm;
+  it.vm_weight = o.options.enable_merging() ? eta_vcm : 0.0f;
+  it.vm_normalization = 1.0f / eta_vcm;
+}
+
 // vcm_cpu.cxx:95-241, one full iteration (light pass, grid build, camera pass)
 void run_iteration(Oracle& o, uint32_t threads) {
   auto t0 = std::chrono::steady_clock::now();
@@ -549,18 +565,7 @@ void run_iteration(Oracle& o, uint32_t threads) {
   auto& it = o.iteration;
   const uint32_t pixel_count = o.pixel_count();
 
-  // start_next_iteration (:95-124)
-  float used_radius = o.options.initial_radius;
-  if (used_radius == 0.0f) {
-    uint32_t max_dim = max(o.width, o.height);
-    used_radius = 5.0f * scene.bounding_sphere_radius / float(max_dim);
-  }
-  float radius_scale = 1.0f / (1.0f + float(it.iteration) / float(o.options.radius_decay));
-  it.current_radius = used_radius * radius_scale;
-  float eta_vcm = kPi * sqr(it.current_radius) * float(pixel_count);
-  it.vc_weight = 1.0f / eta_vcm;
-  it.vm_weight = o.options.enable_merging() ? eta_vcm : 0.0f;
-  it.vm_normalization = 1.0f / eta_vcm;
+  start_next_iteration(o);
 
   o.light_paths.assign(pixel_count, VCMLightPath{});
   o.light_vertices.clear();
@@ -1106,6 +1111,94 @@ void oracle_bsdf_eval(void* h, const etxb_closure_query* queries, uint32_t count
       dst[26] = double(unsupported);
       for (uint32_t k = 27; k < ETXB_CLOSURE_STATS; ++k)
         dst[k] = 0.0;
+    }
+  });
+}
+
+// The reference's own photon gather (VCMSpatialGridData::gather, vcm_shared.hxx:886-924) for etxb_debug_merge's inputs: the light-vertex
+// records (device layout, 96 B) become o.light_vertices and build_grid runs on them at the current iteration; each query becomes the
+// Intersection make_intersection builds for its hit (as oracle_trace does) and a VCMPathState, and is gathered `repetitions` times on
+// Sampler(seed, r).  out = double[8] per query: the mean and the (population) variance of the merged rgb over the repetitions, the sampler
+// state after repetition 0, 0.  grid_out = bbox min, bbox max, cell size, radius squared, hash table mask, photon count.
+struct MergeRecord {
+  float thr[3], d_vcm, w_i[3], d_vc, bc[3], d_vm, pos[3];
+  uint32_t tri;
+  float nrm[3];
+  uint32_t material, medium, path_length, path_index, ordinal;
+};
+static_assert(sizeof(MergeRecord) == 96);
+static_assert(sizeof(etxb_merge_query) == 64);
+void oracle_merge(void* h, const void* records, uint32_t record_count, const float* light_wavelengths, const etxb_merge_query* queries, uint32_t count,
+                  uint32_t repetitions, uint32_t threads, double* out, double* grid_out) {
+  auto* o = static_cast<Oracle*>(h);
+  const Scene& scene = o->scene;
+  const bool spectral = scene.spectral();
+  auto response = [spectral](float wavelength, const float* v) {
+    return spectral ? SpectralResponse{SpectralQuery{wavelength, SpectralQuery::Spectral}, v[0]} : SpectralResponse{SpectralQuery::sample(), float3{v[0], v[1], v[2]}};
+  };
+  start_next_iteration(*o);
+  o->light_vertices.assign(record_count, VCMLightVertex{});
+  const auto* recs = static_cast<const MergeRecord*>(records);
+  for (uint32_t k = 0; k < record_count; ++k) {
+    const MergeRecord& r = recs[k];
+    VCMLightVertex& v = o->light_vertices[k];
+    v.throughput = response(light_wavelengths[r.path_index], r.thr);
+    v.w_i = {r.w_i[0], r.w_i[1], r.w_i[2]};
+    v.d_vcm = r.d_vcm;
+    v.bc = {r.bc[0], r.bc[1], r.bc[2]};
+    v.d_vc = r.d_vc;
+    v.pos = {r.pos[0], r.pos[1], r.pos[2]};
+    v.d_vm = r.d_vm;
+    v.nrm = {r.nrm[0], r.nrm[1], r.nrm[2]};
+    v.triangle_index = r.tri;
+    v.material_index = r.material;
+    v.medium_index = r.medium;
+    v.is_medium = (r.tri == kInvalidIndex);
+    v.path_length = r.path_length;
+    v.path_index = r.path_index;
+  }
+  if (o->options.merge_vertices()) {
+    build_grid(*o);
+  } else {
+    o->grid = {};
+  }
+  const VCMSpatialGridData& grid = o->grid;
+  const double g[10] = {grid.bounding_box.p_min.x, grid.bounding_box.p_min.y, grid.bounding_box.p_min.z, grid.bounding_box.p_max.x, grid.bounding_box.p_max.y,
+    grid.bounding_box.p_max.z, grid.cell_size, grid.radius_squared, double(grid.hash_table_mask), double(grid.positions.count)};
+  for (uint32_t k = 0; k < 10; ++k)
+    grid_out[k] = g[k];
+  parallel_ranges(count, threads, [&](uint32_t begin, uint32_t end, uint32_t, uint32_t) {
+    for (uint32_t i = begin; i < end; ++i) {
+      const etxb_merge_query& q = queries[i];
+      const float3 w_i = {q.w_i[0], q.w_i[1], q.w_i[2]};
+      const Intersection isect = make_intersection(scene, w_i, IntersectionBase{{q.u, q.v}, q.tri, 0.0f});
+      double mean[3] = {}, m2[3] = {};
+      double* dst = out + size_t(i) * 8u;
+      for (uint32_t r = 0; r < repetitions; ++r) {
+        VCMPathState state = {};
+        state.throughput = response(q.wavelength, q.throughput);
+        state.spect = state.throughput;
+        state.ray.d = w_i;
+        state.d_vcm = q.d_vcm;
+        state.d_vm = q.d_vm;
+        state.total_path_depth = q.total_path_depth;
+        state.medium_index = q.medium;
+        state.sampler = Sampler(q.seed, r);
+        const float3 m = grid.gather(scene, state, o->options, isect, o->iteration.vc_weight);
+        const double v[3] = {m.x, m.y, m.z};
+        for (uint32_t k = 0; k < 3; ++k) {
+          const double delta = v[k] - mean[k];
+          mean[k] += delta / double(r + 1u);
+          m2[k] += delta * (v[k] - mean[k]);
+        }
+        if (r == 0)
+          dst[6] = double(state.sampler.seed);
+      }
+      for (uint32_t k = 0; k < 3; ++k) {
+        dst[k] = mean[k];
+        dst[3 + k] = m2[k] / double(std::max(repetitions, 1u));
+      }
+      dst[7] = 0.0;
     }
   });
 }
