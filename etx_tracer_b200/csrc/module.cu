@@ -17,6 +17,7 @@
 #include <ctime>
 #include <deque>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include <dlfcn.h>
@@ -76,10 +77,24 @@ const char* kKernelNames[K_COUNT] = {"light_begin", "trace_closest(light)", "lig
 //   sort_queue_min          path queues and connection lists are grouped by material (scenes with stochastic BSDFs)
 constexpr etxb_debug_thresholds kDefaultThresholds = {16384u, 32u, 8192u, 1024u, 0u};
 
+// A device allocation with one owner: it is freed when the buffer is destroyed, on the device that is current then.
 template <class T>
 struct DevBuf {
   T* ptr = nullptr;
   size_t count = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  DevBuf(DevBuf&& o) noexcept : ptr(std::exchange(o.ptr, nullptr)), count(std::exchange(o.count, size_t(0))) {}
+  DevBuf& operator=(DevBuf&& o) noexcept {
+    if (this != &o) {
+      release();
+      ptr = std::exchange(o.ptr, nullptr);
+      count = std::exchange(o.count, size_t(0));
+    }
+    return *this;
+  }
+  ~DevBuf() { release(); }
   cudaError_t alloc(size_t n) {
     release();
     count = n;
@@ -262,6 +277,102 @@ struct etxb_ctx {
   size_t event_cursor = 0;
   float kernel_ms[K_COUNT] = {};
   uint32_t kernel_count[K_COUNT] = {};
+
+  // frees the device buffers; a C++ symbol, kept out of the library's exports (the interface is etxb_destroy)
+  __attribute__((visibility("hidden"))) ~etxb_ctx() = default;
+};
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Iterations in flight (etxb_group): L contexts on one device, one host thread each, pulling iteration indices from a shared
+// counter.  VCM iterations are independent (vcm_cpu.cxx:95-113: the index only sets the merge radius and the sampler seeds), and
+// the bounce loop of one iteration ends in a long latency-bound tail (a few thousand paths, ~50 bounces); with several iterations in
+// flight that tail overlaps the full-width head of another iteration.  The film is the mean of the lanes' films weighted by the
+// iterations each lane finished — the same set of iterations, hence the same estimate, as one context running them in sequence.
+// ---------------------------------------------------------------------------------------------------------------------
+extern "C" {  // the film-combine kernels keep unmangled names in the module
+constexpr uint32_t kMaxLanes = 9;  // 8 whole-iteration lanes + the camera-split lane of the replica mode
+struct FilmLanes {
+  const float4* camera[kMaxLanes];
+  const float4* light[kMaxLanes];
+  float weight[kMaxLanes];        // camera layer
+  float weight_light[kMaxLanes];  // light layer (differs from `weight` only for a camera-split lane that is not part 0)
+  float weight_count[kMaxLanes];  // raw mode: what the lane adds to .w
+  uint32_t lanes, layer, pixels;
+  uint32_t raw;  // 1: no clamp, alpha = sum of the weights (a partial sum that another stage finishes)
+};
+__global__ void __launch_bounds__(256) k_film_combine(FilmLanes f, float4* out) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= f.pixels) return;
+  float x = 0.0f, y = 0.0f, z = 0.0f;
+  for (uint32_t l = 0; l < f.lanes; ++l) {
+    float4 c = (f.layer != ETXB_FILM_LIGHT) ? f.camera[l][i] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    float4 g = (f.layer != ETXB_FILM_CAMERA) ? f.light[l][i] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    x += f.weight[l] * c.x + f.weight_light[l] * g.x;
+    y += f.weight[l] * c.y + f.weight_light[l] * g.y;
+    z += f.weight[l] * c.z + f.weight_light[l] * g.z;
+  }
+  if (f.raw) {
+    float w = 0.0f;
+    for (uint32_t l = 0; l < f.lanes; ++l) w += f.weight_count[l];
+    out[i] = make_float4(x, y, z, w);
+    return;
+  }
+  if (f.layer == ETXB_FILM_RESULT) {  // Film::layer(Result): max(0, camera + light) (film.cxx:381-418)
+    x = fmaxf(0.0f, x);
+    y = fmaxf(0.0f, y);
+    z = fmaxf(0.0f, z);
+  }
+  out[i] = make_float4(x, y, z, 1.0f);
+}
+// rank 0 of a replica run: the reduced sum of (iterations x mean film) over the ranks -> the mean over all iterations (.w carries the count)
+__global__ void __launch_bounds__(256) k_film_finish_mean(const float4* sum, float4* out, uint32_t pixels, uint32_t clamp) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= pixels) return;
+  float4 v = sum[i];
+  float inv = (v.w > 0.0f) ? 1.0f / v.w : 0.0f;
+  float x = v.x * inv, y = v.y * inv, z = v.z * inv;
+  if (clamp) {
+    x = fmaxf(0.0f, x);
+    y = fmaxf(0.0f, y);
+    z = fmaxf(0.0f, z);
+  }
+  out[i] = make_float4(x, y, z, 1.0f);
+}
+}  // extern "C"
+
+struct etxb_group {
+  std::vector<etxb_ctx*> lanes;
+  std::vector<std::thread> workers;
+  std::mutex m;
+  std::condition_variable cv_work, cv_idle;
+  uint32_t first_iteration = 0, stride = 1, taken = 0;  // the k-th iteration handed out renders index first + k * stride
+  uint32_t pending = 0, in_flight = 0;
+  bool quit = false;
+  int error = ETXB_OK;
+  std::string error_text;
+  std::chrono::steady_clock::time_point busy_since;
+  double busy_seconds = 0.0;   // wall time with at least one iteration queued or in flight
+  double last_iteration_seconds = 0.0;
+  DevBuf<float4> combined;
+  int device = 0;
+  // pixel-tile sharding over several processes (etxb_group_comm_init): every lane has its own communicator, and the k-th iteration of lane l is
+  // the ordinal l + k * lanes on EVERY rank (the shared counter of the single-GPU mode would pair different iterations across ranks)
+  bool sharded = false;
+  struct ReplicaItem {
+    uint32_t index;        // ordinal of the iteration within the job
+    uint32_t part, parts;  // parts == 1: the whole frame; else the camera pass of part `part` (tile % parts == part), light pass in full
+  };
+  std::deque<ReplicaItem> whole_queue, split_queue;
+  uint32_t split_lane = 0xffffffffu;  // replicas: the lane reserved for camera-split iterations (etxb_group_reserve_split_lane), or none
+  uint32_t split_part = 0, split_parts = 0;  // the (part, parts) that lane's film is made of; 0 parts = not used yet
+  bool replicas = false;             // etxb_group_comm_init_replicas: whole-frame iterations dealt to the ranks (global index j -> rank j % world), one film reduce
+  uint32_t job_enqueued = 0;         // replicas: iterations enqueued for the whole job
+  uint32_t world = 1, rank = 0;
+  uint32_t enqueued_total = 0;
+  std::vector<uint32_t> lane_next;
+  ncclComm_t reduce_comm = nullptr;  // the frame reduce has its own communicator: the lanes' ones are busy with iterations in flight
+  cudaStream_t stream = nullptr;
+  DevBuf<float4> combined_light, reduced;
 };
 
 namespace {
@@ -307,8 +418,6 @@ NcclApi* nccl_api() {
   });
   return api.handle ? &api : nullptr;
 }
-
-int ctx_drain_impl(etxb_ctx* ctx);
 
 int fail(etxb_ctx* ctx, int code, const char* fmt, ...) {
   char buf[1024];
@@ -514,26 +623,27 @@ int launch_shadow_resolve(etxb_ctx* ctx, const LaunchParams& p, uint32_t active)
   return ETXB_OK;
 }
 
-template <bool SP>
-int run_light_pass(etxb_ctx* ctx) {
-  LaunchParams p = make_params(ctx);
-  uint32_t* counts = ctx->queue_counts.ptr;  // [0] = current, [1] = next
+// The wavefront bounce loop of a pass.  `begin(queue, count)` launches the pass's first kernel, which fills the first queue and its
+// device-side count.  Every bounce traces the closest hits of the queue (timer `trace_kernel`), groups the queue by material when it is
+// long enough, clears the next count and calls `bounce(q, count, next_queue, next_count, active)` for the rest: its stages read queue `q`
+// and the count, and write the surviving paths to the next queue and count.  `active` is an upper bound of the count (kTailBatch), exact
+// whenever active >= thresholds.tail_queue.  The first count is stored to `first_active` when it is given.
+template <class Begin, class Bounce>
+int run_bounces(etxb_ctx* ctx, const LaunchParams& p, uint32_t trace_kernel, Begin&& begin, Bounce&& bounce, uint32_t* first_active = nullptr) {
+  uint32_t* counts = ctx->queue_counts.ptr;  // [cur] = this bounce's queue, [cur ^ 1] = the next one's
   CUDA_OK(ctx, cudaMemsetAsync(counts, 0, 8, ctx->stream));
-  CUDA_OK(ctx, cudaMemsetAsync(ctx->lv_tmp_count.ptr, 0, 4, ctx->stream));
   uint32_t* qin = ctx->queue_a.ptr;
   uint32_t* qout = ctx->queue_b.ptr;
-  {
-    LaunchTimer t(ctx, K_LIGHT_BEGIN);
-    k_light_begin<SP><<<blocks_for(ctx->path_count, 128), 128, 0, ctx->stream>>>(p, qin, counts + 0);
-  }
+  if (int rc = begin(qin, counts + 0)) return rc;
   uint32_t active = 0;
   if (int rc = read_u32(ctx, counts + 0, active)) return rc;
+  if (first_active) *first_active = active;
   uint32_t cur = 0, unsynced = 0;
   while (active > 0) {
     const bool sorted = sorts_queue(ctx, active);
-    const uint32_t* q = qin;
+    const uint32_t* q = qin;  // the queue every stage of this bounce reads
     {
-      LaunchTimer t(ctx, K_TRACE_LIGHT);
+      LaunchTimer t(ctx, trace_kernel);
       if (int rc = launch_trace_closest(ctx, p, qin, counts + cur, sorted ? ctx->queue_keys.ptr : nullptr, active)) return rc;
     }
     if (sorted) {
@@ -541,25 +651,38 @@ int run_light_pass(etxb_ctx* ctx) {
       if (int rc = sort_queue_by_material(ctx, qin, active, &q)) return rc;
     }
     CUDA_OK(ctx, cudaMemsetAsync(counts + (cur ^ 1u), 0, 4, ctx->stream));
+    if (int rc = bounce(q, counts + cur, qout, counts + (cur ^ 1u), active)) return rc;
+    cur ^= 1u;
+    std::swap(qin, qout);
+    if (int rc = next_queue_size(ctx, counts + cur, active, unsynced)) return rc;
+  }
+  CUDA_OK(ctx, cudaGetLastError());
+  return ETXB_OK;
+}
+
+template <bool SP, bool PLAIN>
+int run_light_pass(etxb_ctx* ctx) {
+  LaunchParams p = make_params(ctx);
+  auto begin = [&](uint32_t* queue, uint32_t* count) -> int {
+    CUDA_OK(ctx, cudaMemsetAsync(ctx->lv_tmp_count.ptr, 0, 4, ctx->stream));
+    LaunchTimer t(ctx, K_LIGHT_BEGIN);
+    k_light_begin<SP><<<blocks_for(ctx->path_count, 128), 128, 0, ctx->stream>>>(p, queue, count);
+    return ETXB_OK;
+  };
+  auto bounce = [&](const uint32_t* q, const uint32_t* count, uint32_t* next_queue, uint32_t* next_count, uint32_t active) -> int {
     if (p.shadow_atomic) CUDA_OK(ctx, cudaMemsetAsync(ctx->shadow_count.ptr, 0, 8, ctx->stream));
     {
       LaunchTimer t(ctx, K_LIGHT_BOUNCE);
-      if (ctx->plain_scene) {
-        k_light_bounce<SP, true><<<blocks_for(active, 128), 128, 0, ctx->stream>>>(p, q, counts + cur, qout, counts + (cur ^ 1u));
-      } else {
-        k_light_bounce<SP, false><<<blocks_for(active, 128), 128, 0, ctx->stream>>>(p, q, counts + cur, qout, counts + (cur ^ 1u));
-      }
+      k_light_bounce<SP, PLAIN><<<blocks_for(active, 128), 128, 0, ctx->stream>>>(p, q, count, next_queue, next_count);
     }
     if (p.shadow_atomic) {
       // the light-to-camera connections of this bounce: segments -> splats (light image)
       LaunchTimer t(ctx, K_SHADOW_TRACE);
       if (int rc = launch_shadow_resolve(ctx, p, active)) return rc;
     }
-    cur ^= 1u;
-    std::swap(qin, qout);
-    if (int rc = next_queue_size(ctx, counts + cur, active, unsynced)) return rc;
-  }
-  CUDA_OK(ctx, cudaGetLastError());
+    return ETXB_OK;
+  };
+  if (int rc = run_bounces(ctx, p, K_TRACE_LIGHT, begin, bounce)) return rc;
 
   // path-major vertex pool: offsets = exclusive scan of per-path counts (VCMLightPath::index)
   uint32_t total = 0;
@@ -697,42 +820,21 @@ int launch_merge(etxb_ctx* ctx, const LaunchParams& p, const uint32_t* q, const 
   return ETXB_OK;
 }
 
-template <bool SP>
+template <bool SP, bool PLAIN>
 int run_camera_pass(etxb_ctx* ctx) {
   LaunchParams p = make_params(ctx);
-  uint32_t* counts = ctx->queue_counts.ptr;
-  CUDA_OK(ctx, cudaMemsetAsync(counts, 0, 8, ctx->stream));
-  uint32_t* qin = ctx->queue_a.ptr;
-  uint32_t* qout = ctx->queue_b.ptr;
-  {
-    LaunchTimer t(ctx, K_CAMERA_BEGIN);
-    k_camera_begin<SP><<<blocks_for(ctx->path_count, 128), 128, 0, ctx->stream>>>(p, qin, counts + 0);
-  }
-  uint32_t active = 0;
-  if (int rc = read_u32(ctx, counts + 0, active)) return rc;
-  uint32_t cur = 0, unsynced = 0;
   const bool merging = (ctx->options.options & ETXB_VCM_ENABLE_MERGING) && (ctx->options.options & ETXB_VCM_MERGE_VERTICES);
-  while (active > 0) {
-    const bool sorted = sorts_queue(ctx, active);
-    const uint32_t* q = qin;  // the queue every stage of this bounce reads
-    {
-      LaunchTimer t(ctx, K_TRACE_CAMERA);
-      if (int rc = launch_trace_closest(ctx, p, qin, counts + cur, sorted ? ctx->queue_keys.ptr : nullptr, active)) return rc;
-    }
-    if (sorted) {
-      LaunchTimer t(ctx, K_QUEUE_SORT);
-      if (int rc = sort_queue_by_material(ctx, qin, active, &q)) return rc;
-    }
-    CUDA_OK(ctx, cudaMemsetAsync(counts + (cur ^ 1u), 0, 4, ctx->stream));
+  auto begin = [&](uint32_t* queue, uint32_t* count) -> int {
+    LaunchTimer t(ctx, K_CAMERA_BEGIN);
+    k_camera_begin<SP><<<blocks_for(ctx->path_count, 128), 128, 0, ctx->stream>>>(p, queue, count);
+    return ETXB_OK;
+  };
+  auto bounce = [&](const uint32_t* q, const uint32_t* count, uint32_t* next_queue, uint32_t* next_count, uint32_t active) -> int {
     if (p.connect_stage) CUDA_OK(ctx, cudaMemsetAsync(ctx->conn_count.ptr, 0, 4, ctx->stream));
     if (p.shadow_stage || p.shadow_atomic) CUDA_OK(ctx, cudaMemsetAsync(ctx->shadow_count.ptr, 0, 8, ctx->stream));
     {
       LaunchTimer t(ctx, K_CAMERA_SHADE);
-      if (ctx->plain_scene) {
-        k_camera_shade<SP, true><<<blocks_for(active, 128), 128, 0, ctx->stream>>>(p, q, counts + cur);
-      } else {
-        k_camera_shade<SP, false><<<blocks_for(active, 128), 128, 0, ctx->stream>>>(p, q, counts + cur);
-      }
+      k_camera_shade<SP, PLAIN><<<blocks_for(active, 128), 128, 0, ctx->stream>>>(p, q, count);
     }
     if (p.shadow_stage && (ctx->options.options & ETXB_VCM_CONNECT_VERTICES)) {
       // one thread per (camera vertex, light vertex) pair of the bounce, grid-stride over the reserved shadow slots (count on the device)
@@ -752,11 +854,7 @@ int run_camera_pass(etxb_ctx* ctx) {
         // tail of the pass: the pair count stays on the device (k_camera_connect is grid-stride), no host round trip per bounce
         LaunchTimer t(ctx, K_CAMERA_CONNECT);
         const uint32_t blocks = std::min<uint32_t>(ctx->sm_count * 4u, blocks_for(active * 4u, 128));
-        if (ctx->plain_scene) {
-          k_camera_connect<SP, true><<<blocks, 128, 0, ctx->stream>>>(p, ctx->conn_list.ptr);
-        } else {
-          k_camera_connect<SP, false><<<blocks, 128, 0, ctx->stream>>>(p, ctx->conn_list.ptr);
-        }
+        k_camera_connect<SP, PLAIN><<<blocks, 128, 0, ctx->stream>>>(p, ctx->conn_list.ptr);
       } else {
         uint32_t pending = 0;
         if (int rc = read_u32(ctx, ctx->conn_count.ptr, pending)) return rc;
@@ -774,11 +872,7 @@ int run_camera_pass(etxb_ctx* ctx) {
           }
           ctx->branch_counts.connect_launches += 1;
           LaunchTimer t(ctx, K_CAMERA_CONNECT);
-          if (ctx->plain_scene) {
-            k_camera_connect<SP, true><<<blocks_for(pending, 128), 128, 0, ctx->stream>>>(p, list);
-          } else {
-            k_camera_connect<SP, false><<<blocks_for(pending, 128), 128, 0, ctx->stream>>>(p, list);
-          }
+          k_camera_connect<SP, PLAIN><<<blocks_for(pending, 128), 128, 0, ctx->stream>>>(p, list);
         }
       }
     }
@@ -789,18 +883,13 @@ int run_camera_pass(etxb_ctx* ctx) {
       if (int rc = launch_shadow_resolve(ctx, p, active)) return rc;
     }
     if (merging) {
-      if (int rc = launch_merge<SP>(ctx, p, q, counts + cur, active)) return rc;
+      if (int rc = launch_merge<SP>(ctx, p, q, count, active)) return rc;
     }
-    {
-      LaunchTimer t(ctx, K_CAMERA_CONTINUE);
-      k_camera_continue<SP><<<blocks_for(active, 128), 128, 0, ctx->stream>>>(p, q, counts + cur, qout, counts + (cur ^ 1u));
-    }
-    cur ^= 1u;
-    std::swap(qin, qout);
-    if (int rc = next_queue_size(ctx, counts + cur, active, unsynced)) return rc;
-  }
-  CUDA_OK(ctx, cudaGetLastError());
-  return ETXB_OK;
+    LaunchTimer t(ctx, K_CAMERA_CONTINUE);
+    k_camera_continue<SP><<<blocks_for(active, 128), 128, 0, ctx->stream>>>(p, q, count, next_queue, next_count);
+    return ETXB_OK;
+  };
+  return run_bounces(ctx, p, K_TRACE_CAMERA, begin, bounce);
 }
 
 // Pixel-tile sharding (SURVEY 8(e), north star): between the light pass and the grid build of an iteration the ranks exchange what is global —
@@ -934,7 +1023,7 @@ int pt_estimate_noise_levels(etxb_ctx* ctx, uint32_t sample_index) {
 
 // One CPUPathTracingImpl task (path_tracing.cxx:50-83) followed by update()'s bookkeeping (:85-110): every active pixel's path, the film update,
 // the noise estimate.
-template <bool SP>
+template <bool SP, bool PLAIN>
 int run_pt_iteration(etxb_ctx* ctx) {
   CUDA_OK(ctx, cudaEventRecord(ctx->ev_iter_start, ctx->stream));
   if (int rc = pt_ensure_film(ctx)) return rc;
@@ -951,48 +1040,24 @@ int run_pt_iteration(etxb_ctx* ctx) {
   pt.pixel_sampler_radius = ctx->pixel_sampler_radius;
   pt.radiance_clamp = ctx->radiance_clamp;
   PtFilm pf = make_pt_film(ctx);
-  const bool plain = ctx->plain_scene;
-  uint32_t* counts = ctx->queue_counts.ptr;
-  CUDA_OK(ctx, cudaMemsetAsync(counts, 0, 8, ctx->stream));
-  uint32_t* qin = ctx->queue_a.ptr;
-  uint32_t* qout = ctx->queue_b.ptr;
-  {
+  auto begin = [&](uint32_t* queue, uint32_t* count) -> int {
     LaunchTimer t(ctx, K_PT_BEGIN);
-    k_pt_begin<SP><<<blocks_for(ctx->path_count, 128), 128, 0, ctx->stream>>>(p, pt, pf, qin, counts + 0);
-  }
-  uint32_t active = 0;
-  if (int rc = read_u32(ctx, counts + 0, active)) return rc;
-  ctx->pt_pixels_processed = active;
-  uint32_t cur = 0, unsynced = 0;
-  while (active > 0) {
-    const bool sorted = sorts_queue(ctx, active);
-    const uint32_t* q = qin;
-    {
-      LaunchTimer t(ctx, K_TRACE_CAMERA);
-      if (int rc = launch_trace_closest(ctx, p, qin, counts + cur, sorted ? ctx->queue_keys.ptr : nullptr, active)) return rc;
-    }
-    if (sorted) {
-      LaunchTimer t(ctx, K_QUEUE_SORT);
-      if (int rc = sort_queue_by_material(ctx, qin, active, &q)) return rc;
-    }
-    CUDA_OK(ctx, cudaMemsetAsync(counts + (cur ^ 1u), 0, 4, ctx->stream));
+    k_pt_begin<SP><<<blocks_for(ctx->path_count, 128), 128, 0, ctx->stream>>>(p, pt, pf, queue, count);
+    return ETXB_OK;
+  };
+  auto bounce = [&](const uint32_t* q, const uint32_t* count, uint32_t* next_queue, uint32_t* next_count, uint32_t active) -> int {
     if (p.shadow_atomic) CUDA_OK(ctx, cudaMemsetAsync(ctx->shadow_count.ptr, 0, 8, ctx->stream));
     {
       LaunchTimer t(ctx, K_PT_SHADE);
-      if (plain) {
-        k_pt_shade<SP, true><<<blocks_for(active, 128), 128, 0, ctx->stream>>>(p, pt, q, counts + cur, qout, counts + (cur ^ 1u));
-      } else {
-        k_pt_shade<SP, false><<<blocks_for(active, 128), 128, 0, ctx->stream>>>(p, pt, q, counts + cur, qout, counts + (cur ^ 1u));
-      }
+      k_pt_shade<SP, PLAIN><<<blocks_for(active, 128), 128, 0, ctx->stream>>>(p, pt, q, count, next_queue, next_count);
     }
     if (p.shadow_atomic) {
       LaunchTimer t(ctx, K_SHADOW_TRACE);
       if (int rc = launch_shadow_resolve(ctx, p, active)) return rc;
     }
-    cur ^= 1u;
-    std::swap(qin, qout);
-    if (int rc = next_queue_size(ctx, counts + cur, active, unsynced)) return rc;
-  }
+    return ETXB_OK;
+  };
+  if (int rc = run_bounces(ctx, p, K_TRACE_CAMERA, begin, bounce, &ctx->pt_pixels_processed)) return rc;
   {
     LaunchTimer t(ctx, K_PT_ACCUMULATE);
     k_pt_accumulate<SP><<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(p, pt, pf);
@@ -1002,177 +1067,10 @@ int run_pt_iteration(etxb_ctx* ctx) {
   return finish_iteration(ctx);
 }
 
-}  // namespace
-
-// ---------------------------------------------------------------------------------------------------------------------
-extern "C" {
-
-const char* etxb_build_flavor(void) { return kFlavor; }
-
-int etxb_device_count(void) {
-  int n = 0;
-  cudaError_t err = cudaGetDeviceCount(&n);
-  if (err != cudaSuccess) return ETXB_ERR_NO_DEVICE;
-  return n;
-}
-
-int etxb_create(etxb_ctx** out_ctx, const etxb_device_config* cfg) {
-  if (!out_ctx) return ETXB_ERR_INVALID_ARGUMENT;
-  *out_ctx = nullptr;
-  int n = etxb_device_count();
-  if (n <= 0) return ETXB_ERR_NO_DEVICE;
-  int device = cfg ? cfg->device_index : 0;
-  if (device < 0 || device >= n) return ETXB_ERR_INVALID_ARGUMENT;
-  if (cudaSetDevice(device) != cudaSuccess) return ETXB_ERR_CUDA;
-  auto* ctx = new etxb_ctx();
-  ctx->device = device;
-  int sms = 0;
-  if ((cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) == cudaSuccess) && (sms > 0)) ctx->sm_count = uint32_t(sms);
-  ctx->max_light_vertices_cfg = cfg ? cfg->max_light_vertices : 0;
-  ctx->profile = cfg ? (cfg->flags & 1u) != 0 : false;
-  if (ctx->profile) {
-    // the per-launch timing events of an iteration (two per launch, a few thousand per iteration) exist from the start: a lane that renders its first
-    // iteration inside a timed region (the camera-split lane of the replica mode) must not pay for creating them there
-    ctx->event_pool.reserve(8192);
-    for (uint32_t k = 0; k < 6144u; ++k) {
-      cudaEvent_t e = nullptr;
-      if (cudaEventCreate(&e) != cudaSuccess) break;
-      ctx->event_pool.push_back(e);
-    }
-  }
-  if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess) {
-    delete ctx;
-    return ETXB_ERR_CUDA;
-  }
-  cudaEventCreate(&ctx->ev_iter_start);
-  cudaEventCreate(&ctx->ev_iter_stop);
-  etxb_options_default(&ctx->options);
-  *out_ctx = ctx;
-  return ETXB_OK;
-}
-
-void etxb_destroy(etxb_ctx* ctx) {
-  if (!ctx) return;
-  if (ctx->worker.joinable()) {
-    {
-      std::lock_guard<std::mutex> lock(ctx->worker_m);
-      ctx->worker_queued = 0;
-      ctx->worker_quit = true;
-    }
-    ctx->worker_cv.notify_all();
-    ctx->worker.join();
-  }
-  cudaSetDevice(ctx->device);
-  cudaStreamSynchronize(ctx->stream);
-  if (ctx->comm != nullptr) {
-    if (NcclApi* n = nccl_api()) n->CommDestroy(ctx->comm);
-    ctx->comm = nullptr;
-  }
-  ctx->comm_counts.release();
-  ctx->film_reduced.release();
-  if (ctx->comm_stream) cudaStreamDestroy(ctx->comm_stream);
-  if (ctx->comm_ev_in) cudaEventDestroy(ctx->comm_ev_in);
-  if (ctx->comm_ev_out) cudaEventDestroy(ctx->comm_ev_out);
-  for (auto e : ctx->event_pool) cudaEventDestroy(e);
-  cudaEventDestroy(ctx->ev_iter_start);
-  cudaEventDestroy(ctx->ev_iter_stop);
-  DevBuf<float4>* f4[] = {&ctx->ray_o, &ctx->ray_d, &ctx->thr, &ctx->mis, &ctx->hit, &ctx->gathered, &ctx->merged, &ctx->camera_value, &ctx->bvh_tris, &ctx->g_pos, &ctx->g_nrm,
-    &ctx->g_win, &ctx->g_thr, &ctx->film_camera, &ctx->film_light, &ctx->film_light_iteration, &ctx->film_out, &ctx->conn_rec};
-  for (auto* b : f4) b->release();
-  DevBuf<uint32_t>* u32[] = {&ctx->tri_emitter, &ctx->lv_count, &ctx->lp_offset, &ctx->queue_a, &ctx->queue_b, &ctx->queue_counts, &ctx->sampler_end_light,
-    &ctx->sampler_end_camera, &ctx->merge_key, &ctx->conn_count, &ctx->lv_tmp_count, &ctx->overflow, &ctx->grid_bbox, &ctx->keys_in, &ctx->keys_out, &ctx->vals_in, &ctx->vals_out};
-  for (auto* b : u32) b->release();
-  ctx->vertices.release();
-  ctx->triangles.release();
-  ctx->materials.release();
-  ctx->profiles.release();
-  ctx->emitters.release();
-  ctx->spectra.release();
-  ctx->images.release();
-  ctx->mediums.release();
-  for (auto& b : ctx->medium_density) b.release();
-  for (auto& b : ctx->image_pixels) b.release();
-  for (auto& b : ctx->image_dists) b.release();
-  ctx->emitter_dist.release();
-  ctx->bvh_nodes.release();
-  ctx->wide_nodes.release();
-  ctx->xyz_table.release();
-  ctx->rgb_response_table.release();
-  ctx->bn_sobol.release();
-  ctx->bn_scrambling.release();
-  ctx->bn_ranking.release();
-  ctx->misc.release();
-  ctx->wavelength.release();
-  ctx->lv_tmp.release();
-  ctx->lv_final.release();
-  ctx->cell_range.release();
-  ctx->conn_list.release();
-  ctx->conn_list_sorted.release();
-  ctx->queue_sorted.release();
-  ctx->queue_keys.release();
-  ctx->queue_keys_sorted.release();
-  ctx->shadow_span.release();
-  ctx->shadow_p0.release();
-  ctx->shadow_p1.release();
-  ctx->shadow_value.release();
-  ctx->shadow_result.release();
-  ctx->shadow_count.release();
-  ctx->trace_cursor.release();
-  ctx->bs_props.release();
-  ctx->bs_weight_pdf.release();
-  ctx->bs_wo_eta.release();
-  ctx->film_ldr.release();
-  ctx->film_normals.release();
-  ctx->film_albedo.release();
-  ctx->film_adaptive.release();
-  ctx->pt_info.release();
-  ctx->pt_info_next.release();
-  ctx->pt_stats.release();
-  ctx->pt_error.release();
-  ctx->cub_temp.release();
-  ctx->counters.release();
-  cudaStreamDestroy(ctx->stream);
-  delete ctx;
-}
-
-const char* etxb_last_error(const etxb_ctx* ctx) { return ctx ? ctx->error.c_str() : "null context"; }
-
-int etxb_upload_color_tables(etxb_ctx* ctx, const float* xyz_441x3, const float* rgb_response_391x3) {
-  if (!ctx || !xyz_441x3 || !rgb_response_391x3) return ETXB_ERR_INVALID_ARGUMENT;
-  cudaSetDevice(ctx->device);
-  if (int rc = upload(ctx, ctx->xyz_table, xyz_441x3, 441 * 3)) return rc;
-  if (int rc = upload(ctx, ctx->rgb_response_table, rgb_response_391x3, 391 * 3)) return rc;
-  float sum = 0.0f;  // spectrum::kYIntegral (spectrum.hxx:187-193): float sum in table order
-  for (int i = 0; i < 441; ++i) sum += xyz_441x3[i * 3 + 1];
-  ctx->y_integral = sum;
-  ctx->dscene.xyz_table = ctx->xyz_table.ptr;
-  ctx->dscene.rgb_response_table = ctx->rgb_response_table.ptr;
-  ctx->dscene.y_scale = 1.0f / sum;
-  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-  return ETXB_OK;
-}
-
-int etxb_upload_blue_noise(etxb_ctx* ctx, const uint8_t* sobol_256x256, const uint8_t* scrambling, const uint8_t* ranking) {
-  if (!ctx || !sobol_256x256 || !scrambling || !ranking) return ETXB_ERR_INVALID_ARGUMENT;
-  cudaSetDevice(ctx->device);
-  if (int rc = upload(ctx, ctx->bn_sobol, sobol_256x256, 256 * 256)) return rc;
-  if (int rc = upload(ctx, ctx->bn_scrambling, scrambling, 128 * 128 * 8)) return rc;
-  if (int rc = upload(ctx, ctx->bn_ranking, ranking, 128 * 128 * 8)) return rc;
-  ctx->dscene.bn_sobol = ctx->bn_sobol.ptr;
-  ctx->dscene.bn_scrambling = ctx->bn_scrambling.ptr;
-  ctx->dscene.bn_ranking = ctx->bn_ranking.ptr;
-  ctx->dscene.has_blue_noise = 1;
-  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-  return ETXB_OK;
-}
-
 // ---- scene upload / update ------------------------------------------------------------------------------------------------------------------
 // etxb_upload_scene and etxb_update_scene run the same stages: validate_scene makes every check and touches nothing on the device,
 // prepare_scene hashes the bulk arrays (prepare_bvh builds the host BVH when the geometry is new), commit_scene copies to the device.  An
 // update keeps the device copies whose content hashes did not change; everything small is derived from the PODs again on every call.
-extern "C++" {
-namespace {
-
 struct SceneClass {
   bool stochastic = false;  // has_stochastic_merge
   bool boundaries = false, subsurface = false, deferred = false, opaque = false, plain = false;
@@ -1399,7 +1297,6 @@ int commit_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, Sce
   {
     const auto* meds = static_cast<const etxb_medium*>(s.mediums.a);
     std::vector<DMedium> dmeds(s.mediums.count);
-    for (size_t i = s.mediums.count; i < ctx->medium_density.size(); ++i) ctx->medium_density[i].release();
     ctx->medium_density.resize(s.mediums.count);
     for (uint64_t i = 0; i < s.mediums.count; ++i) {
       const etxb_medium& md = meds[i];
@@ -1443,11 +1340,6 @@ int commit_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, Sce
   {
     const auto* imgs = static_cast<const etxb_image*>(s.images.a);
     std::vector<DImage> dimgs(s.images.count);
-    for (size_t i = s.images.count; i < ctx->image_pixels.size(); ++i) {
-      ctx->image_pixels[i].release();
-      ctx->image_dists[i * 2].release();
-      ctx->image_dists[i * 2 + 1].release();
-    }
     ctx->image_pixels.resize(s.images.count);
     ctx->image_dists.resize(s.images.count * 2);
     for (uint64_t i = 0; i < s.images.count; ++i) {
@@ -1711,13 +1603,340 @@ int commit_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, Sce
   return etxb_begin(ctx, 0);
 }
 
+// one whole iteration on the calling thread; returns when it has finished (the bounce loops read queue sizes back)
+int run_iteration_blocking(etxb_ctx* ctx) {
+  if (ctx->integrator == ETXB_INTEGRATOR_PT) {
+    cudaSetDevice(ctx->device);
+    if (ctx->spectral) return ctx->plain_scene ? run_pt_iteration<true, true>(ctx) : run_pt_iteration<true, false>(ctx);
+    return ctx->plain_scene ? run_pt_iteration<false, true>(ctx) : run_pt_iteration<false, false>(ctx);
+  }
+  if (int rc = etxb_enqueue_light_pass(ctx)) return rc;
+  const void* records = nullptr;
+  uint64_t count = 0;
+  if (ctx->comm != nullptr) {  // pixel tiles over several GPUs: light image + photon records are exchanged here (comm_exchange)
+    if (int rc = comm_exchange(ctx, &records, &count)) return rc;
+  }
+  if (int rc = etxb_enqueue_grid_build(ctx, records, count)) return rc;
+  return etxb_enqueue_camera_pass(ctx);
+}
+
+void ctx_worker(etxb_ctx* ctx) {
+  std::unique_lock<std::mutex> lock(ctx->worker_m);
+  for (;;) {
+    ctx->worker_cv.wait(lock, [&] { return ctx->worker_quit || (ctx->worker_queued > 0); });
+    if (ctx->worker_quit) return;
+    ctx->worker_queued -= 1;
+    ctx->worker_busy = true;
+    lock.unlock();
+    int rc = run_iteration_blocking(ctx);
+    lock.lock();
+    ctx->worker_busy = false;
+    if ((rc != ETXB_OK) && (ctx->worker_error == ETXB_OK)) {
+      ctx->worker_error = rc;
+      ctx->worker_queued = 0;
+    }
+    if (ctx->worker_queued == 0) ctx->worker_idle.notify_all();
+  }
+}
+
+// blocks until every queued iteration has finished; returns (and clears) the first error one of them hit
+int ctx_drain(etxb_ctx* ctx) {
+  std::unique_lock<std::mutex> lock(ctx->worker_m);
+  ctx->worker_idle.wait(lock, [&] { return (ctx->worker_queued == 0) && !ctx->worker_busy; });
+  int rc = ctx->worker_error;
+  ctx->worker_error = ETXB_OK;
+  return rc;
+}
+
+// Film::layer (film.cxx:381-418): the device buffer that holds `layer` as float4 (computed into film_out where the layer is derived)
+int film_layer_source(etxb_ctx* ctx, uint32_t layer, const float4** out_src) {
+  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
+  cudaSetDevice(ctx->device);
+  const float4* src = nullptr;
+  switch (layer) {
+    case ETXB_FILM_RESULT: {
+      FilmBuffers film = {ctx->film_camera.ptr, ctx->film_light.ptr, ctx->film_light_iteration.ptr, ctx->width, ctx->height};
+      k_film_resolve<<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(film, ctx->film_out.ptr);
+      ctx->kernel_launches += 1;
+      src = ctx->film_out.ptr;
+      break;
+    }
+    case ETXB_FILM_CAMERA:
+      src = ctx->film_camera.ptr;
+      break;
+    case ETXB_FILM_LIGHT:
+      src = ctx->film_light.ptr;
+      break;
+    case ETXB_FILM_LIGHT_ITERATION:
+      src = ctx->film_light_iteration.ptr;
+      break;
+    case ETXB_FILM_NORMALS:
+    case ETXB_FILM_ALBEDO:
+    case ETXB_FILM_CAMERA_ADAPTIVE: {
+      if (int rc = pt_ensure_film(ctx)) return rc;
+      if (layer == ETXB_FILM_NORMALS) {
+        k_film_layer_normals<<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(ctx->film_normals.ptr, ctx->film_out.ptr, ctx->path_count);
+        ctx->kernel_launches += 1;
+        src = ctx->film_out.ptr;
+      } else {
+        src = (layer == ETXB_FILM_ALBEDO) ? ctx->film_albedo.ptr : ctx->film_adaptive.ptr;
+      }
+      break;
+    }
+    default:
+      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "unknown film layer %u", layer);
+  }
+  *out_src = src;
+  return ETXB_OK;
+}
+
+template <bool SP>
+int debug_merge(etxb_ctx* ctx, uint32_t record_count, const etxb_merge_query* d_queries, uint32_t count, float4* d_pos_nrm) {
+  if (int rc = run_grid_build<SP>(ctx, ctx->lv_final.ptr, record_count)) return rc;
+  LaunchParams p = make_params(ctx);
+  if (count) k_debug_merge_stage<SP><<<blocks_for(count, 128), 128, 0, ctx->stream>>>(p, d_queries, count, ctx->queue_a.ptr, d_pos_nrm);
+  ctx->kernel_launches += 1;
+  CUDA_OK(ctx, cudaMemcpyAsync(ctx->queue_counts.ptr, &count, 4, cudaMemcpyHostToDevice, ctx->stream));
+  if (count == 0) return ETXB_OK;
+  return launch_merge<SP>(ctx, p, ctx->queue_a.ptr, ctx->queue_counts.ptr, count);
+}
+
+// What one rank takes of `iterations` more iterations of a replica-mode job (ordinals base .. base + iterations - 1).  Whole frames are dealt
+// round-robin (ordinal j on rank j % world).  What is left when the count is not a multiple of the ranks would leave some ranks a whole iteration
+// behind the others (20 iterations on 8 ranks: 3, 3, 3, 3, 2, 2, 2, 2): with a split lane those R iterations are split instead, each over
+// P = world / R ranks by camera tile — every part traces the whole light pass itself (same photon map, no exchange) and the camera pass of its
+// tiles; the parts meet in the frame reduce.  A split lane's film is made of ONE (part, parts) geometry: a later round that would need another
+// one is dealt as whole frames.  Returns the parts of this round's split (0: none).
+uint32_t replica_plan(uint32_t world, uint32_t rank, uint32_t base, uint32_t iterations, bool split_lane, uint32_t have_part, uint32_t have_parts,
+                             std::vector<etxb_group::ReplicaItem>& out) {
+  uint32_t whole = iterations, rest = 0, parts = 1;
+  if ((iterations >= world) && split_lane) {
+    rest = iterations % world;
+    parts = rest ? (world / rest) : 1u;
+    if ((parts >= 2u) && ((have_parts == 0u) || (have_parts == parts))) {
+      whole = iterations - rest;
+    } else {
+      rest = 0;
+    }
+  }
+  for (uint32_t j = base; j < base + whole; ++j)
+    if ((j % world) == rank) out.push_back({j, 0u, 1u});
+  for (uint32_t r = 0; r < rest; ++r) {
+    if ((rank / parts) != r) continue;
+    const uint32_t part = rank % parts;
+    if ((have_parts != 0u) && (have_part != part)) continue;  // cannot happen while `parts` stays the same: a rank's part is rank % parts
+    out.push_back({base + whole + r, part, parts});
+  }
+  return rest ? parts : 0u;
+}
+
+bool group_has_work(const etxb_group* grp, uint32_t lane) {
+  if (grp->replicas) return (lane == grp->split_lane) ? !grp->split_queue.empty() : !grp->whole_queue.empty();
+  if (lane == grp->split_lane) return false;
+  return grp->sharded ? (grp->lane_next[lane] < grp->enqueued_total) : (grp->pending > 0);
+}
+bool group_idle(const etxb_group* grp) {
+  if (grp->in_flight > 0) return false;
+  if (grp->replicas) return grp->whole_queue.empty() && grp->split_queue.empty();
+  if (!grp->sharded) return grp->pending == 0;
+  for (uint32_t next : grp->lane_next)
+    if (next < grp->enqueued_total) return false;
+  return true;
+}
+
+void group_worker(etxb_group* grp, uint32_t lane) {
+  cudaSetDevice(grp->device);
+  etxb_ctx* ctx = grp->lanes[lane];
+  std::unique_lock<std::mutex> lock(grp->m);
+  for (;;) {
+    grp->cv_work.wait(lock, [&] { return grp->quit || group_has_work(grp, lane); });
+    if (grp->quit) return;
+    uint32_t ordinal = 0;
+    etxb_group::ReplicaItem item = {0u, 0u, 1u};
+    if (grp->replicas) {
+      auto& queue = (lane == grp->split_lane) ? grp->split_queue : grp->whole_queue;
+      item = queue.front();
+      queue.pop_front();
+      ordinal = item.index;
+      grp->taken = std::max(grp->taken, ordinal + 1u);
+    } else if (grp->sharded) {
+      ordinal = grp->lane_next[lane];
+      grp->lane_next[lane] += uint32_t(grp->lanes.size());
+      grp->taken = std::max(grp->taken, ordinal + 1u);
+    } else {
+      ordinal = grp->taken++;
+      grp->pending -= 1;
+    }
+    uint32_t iteration = grp->first_iteration + ordinal * grp->stride;
+    grp->in_flight += 1;
+    lock.unlock();
+    if (grp->replicas && (lane == grp->split_lane)) {
+      // this lane renders the camera pass of its part only; the light pass (and so the photon map) in full
+      ctx->rank = item.part;
+      ctx->world = item.parts;
+      ctx->light_full = true;
+    }
+    int rc = etxb_set_next_iteration(ctx, iteration);
+    if (rc == ETXB_OK) rc = run_iteration_blocking(ctx);  // returns when the iteration has finished (the bounce loops read queue sizes back)
+    lock.lock();
+    grp->in_flight -= 1;
+    grp->last_iteration_seconds = ctx->last_iteration_time;
+    if ((rc != ETXB_OK) && (grp->error == ETXB_OK)) {
+      grp->error = rc;
+      grp->error_text = etxb_last_error(ctx);
+      grp->pending = 0;
+      grp->whole_queue.clear();
+      grp->split_queue.clear();
+      for (auto& next : grp->lane_next) next = 0xffffffffu;
+    }
+    if (group_idle(grp)) {
+      grp->busy_seconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - grp->busy_since).count();
+      grp->cv_idle.notify_all();
+    }
+  }
+}
+
+int group_combine_into(etxb_group* grp, uint32_t layer, DevBuf<float4>& target, uint32_t* completed, bool raw = false) {
+  etxb_ctx* first = grp->lanes[0];
+  if (!first->scene_ready) return fail(first, ETXB_ERR_NOT_READY, "no scene uploaded");
+  size_t n = first->path_count;
+  cudaSetDevice(grp->device);
+  if (target.count < n) CUDA_OK(first, target.alloc(n));
+  FilmLanes f = {};
+  f.lanes = uint32_t(grp->lanes.size());
+  f.layer = layer;
+  f.pixels = uint32_t(n);
+  uint32_t total = 0;
+  for (auto* c : grp->lanes) total += c->completed;
+  for (uint32_t l = 0; l < f.lanes; ++l) {
+    f.camera[l] = grp->lanes[l]->film_camera.ptr;
+    f.light[l] = grp->lanes[l]->film_light.ptr;
+    f.weight[l] = raw ? float(grp->lanes[l]->completed) : (total ? float(double(grp->lanes[l]->completed) / double(total)) : 0.0f);
+    f.weight_light[l] = f.weight[l];
+    f.weight_count[l] = f.weight[l];
+    if (raw && (l == grp->split_lane) && (grp->split_part != 0u)) {
+      // a camera-split lane that is not part 0: its camera tiles count, its (complete, redundant) light image and its iteration count do not
+      f.weight_light[l] = 0.0f;
+      f.weight_count[l] = 0.0f;
+    }
+  }
+  f.raw = raw ? 1u : 0u;
+  // lanes that are still rendering keep updating their films (a preview, like reading the reference's film while it runs); after
+  // etxb_group_wait every lane has synchronised its stream and the result is exact
+  k_film_combine<<<blocks_for(f.pixels, 256), 256, 0, grp->stream>>>(f, target.ptr);
+  CUDA_OK(first, cudaStreamSynchronize(grp->stream));
+  if (completed) *completed = total;
+  return ETXB_OK;
+}
+
 }  // namespace
-}  // extern "C++"
+
+const char* etxb_build_flavor(void) { return kFlavor; }
+
+int etxb_device_count(void) {
+  int n = 0;
+  cudaError_t err = cudaGetDeviceCount(&n);
+  if (err != cudaSuccess) return ETXB_ERR_NO_DEVICE;
+  return n;
+}
+
+int etxb_create(etxb_ctx** out_ctx, const etxb_device_config* cfg) {
+  if (!out_ctx) return ETXB_ERR_INVALID_ARGUMENT;
+  *out_ctx = nullptr;
+  int n = etxb_device_count();
+  if (n <= 0) return ETXB_ERR_NO_DEVICE;
+  int device = cfg ? cfg->device_index : 0;
+  if (device < 0 || device >= n) return ETXB_ERR_INVALID_ARGUMENT;
+  if (cudaSetDevice(device) != cudaSuccess) return ETXB_ERR_CUDA;
+  auto* ctx = new etxb_ctx();
+  ctx->device = device;
+  int sms = 0;
+  if ((cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) == cudaSuccess) && (sms > 0)) ctx->sm_count = uint32_t(sms);
+  ctx->max_light_vertices_cfg = cfg ? cfg->max_light_vertices : 0;
+  ctx->profile = cfg ? (cfg->flags & 1u) != 0 : false;
+  if (ctx->profile) {
+    // the per-launch timing events of an iteration (two per launch, a few thousand per iteration) exist from the start: a lane that renders its first
+    // iteration inside a timed region (the camera-split lane of the replica mode) must not pay for creating them there
+    ctx->event_pool.reserve(8192);
+    for (uint32_t k = 0; k < 6144u; ++k) {
+      cudaEvent_t e = nullptr;
+      if (cudaEventCreate(&e) != cudaSuccess) break;
+      ctx->event_pool.push_back(e);
+    }
+  }
+  if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess) {
+    delete ctx;
+    return ETXB_ERR_CUDA;
+  }
+  cudaEventCreate(&ctx->ev_iter_start);
+  cudaEventCreate(&ctx->ev_iter_stop);
+  etxb_options_default(&ctx->options);
+  *out_ctx = ctx;
+  return ETXB_OK;
+}
+
+void etxb_destroy(etxb_ctx* ctx) {
+  if (!ctx) return;
+  if (ctx->worker.joinable()) {
+    {
+      std::lock_guard<std::mutex> lock(ctx->worker_m);
+      ctx->worker_queued = 0;
+      ctx->worker_quit = true;
+    }
+    ctx->worker_cv.notify_all();
+    ctx->worker.join();
+  }
+  cudaSetDevice(ctx->device);
+  cudaStreamSynchronize(ctx->stream);
+  if (ctx->comm != nullptr) {
+    if (NcclApi* n = nccl_api()) n->CommDestroy(ctx->comm);
+    ctx->comm = nullptr;
+  }
+  if (ctx->comm_stream) cudaStreamDestroy(ctx->comm_stream);
+  if (ctx->comm_ev_in) cudaEventDestroy(ctx->comm_ev_in);
+  if (ctx->comm_ev_out) cudaEventDestroy(ctx->comm_ev_out);
+  for (auto e : ctx->event_pool) cudaEventDestroy(e);
+  cudaEventDestroy(ctx->ev_iter_start);
+  cudaEventDestroy(ctx->ev_iter_stop);
+  cudaStreamDestroy(ctx->stream);
+  delete ctx;  // the device buffers free themselves, on ctx->device
+}
+
+const char* etxb_last_error(const etxb_ctx* ctx) { return ctx ? ctx->error.c_str() : "null context"; }
+
+int etxb_upload_color_tables(etxb_ctx* ctx, const float* xyz_441x3, const float* rgb_response_391x3) {
+  if (!ctx || !xyz_441x3 || !rgb_response_391x3) return ETXB_ERR_INVALID_ARGUMENT;
+  cudaSetDevice(ctx->device);
+  if (int rc = upload(ctx, ctx->xyz_table, xyz_441x3, 441 * 3)) return rc;
+  if (int rc = upload(ctx, ctx->rgb_response_table, rgb_response_391x3, 391 * 3)) return rc;
+  float sum = 0.0f;  // spectrum::kYIntegral (spectrum.hxx:187-193): float sum in table order
+  for (int i = 0; i < 441; ++i) sum += xyz_441x3[i * 3 + 1];
+  ctx->y_integral = sum;
+  ctx->dscene.xyz_table = ctx->xyz_table.ptr;
+  ctx->dscene.rgb_response_table = ctx->rgb_response_table.ptr;
+  ctx->dscene.y_scale = 1.0f / sum;
+  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+  return ETXB_OK;
+}
+
+int etxb_upload_blue_noise(etxb_ctx* ctx, const uint8_t* sobol_256x256, const uint8_t* scrambling, const uint8_t* ranking) {
+  if (!ctx || !sobol_256x256 || !scrambling || !ranking) return ETXB_ERR_INVALID_ARGUMENT;
+  cudaSetDevice(ctx->device);
+  if (int rc = upload(ctx, ctx->bn_sobol, sobol_256x256, 256 * 256)) return rc;
+  if (int rc = upload(ctx, ctx->bn_scrambling, scrambling, 128 * 128 * 8)) return rc;
+  if (int rc = upload(ctx, ctx->bn_ranking, ranking, 128 * 128 * 8)) return rc;
+  ctx->dscene.bn_sobol = ctx->bn_sobol.ptr;
+  ctx->dscene.bn_scrambling = ctx->bn_scrambling.ptr;
+  ctx->dscene.bn_ranking = ctx->bn_ranking.ptr;
+  ctx->dscene.has_blue_noise = 1;
+  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+  return ETXB_OK;
+}
 
 int etxb_upload_scene(etxb_ctx* ctx, const void* scene_blob, uint64_t scene_bytes, const void* camera_blob, uint64_t camera_bytes) {
   if (!ctx || !scene_blob || !camera_blob) return ETXB_ERR_INVALID_ARGUMENT;
   if (int rc = check_scene_args(ctx, scene_bytes, camera_bytes)) return rc;
-  ctx_drain_impl(ctx);
+  ctx_drain(ctx);
   cudaSetDevice(ctx->device);
   ctx->scene_ready = false;
   const etxb_scene& s = *static_cast<const etxb_scene*>(scene_blob);
@@ -1733,7 +1952,7 @@ int etxb_update_scene(etxb_ctx* ctx, const void* scene_blob, uint64_t scene_byte
   if (!ctx || !scene_blob || !camera_blob) return ETXB_ERR_INVALID_ARGUMENT;
   if (int rc = check_scene_args(ctx, scene_bytes, camera_bytes)) return rc;
   if (ctx->comm != nullptr) return fail(ctx, ETXB_ERR_UNSUPPORTED, "etxb_update_scene: a context with a communicator takes a new scene through etxb_upload_scene");
-  ctx_drain_impl(ctx);
+  ctx_drain(ctx);
   cudaSetDevice(ctx->device);
   const etxb_scene& s = *static_cast<const etxb_scene*>(scene_blob);
   const etxb_camera& cam = *static_cast<const etxb_camera*>(camera_blob);
@@ -1802,7 +2021,7 @@ int etxb_set_next_iteration(etxb_ctx* ctx, uint32_t iteration) {
 int etxb_begin(etxb_ctx* ctx, uint32_t first_iteration) {
   if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;
   if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
-  ctx_drain_impl(ctx);  // Integrator::run first stops what is running (vcm_cpu.cxx:255-262)
+  ctx_drain(ctx);  // Integrator::run first stops what is running (vcm_cpu.cxx:255-262)
   cudaSetDevice(ctx->device);
   size_t n = ctx->path_count;
   CUDA_OK(ctx, cudaMemsetAsync(ctx->film_camera.ptr, 0, n * 16, ctx->stream));
@@ -1839,7 +2058,8 @@ int etxb_enqueue_light_pass(etxb_ctx* ctx) {
   if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
   cudaSetDevice(ctx->device);
   CUDA_OK(ctx, cudaEventRecord(ctx->ev_iter_start, ctx->stream));
-  return ctx->spectral ? run_light_pass<true>(ctx) : run_light_pass<false>(ctx);
+  if (ctx->spectral) return ctx->plain_scene ? run_light_pass<true, true>(ctx) : run_light_pass<true, false>(ctx);
+  return ctx->plain_scene ? run_light_pass<false, true>(ctx) : run_light_pass<false, false>(ctx);
 }
 
 int etxb_enqueue_grid_build(etxb_ctx* ctx, const void* device_photon_records, uint64_t photon_count) {
@@ -1861,59 +2081,11 @@ int etxb_enqueue_camera_pass(etxb_ctx* ctx) {
   if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;
   if (!ctx->light_pass_done || !ctx->grid_done) return fail(ctx, ETXB_ERR_NOT_READY, "light pass / grid build have not run");
   cudaSetDevice(ctx->device);
-  int rc = ctx->spectral ? run_camera_pass<true>(ctx) : run_camera_pass<false>(ctx);
+  int rc = ctx->spectral ? (ctx->plain_scene ? run_camera_pass<true, true>(ctx) : run_camera_pass<true, false>(ctx))
+                         : (ctx->plain_scene ? run_camera_pass<false, true>(ctx) : run_camera_pass<false, false>(ctx));
   if (rc) return rc;
   return finish_iteration(ctx);
 }
-
-// one whole iteration on the calling thread; returns when it has finished (the bounce loops read queue sizes back)
-static int run_iteration_blocking(etxb_ctx* ctx) {
-  if (ctx->integrator == ETXB_INTEGRATOR_PT) {
-    cudaSetDevice(ctx->device);
-    return ctx->spectral ? run_pt_iteration<true>(ctx) : run_pt_iteration<false>(ctx);
-  }
-  if (int rc = etxb_enqueue_light_pass(ctx)) return rc;
-  const void* records = nullptr;
-  uint64_t count = 0;
-  if (ctx->comm != nullptr) {  // pixel tiles over several GPUs: light image + photon records are exchanged here (comm_exchange)
-    if (int rc = comm_exchange(ctx, &records, &count)) return rc;
-  }
-  if (int rc = etxb_enqueue_grid_build(ctx, records, count)) return rc;
-  return etxb_enqueue_camera_pass(ctx);
-}
-
-static void ctx_worker(etxb_ctx* ctx) {
-  std::unique_lock<std::mutex> lock(ctx->worker_m);
-  for (;;) {
-    ctx->worker_cv.wait(lock, [&] { return ctx->worker_quit || (ctx->worker_queued > 0); });
-    if (ctx->worker_quit) return;
-    ctx->worker_queued -= 1;
-    ctx->worker_busy = true;
-    lock.unlock();
-    int rc = run_iteration_blocking(ctx);
-    lock.lock();
-    ctx->worker_busy = false;
-    if ((rc != ETXB_OK) && (ctx->worker_error == ETXB_OK)) {
-      ctx->worker_error = rc;
-      ctx->worker_queued = 0;
-    }
-    if (ctx->worker_queued == 0) ctx->worker_idle.notify_all();
-  }
-}
-
-// blocks until every queued iteration has finished; returns (and clears) the first error one of them hit
-static int ctx_drain(etxb_ctx* ctx) { return ctx_drain_impl(ctx); }
-extern "C++" {
-namespace {
-int ctx_drain_impl(etxb_ctx* ctx) {
-  std::unique_lock<std::mutex> lock(ctx->worker_m);
-  ctx->worker_idle.wait(lock, [&] { return (ctx->worker_queued == 0) && !ctx->worker_busy; });
-  int rc = ctx->worker_error;
-  ctx->worker_error = ETXB_OK;
-  return rc;
-}
-}  // namespace
-}  // extern "C++"
 
 int etxb_enqueue_iteration(etxb_ctx* ctx) {
   if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;
@@ -1951,14 +2123,14 @@ int etxb_pt_options_set_key(etxb_pt_options* opt, const char* key, double value)
 
 int etxb_pt_set_options(etxb_ctx* ctx, const etxb_pt_options* opt) {
   if (!ctx || !opt) return ETXB_ERR_INVALID_ARGUMENT;
-  if (int rc = ctx_drain_impl(ctx)) return rc;
+  if (int rc = ctx_drain(ctx)) return rc;
   ctx->pt_options = *opt;
   return ETXB_OK;
 }
 
 int etxb_set_integrator(etxb_ctx* ctx, uint32_t integrator) {
   if (!ctx || (integrator > ETXB_INTEGRATOR_PT)) return ETXB_ERR_INVALID_ARGUMENT;
-  if (int rc = ctx_drain_impl(ctx)) return rc;
+  if (int rc = ctx_drain(ctx)) return rc;
   if ((integrator == ETXB_INTEGRATOR_PT) && (ctx->world > 1u)) return fail(ctx, ETXB_ERR_UNSUPPORTED, "the path tracer runs on one GPU per context");
   ctx->integrator = integrator;
   return ETXB_OK;
@@ -1977,7 +2149,7 @@ int etxb_pt_get_status(etxb_ctx* ctx, etxb_pt_status* out) {
 // Scene::noise_threshold / radiance_clamp / samples are scene settings the application edits between runs (ui.cxx) without a new upload
 int etxb_set_scene_settings(etxb_ctx* ctx, float noise_threshold, float radiance_clamp) {
   if (!ctx || !(noise_threshold >= 0.0f) || !(radiance_clamp >= 0.0f)) return ETXB_ERR_INVALID_ARGUMENT;
-  if (int rc = ctx_drain_impl(ctx)) return rc;
+  if (int rc = ctx_drain(ctx)) return rc;
   ctx->noise_threshold = noise_threshold;
   ctx->radiance_clamp = radiance_clamp;
   return ETXB_OK;
@@ -2027,7 +2199,7 @@ int etxb_comm_reduce_film(etxb_ctx* ctx, uint32_t layer, float* dst_rgba, uint64
   if (!ctx || (layer > ETXB_FILM_LIGHT)) return ETXB_ERR_INVALID_ARGUMENT;
   if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
   if (ctx->comm == nullptr) return etxb_read_film(ctx, layer, dst_rgba, dst_bytes);
-  if (int rc = ctx_drain_impl(ctx)) return rc;
+  if (int rc = ctx_drain(ctx)) return rc;
   NcclApi* n = nccl_api();
   cudaSetDevice(ctx->device);
   const size_t px = ctx->path_count;
@@ -2094,48 +2266,6 @@ int etxb_film_size(const etxb_ctx* ctx, uint32_t* width, uint32_t* height) {
   return ETXB_OK;
 }
 
-// Film::layer (film.cxx:381-418): the device buffer that holds `layer` as float4 (computed into film_out where the layer is derived)
-static int film_layer_source(etxb_ctx* ctx, uint32_t layer, const float4** out_src) {
-  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
-  cudaSetDevice(ctx->device);
-  const float4* src = nullptr;
-  switch (layer) {
-    case ETXB_FILM_RESULT: {
-      FilmBuffers film = {ctx->film_camera.ptr, ctx->film_light.ptr, ctx->film_light_iteration.ptr, ctx->width, ctx->height};
-      k_film_resolve<<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(film, ctx->film_out.ptr);
-      ctx->kernel_launches += 1;
-      src = ctx->film_out.ptr;
-      break;
-    }
-    case ETXB_FILM_CAMERA:
-      src = ctx->film_camera.ptr;
-      break;
-    case ETXB_FILM_LIGHT:
-      src = ctx->film_light.ptr;
-      break;
-    case ETXB_FILM_LIGHT_ITERATION:
-      src = ctx->film_light_iteration.ptr;
-      break;
-    case ETXB_FILM_NORMALS:
-    case ETXB_FILM_ALBEDO:
-    case ETXB_FILM_CAMERA_ADAPTIVE: {
-      if (int rc = pt_ensure_film(ctx)) return rc;
-      if (layer == ETXB_FILM_NORMALS) {
-        k_film_layer_normals<<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(ctx->film_normals.ptr, ctx->film_out.ptr, ctx->path_count);
-        ctx->kernel_launches += 1;
-        src = ctx->film_out.ptr;
-      } else {
-        src = (layer == ETXB_FILM_ALBEDO) ? ctx->film_albedo.ptr : ctx->film_adaptive.ptr;
-      }
-      break;
-    }
-    default:
-      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "unknown film layer %u", layer);
-  }
-  *out_src = src;
-  return ETXB_OK;
-}
-
 int etxb_read_film(etxb_ctx* ctx, uint32_t layer, float* dst_rgba, uint64_t dst_bytes) {
   if (!ctx || !dst_rgba) return ETXB_ERR_INVALID_ARGUMENT;
   size_t n = ctx->path_count;
@@ -2168,7 +2298,7 @@ int etxb_read_film_ldr(etxb_ctx* ctx, uint32_t layer, float exposure, uint8_t* d
 int etxb_save_film(etxb_ctx* ctx, uint32_t layer, const char* file_name, uint32_t mode, float exposure) {
   if (!ctx || !file_name || (mode > ETXB_SAVE_PNG_TONEMAPPED)) return ETXB_ERR_INVALID_ARGUMENT;
   if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
-  if (int rc = ctx_drain_impl(ctx)) return rc;
+  if (int rc = ctx_drain(ctx)) return rc;
   const size_t n = ctx->path_count;
   int rc = ETXB_OK;
   if (mode == ETXB_SAVE_EXR) {
@@ -2245,7 +2375,7 @@ int etxb_device_pointer(etxb_ctx* ctx, uint32_t buffer_id, void** out_ptr, uint6
 
 int etxb_read_buffer(etxb_ctx* ctx, uint32_t buffer_id, void* dst, uint64_t dst_bytes, uint64_t* out_bytes) {
   if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;
-  if (int rc = ctx_drain_impl(ctx)) return rc;
+  if (int rc = ctx_drain(ctx)) return rc;
   cudaSetDevice(ctx->device);
   size_t lv = ctx->last_light_vertices;
   if (buffer_id == ETXB_BUF_LV_POS || buffer_id == ETXB_BUF_LV_THROUGHPUT || buffer_id == ETXB_BUF_LV_MIS) {
@@ -2299,12 +2429,10 @@ int etxb_debug_trace(etxb_ctx* ctx, const float* rays, uint32_t* seeds, uint32_t
   cudaSetDevice(ctx->device);
   DevBuf<float> d_rays, d_uvt;
   DevBuf<uint32_t> d_seeds, d_tri;
-  CUDA_OK(ctx, d_rays.alloc(size_t(count) * 8));
+  if (int rc = upload(ctx, d_rays, rays, size_t(count) * 8)) return rc;
+  if (int rc = upload(ctx, d_seeds, seeds, count)) return rc;
   CUDA_OK(ctx, d_uvt.alloc(size_t(count) * 3));
-  CUDA_OK(ctx, d_seeds.alloc(count));
   CUDA_OK(ctx, d_tri.alloc(count));
-  CUDA_OK(ctx, cudaMemcpy(d_rays.ptr, rays, d_rays.bytes(), cudaMemcpyHostToDevice));
-  CUDA_OK(ctx, cudaMemcpy(d_seeds.ptr, seeds, d_seeds.bytes(), cudaMemcpyHostToDevice));
   if (ctx->debug_trace_wide && (ctx->dscene.wide_nodes != nullptr)) {
     k_debug_trace_wide<<<blocks_for(count, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_rays.ptr, d_seeds.ptr, count, d_uvt.ptr, d_tri.ptr);
   } else {
@@ -2312,13 +2440,9 @@ int etxb_debug_trace(etxb_ctx* ctx, const float* rays, uint32_t* seeds, uint32_t
   }
   ctx->kernel_launches += 1;
   CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-  CUDA_OK(ctx, cudaMemcpy(seeds, d_seeds.ptr, d_seeds.bytes(), cudaMemcpyDeviceToHost));
+  CUDA_OK(ctx, cudaMemcpy(seeds, d_seeds.ptr, size_t(count) * 4, cudaMemcpyDeviceToHost));
   CUDA_OK(ctx, cudaMemcpy(hits_uv_t, d_uvt.ptr, d_uvt.bytes(), cudaMemcpyDeviceToHost));
   CUDA_OK(ctx, cudaMemcpy(hits_tri, d_tri.ptr, d_tri.bytes(), cudaMemcpyDeviceToHost));
-  d_rays.release();
-  d_uvt.release();
-  d_seeds.release();
-  d_tri.release();
   return ETXB_OK;
 }
 
@@ -2329,16 +2453,13 @@ int etxb_debug_occluded(etxb_ctx* ctx, const float* segments, uint32_t count, ui
   cudaSetDevice(ctx->device);
   DevBuf<float> d_segments;
   DevBuf<uint32_t> d_occluded;
-  CUDA_OK(ctx, d_segments.alloc(size_t(count) * 6));
+  if (int rc = upload(ctx, d_segments, segments, size_t(count) * 6)) return rc;
   CUDA_OK(ctx, d_occluded.alloc(count));
-  CUDA_OK(ctx, cudaMemcpy(d_segments.ptr, segments, d_segments.bytes(), cudaMemcpyHostToDevice));
   const uint32_t wide = (ctx->debug_trace_wide && (ctx->dscene.wide_nodes != nullptr)) ? 1u : 0u;
   k_debug_occluded<<<blocks_for(count, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_segments.ptr, count, wide, d_occluded.ptr);
   ctx->kernel_launches += 1;
   CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
   CUDA_OK(ctx, cudaMemcpy(occluded, d_occluded.ptr, d_occluded.bytes(), cudaMemcpyDeviceToHost));
-  d_segments.release();
-  d_occluded.release();
   return ETXB_OK;
 }
 
@@ -2355,21 +2476,15 @@ int etxb_debug_sampler(etxb_ctx* ctx, const uint32_t* a, const uint32_t* b, uint
   cudaSetDevice(ctx->device);
   DevBuf<uint32_t> da, db, ds;
   DevBuf<float> dv;
-  CUDA_OK(ctx, da.alloc(count));
-  CUDA_OK(ctx, db.alloc(count));
+  if (int rc = upload(ctx, da, a, count)) return rc;
+  if (int rc = upload(ctx, db, b, count)) return rc;
   CUDA_OK(ctx, ds.alloc(size_t(count) * (draws + 1)));
   CUDA_OK(ctx, dv.alloc(size_t(count) * std::max(draws, 1u)));
-  CUDA_OK(ctx, cudaMemcpy(da.ptr, a, da.bytes(), cudaMemcpyHostToDevice));
-  CUDA_OK(ctx, cudaMemcpy(db.ptr, b, db.bytes(), cudaMemcpyHostToDevice));
   k_debug_sampler<<<blocks_for(count, 128), 128, 0, ctx->stream>>>(da.ptr, db.ptr, count, draws, ds.ptr, dv.ptr);
   ctx->kernel_launches += 1;
   CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
   CUDA_OK(ctx, cudaMemcpy(out_seed, ds.ptr, ds.bytes(), cudaMemcpyDeviceToHost));
   if (draws) CUDA_OK(ctx, cudaMemcpy(out_values, dv.ptr, size_t(count) * draws * 4, cudaMemcpyDeviceToHost));
-  da.release();
-  db.release();
-  ds.release();
-  dv.release();
   return ETXB_OK;
 }
 
@@ -2377,20 +2492,14 @@ int etxb_debug_math(etxb_ctx* ctx, uint32_t fn, const float* x, const float* y, 
   if (!ctx || !x || !out) return ETXB_ERR_INVALID_ARGUMENT;
   cudaSetDevice(ctx->device);
   DevBuf<float> dx, dy, dout;
-  CUDA_OK(ctx, dx.alloc(count));
+  if (int rc = upload(ctx, dx, x, count)) return rc;
+  if (y)
+    if (int rc = upload(ctx, dy, y, count)) return rc;
   CUDA_OK(ctx, dout.alloc(count));
-  CUDA_OK(ctx, cudaMemcpy(dx.ptr, x, dx.bytes(), cudaMemcpyHostToDevice));
-  if (y) {
-    CUDA_OK(ctx, dy.alloc(count));
-    CUDA_OK(ctx, cudaMemcpy(dy.ptr, y, dy.bytes(), cudaMemcpyHostToDevice));
-  }
   k_debug_math<<<blocks_for(count, 128), 128, 0, ctx->stream>>>(ctx->dscene, fn, dx.ptr, y ? dy.ptr : nullptr, count, dout.ptr);
   ctx->kernel_launches += 1;
   CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
   CUDA_OK(ctx, cudaMemcpy(out, dout.ptr, dout.bytes(), cudaMemcpyDeviceToHost));
-  dx.release();
-  dy.release();
-  dout.release();
   return ETXB_OK;
 }
 
@@ -2405,9 +2514,8 @@ int etxb_debug_closure_eval(etxb_ctx* ctx, const etxb_closure_query* queries, ui
   cudaSetDevice(ctx->device);
   DevBuf<etxb_closure_query> d_queries;
   DevBuf<double> d_out;
-  CUDA_OK(ctx, d_queries.alloc(count));
+  if (int rc = upload(ctx, d_queries, queries, count)) return rc;
   CUDA_OK(ctx, d_out.alloc(size_t(count) * ETXB_CLOSURE_STATS));
-  CUDA_OK(ctx, cudaMemcpy(d_queries.ptr, queries, d_queries.bytes(), cudaMemcpyHostToDevice));
   if (ctx->spectral) {
     k_debug_closure<true><<<blocks_for(count, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
   } else {
@@ -2417,8 +2525,6 @@ int etxb_debug_closure_eval(etxb_ctx* ctx, const etxb_closure_query* queries, ui
   CUDA_OK(ctx, cudaGetLastError());
   CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
   CUDA_OK(ctx, cudaMemcpy(out, d_out.ptr, d_out.bytes(), cudaMemcpyDeviceToHost));
-  d_queries.release();
-  d_out.release();
   return ETXB_OK;
 }
 
@@ -2431,32 +2537,17 @@ int etxb_debug_set_thresholds(etxb_ctx* ctx, const etxb_debug_thresholds* thresh
     // below tail_queue the host enqueues bounces on a stale queue size, and the gather's sort would take in slots past the count
     return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "merge_sort_min_queries (%u) must not be below tail_queue (%u)", t.merge_sort_min_queries, t.tail_queue);
   }
-  ctx_drain_impl(ctx);
+  ctx_drain(ctx);
   ctx->thresholds = t;
   return ETXB_OK;
 }
 
 int etxb_debug_get_branch_counts(etxb_ctx* ctx, etxb_debug_branch_counts* out) {
   if (!ctx || !out) return ETXB_ERR_INVALID_ARGUMENT;
-  if (int rc = ctx_drain_impl(ctx)) return rc;
+  if (int rc = ctx_drain(ctx)) return rc;
   *out = ctx->branch_counts;
   return ETXB_OK;
 }
-
-extern "C++" {
-namespace {
-template <bool SP>
-int debug_merge(etxb_ctx* ctx, uint32_t record_count, const etxb_merge_query* d_queries, uint32_t count, float4* d_pos_nrm) {
-  if (int rc = run_grid_build<SP>(ctx, ctx->lv_final.ptr, record_count)) return rc;
-  LaunchParams p = make_params(ctx);
-  if (count) k_debug_merge_stage<SP><<<blocks_for(count, 128), 128, 0, ctx->stream>>>(p, d_queries, count, ctx->queue_a.ptr, d_pos_nrm);
-  ctx->kernel_launches += 1;
-  CUDA_OK(ctx, cudaMemcpyAsync(ctx->queue_counts.ptr, &count, 4, cudaMemcpyHostToDevice, ctx->stream));
-  if (count == 0) return ETXB_OK;
-  return launch_merge<SP>(ctx, p, ctx->queue_a.ptr, ctx->queue_counts.ptr, count);
-}
-}  // namespace
-}  // extern "C++"
 
 // Test hook: the photon gather query by query (layout and outputs in include/etx_b200.h)
 int etxb_debug_merge(etxb_ctx* ctx, const void* records, uint32_t record_count, const float* light_wavelengths, const etxb_merge_query* queries, uint32_t count,
@@ -2473,7 +2564,7 @@ int etxb_debug_merge(etxb_ctx* ctx, const void* records, uint32_t record_count, 
     if (queries[k].tri >= ctx->triangles.count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "merge query %u: triangle index out of range", k);
     if ((queries[k].medium != ETXB_INVALID_INDEX) && (queries[k].medium >= ctx->dscene.medium_count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "merge query %u: medium index out of range", k);
   }
-  if (int rc = ctx_drain_impl(ctx)) return rc;
+  if (int rc = ctx_drain(ctx)) return rc;
   cudaSetDevice(ctx->device);
   if (record_count) CUDA_OK(ctx, cudaMemcpyAsync(ctx->lv_final.ptr, records, size_t(record_count) * sizeof(LightVertexRec), cudaMemcpyHostToDevice, ctx->stream));
   CUDA_OK(ctx, cudaMemcpyAsync(ctx->wavelength.ptr, light_wavelengths, size_t(ctx->path_count) * 4u, cudaMemcpyHostToDevice, ctx->stream));
@@ -2481,9 +2572,8 @@ int etxb_debug_merge(etxb_ctx* ctx, const void* records, uint32_t record_count, 
   CUDA_OK(ctx, cudaMemcpyAsync(&before, ctx->counters.ptr, sizeof(before), cudaMemcpyDeviceToHost, ctx->stream));
   DevBuf<etxb_merge_query> d_queries;
   DevBuf<float4> d_pos_nrm;
-  CUDA_OK(ctx, d_queries.alloc(std::max<uint32_t>(count, 1u)));
+  if (int rc = upload(ctx, d_queries, queries, count)) return rc;
   CUDA_OK(ctx, d_pos_nrm.alloc(2u * std::max<uint32_t>(count, 1u)));
-  if (count) CUDA_OK(ctx, cudaMemcpyAsync(d_queries.ptr, queries, size_t(count) * sizeof(etxb_merge_query), cudaMemcpyHostToDevice, ctx->stream));
   int rc = ctx->spectral ? debug_merge<true>(ctx, record_count, d_queries.ptr, count, d_pos_nrm.ptr) : debug_merge<false>(ctx, record_count, d_queries.ptr, count, d_pos_nrm.ptr);
   if (rc) return rc;
   CUDA_OK(ctx, cudaGetLastError());
@@ -2518,193 +2608,7 @@ int etxb_debug_merge(etxb_ctx* ctx, const void* records, uint32_t record_count, 
   return ETXB_OK;
 }
 
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Iterations in flight (etxb_group): L contexts on one device, one host thread each, pulling iteration indices from a shared
-// counter.  VCM iterations are independent (vcm_cpu.cxx:95-113: the index only sets the merge radius and the sampler seeds), and
-// the bounce loop of one iteration ends in a long latency-bound tail (a few thousand paths, ~50 bounces); with several iterations in
-// flight that tail overlaps the full-width head of another iteration.  The film is the mean of the lanes' films weighted by the
-// iterations each lane finished — the same set of iterations, hence the same estimate, as one context running them in sequence.
-// ---------------------------------------------------------------------------------------------------------------------
-constexpr uint32_t kMaxLanes = 9;  // 8 whole-iteration lanes + the camera-split lane of the replica mode
-struct FilmLanes {
-  const float4* camera[kMaxLanes];
-  const float4* light[kMaxLanes];
-  float weight[kMaxLanes];        // camera layer
-  float weight_light[kMaxLanes];  // light layer (differs from `weight` only for a camera-split lane that is not part 0)
-  float weight_count[kMaxLanes];  // raw mode: what the lane adds to .w
-  uint32_t lanes, layer, pixels;
-  uint32_t raw;  // 1: no clamp, alpha = sum of the weights (a partial sum that another stage finishes)
-};
-__global__ void __launch_bounds__(256) k_film_combine(FilmLanes f, float4* out) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= f.pixels) return;
-  float x = 0.0f, y = 0.0f, z = 0.0f;
-  for (uint32_t l = 0; l < f.lanes; ++l) {
-    float4 c = (f.layer != ETXB_FILM_LIGHT) ? f.camera[l][i] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-    float4 g = (f.layer != ETXB_FILM_CAMERA) ? f.light[l][i] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-    x += f.weight[l] * c.x + f.weight_light[l] * g.x;
-    y += f.weight[l] * c.y + f.weight_light[l] * g.y;
-    z += f.weight[l] * c.z + f.weight_light[l] * g.z;
-  }
-  if (f.raw) {
-    float w = 0.0f;
-    for (uint32_t l = 0; l < f.lanes; ++l) w += f.weight_count[l];
-    out[i] = make_float4(x, y, z, w);
-    return;
-  }
-  if (f.layer == ETXB_FILM_RESULT) {  // Film::layer(Result): max(0, camera + light) (film.cxx:381-418)
-    x = fmaxf(0.0f, x);
-    y = fmaxf(0.0f, y);
-    z = fmaxf(0.0f, z);
-  }
-  out[i] = make_float4(x, y, z, 1.0f);
-}
-// rank 0 of a replica run: the reduced sum of (iterations x mean film) over the ranks -> the mean over all iterations (.w carries the count)
-__global__ void __launch_bounds__(256) k_film_finish_mean(const float4* sum, float4* out, uint32_t pixels, uint32_t clamp) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= pixels) return;
-  float4 v = sum[i];
-  float inv = (v.w > 0.0f) ? 1.0f / v.w : 0.0f;
-  float x = v.x * inv, y = v.y * inv, z = v.z * inv;
-  if (clamp) {
-    x = fmaxf(0.0f, x);
-    y = fmaxf(0.0f, y);
-    z = fmaxf(0.0f, z);
-  }
-  out[i] = make_float4(x, y, z, 1.0f);
-}
-
-struct etxb_group {
-  std::vector<etxb_ctx*> lanes;
-  std::vector<std::thread> workers;
-  std::mutex m;
-  std::condition_variable cv_work, cv_idle;
-  uint32_t first_iteration = 0, stride = 1, taken = 0;  // the k-th iteration handed out renders index first + k * stride
-  uint32_t pending = 0, in_flight = 0;
-  bool quit = false;
-  int error = ETXB_OK;
-  std::string error_text;
-  std::chrono::steady_clock::time_point busy_since;
-  double busy_seconds = 0.0;   // wall time with at least one iteration queued or in flight
-  double last_iteration_seconds = 0.0;
-  DevBuf<float4> combined;
-  int device = 0;
-  // pixel-tile sharding over several processes (etxb_group_comm_init): every lane has its own communicator, and the k-th iteration of lane l is
-  // the ordinal l + k * lanes on EVERY rank (the shared counter of the single-GPU mode would pair different iterations across ranks)
-  bool sharded = false;
-  struct ReplicaItem {
-    uint32_t index;        // ordinal of the iteration within the job
-    uint32_t part, parts;  // parts == 1: the whole frame; else the camera pass of part `part` (tile % parts == part), light pass in full
-  };
-  std::deque<ReplicaItem> whole_queue, split_queue;
-  uint32_t split_lane = 0xffffffffu;  // replicas: the lane reserved for camera-split iterations (etxb_group_reserve_split_lane), or none
-  uint32_t split_part = 0, split_parts = 0;  // the (part, parts) that lane's film is made of; 0 parts = not used yet
-  bool replicas = false;             // etxb_group_comm_init_replicas: whole-frame iterations dealt to the ranks (global index j -> rank j % world), one film reduce
-  uint32_t job_enqueued = 0;         // replicas: iterations enqueued for the whole job
-  uint32_t world = 1, rank = 0;
-  uint32_t enqueued_total = 0;
-  std::vector<uint32_t> lane_next;
-  ncclComm_t reduce_comm = nullptr;  // the frame reduce has its own communicator: the lanes' ones are busy with iterations in flight
-  cudaStream_t stream = nullptr;
-  DevBuf<float4> combined_light, reduced;
-};
-
-// What one rank takes of `iterations` more iterations of a replica-mode job (ordinals base .. base + iterations - 1).  Whole frames are dealt
-// round-robin (ordinal j on rank j % world).  What is left when the count is not a multiple of the ranks would leave some ranks a whole iteration
-// behind the others (20 iterations on 8 ranks: 3, 3, 3, 3, 2, 2, 2, 2): with a split lane those R iterations are split instead, each over
-// P = world / R ranks by camera tile — every part traces the whole light pass itself (same photon map, no exchange) and the camera pass of its
-// tiles; the parts meet in the frame reduce.  A split lane's film is made of ONE (part, parts) geometry: a later round that would need another
-// one is dealt as whole frames.  Returns the parts of this round's split (0: none).
-static uint32_t replica_plan(uint32_t world, uint32_t rank, uint32_t base, uint32_t iterations, bool split_lane, uint32_t have_part, uint32_t have_parts,
-                             std::vector<etxb_group::ReplicaItem>& out) {
-  uint32_t whole = iterations, rest = 0, parts = 1;
-  if ((iterations >= world) && split_lane) {
-    rest = iterations % world;
-    parts = rest ? (world / rest) : 1u;
-    if ((parts >= 2u) && ((have_parts == 0u) || (have_parts == parts))) {
-      whole = iterations - rest;
-    } else {
-      rest = 0;
-    }
-  }
-  for (uint32_t j = base; j < base + whole; ++j)
-    if ((j % world) == rank) out.push_back({j, 0u, 1u});
-  for (uint32_t r = 0; r < rest; ++r) {
-    if ((rank / parts) != r) continue;
-    const uint32_t part = rank % parts;
-    if ((have_parts != 0u) && (have_part != part)) continue;  // cannot happen while `parts` stays the same: a rank's part is rank % parts
-    out.push_back({base + whole + r, part, parts});
-  }
-  return rest ? parts : 0u;
-}
-
-static bool group_has_work(const etxb_group* grp, uint32_t lane) {
-  if (grp->replicas) return (lane == grp->split_lane) ? !grp->split_queue.empty() : !grp->whole_queue.empty();
-  if (lane == grp->split_lane) return false;
-  return grp->sharded ? (grp->lane_next[lane] < grp->enqueued_total) : (grp->pending > 0);
-}
-static bool group_idle(const etxb_group* grp) {
-  if (grp->in_flight > 0) return false;
-  if (grp->replicas) return grp->whole_queue.empty() && grp->split_queue.empty();
-  if (!grp->sharded) return grp->pending == 0;
-  for (uint32_t next : grp->lane_next)
-    if (next < grp->enqueued_total) return false;
-  return true;
-}
-
-static void group_worker(etxb_group* grp, uint32_t lane) {
-  cudaSetDevice(grp->device);
-  etxb_ctx* ctx = grp->lanes[lane];
-  std::unique_lock<std::mutex> lock(grp->m);
-  for (;;) {
-    grp->cv_work.wait(lock, [&] { return grp->quit || group_has_work(grp, lane); });
-    if (grp->quit) return;
-    uint32_t ordinal = 0;
-    etxb_group::ReplicaItem item = {0u, 0u, 1u};
-    if (grp->replicas) {
-      auto& queue = (lane == grp->split_lane) ? grp->split_queue : grp->whole_queue;
-      item = queue.front();
-      queue.pop_front();
-      ordinal = item.index;
-      grp->taken = std::max(grp->taken, ordinal + 1u);
-    } else if (grp->sharded) {
-      ordinal = grp->lane_next[lane];
-      grp->lane_next[lane] += uint32_t(grp->lanes.size());
-      grp->taken = std::max(grp->taken, ordinal + 1u);
-    } else {
-      ordinal = grp->taken++;
-      grp->pending -= 1;
-    }
-    uint32_t iteration = grp->first_iteration + ordinal * grp->stride;
-    grp->in_flight += 1;
-    lock.unlock();
-    if (grp->replicas && (lane == grp->split_lane)) {
-      // this lane renders the camera pass of its part only; the light pass (and so the photon map) in full
-      ctx->rank = item.part;
-      ctx->world = item.parts;
-      ctx->light_full = true;
-    }
-    int rc = etxb_set_next_iteration(ctx, iteration);
-    if (rc == ETXB_OK) rc = run_iteration_blocking(ctx);  // returns when the iteration has finished (the bounce loops read queue sizes back)
-    lock.lock();
-    grp->in_flight -= 1;
-    grp->last_iteration_seconds = ctx->last_iteration_time;
-    if ((rc != ETXB_OK) && (grp->error == ETXB_OK)) {
-      grp->error = rc;
-      grp->error_text = etxb_last_error(ctx);
-      grp->pending = 0;
-      grp->whole_queue.clear();
-      grp->split_queue.clear();
-      for (auto& next : grp->lane_next) next = 0xffffffffu;
-    }
-    if (group_idle(grp)) {
-      grp->busy_seconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - grp->busy_since).count();
-      grp->cv_idle.notify_all();
-    }
-  }
-}
-
+// ---- iterations in flight (etxb_group) ----------------------------------------------------------------------------------------------------
 int etxb_group_create(etxb_group** out, const etxb_device_config* cfg, uint32_t lanes) {
   if (!out || (lanes == 0) || (lanes > kMaxLanes)) return ETXB_ERR_INVALID_ARGUMENT;
   *out = nullptr;
@@ -2743,9 +2647,6 @@ void etxb_group_destroy(etxb_group* grp) {
   grp->cv_work.notify_all();
   for (auto& w : grp->workers) w.join();
   cudaSetDevice(grp->device);
-  grp->combined.release();
-  grp->combined_light.release();
-  grp->reduced.release();
   if (grp->reduce_comm != nullptr) {
     if (NcclApi* n = nccl_api()) n->CommDestroy(grp->reduce_comm);
   }
@@ -2813,7 +2714,7 @@ int etxb_group_update_scene(etxb_group* grp, const void* scene_blob, uint64_t sc
   for (size_t l = 0; l < grp->lanes.size(); ++l) {
     etxb_ctx* c = grp->lanes[l];
     etxb_update_info lane = {};
-    ctx_drain_impl(c);
+    ctx_drain(c);
     if (int rc = commit_scene(c, s, cam, p, c->scene_ready, &lane)) {
       std::lock_guard<std::mutex> lock(grp->m);
       grp->error_text = etxb_last_error(c);
@@ -2886,42 +2787,6 @@ int etxb_group_poll(etxb_group* grp, etxb_status* status) {
   status->last_iteration_time = grp->last_iteration_seconds;
   status->total_time = grp->busy_seconds;
   if (status->iteration_in_flight) status->total_time += std::chrono::duration<double>(std::chrono::steady_clock::now() - grp->busy_since).count();
-  return ETXB_OK;
-}
-
-static int group_combine_into(etxb_group* grp, uint32_t layer, DevBuf<float4>& target, uint32_t* completed, bool raw = false) {
-  etxb_ctx* first = grp->lanes[0];
-  if (!first->scene_ready) return fail(first, ETXB_ERR_NOT_READY, "no scene uploaded");
-  size_t n = first->path_count;
-  cudaSetDevice(grp->device);
-  if (target.count < n) {
-    target.release();
-    CUDA_OK(first, target.alloc(n));
-  }
-  FilmLanes f = {};
-  f.lanes = uint32_t(grp->lanes.size());
-  f.layer = layer;
-  f.pixels = uint32_t(n);
-  uint32_t total = 0;
-  for (auto* c : grp->lanes) total += c->completed;
-  for (uint32_t l = 0; l < f.lanes; ++l) {
-    f.camera[l] = grp->lanes[l]->film_camera.ptr;
-    f.light[l] = grp->lanes[l]->film_light.ptr;
-    f.weight[l] = raw ? float(grp->lanes[l]->completed) : (total ? float(double(grp->lanes[l]->completed) / double(total)) : 0.0f);
-    f.weight_light[l] = f.weight[l];
-    f.weight_count[l] = f.weight[l];
-    if (raw && (l == grp->split_lane) && (grp->split_part != 0u)) {
-      // a camera-split lane that is not part 0: its camera tiles count, its (complete, redundant) light image and its iteration count do not
-      f.weight_light[l] = 0.0f;
-      f.weight_count[l] = 0.0f;
-    }
-  }
-  f.raw = raw ? 1u : 0u;
-  // lanes that are still rendering keep updating their films (a preview, like reading the reference's film while it runs); after
-  // etxb_group_wait every lane has synchronised its stream and the result is exact
-  k_film_combine<<<blocks_for(f.pixels, 256), 256, 0, grp->stream>>>(f, target.ptr);
-  CUDA_OK(first, cudaStreamSynchronize(grp->stream));
-  if (completed) *completed = total;
   return ETXB_OK;
 }
 
@@ -3068,5 +2933,3 @@ int etxb_group_read_film(etxb_group* grp, uint32_t layer, float* dst_rgba, uint6
   CUDA_OK(first, cudaMemcpy(dst_rgba, src, bytes, cudaMemcpyDeviceToHost));
   return ETXB_OK;
 }
-
-}  // extern "C"
