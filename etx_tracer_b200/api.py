@@ -139,6 +139,19 @@ def _p(a):
     return a.ctypes.data_as(C.c_void_p)
 
 
+def _fields(a):
+    """A one-record struct array as a dict: Python scalars, and copies of its array fields."""
+    return {k: (a[k][0].copy() if a[k][0].ndim else a[k][0].item()) for k in a.dtype.names}
+
+
+def _device_config(device, max_light_vertices, profile):
+    cfg = np.zeros(1, dtype=S.DEVICE_CONFIG)
+    cfg["device_index"] = device
+    cfg["max_light_vertices"] = max_light_vertices
+    cfg["flags"] = 1 if profile else 0
+    return cfg
+
+
 def read_image(file_name, flavor="fast"):
     """The module's image readers (PNG in every form, OpenEXR, Radiance HDR, PFM): (H, W, 4) uint8 or float32, rows in file order."""
     lib = load_library(flavor)
@@ -262,11 +275,7 @@ class GPUVCM:
         if _adopt is not None:
             self.h = C.c_void_p(_adopt)  # a lane of an etxb_group: the group owns the context
         else:
-            cfg = np.zeros(1, dtype=S.DEVICE_CONFIG)
-            cfg["device_index"] = device
-            cfg["max_light_vertices"] = max_light_vertices
-            cfg["flags"] = 1 if profile else 0
-            rc = self.lib.etxb_create(C.byref(self.h), _p(cfg))
+            rc = self.lib.etxb_create(C.byref(self.h), _p(_device_config(device, max_light_vertices, profile)))
             if rc != 0:
                 raise EtxbError(rc, "etxb_create failed (no CUDA device? the module has no CPU fallback)")
         self.options = S.default_vcm_options()
@@ -329,7 +338,7 @@ class GPUVCM:
         info = np.zeros(1, dtype=S.UPDATE_INFO)
         self._check(self.lib.etxb_update_scene(self.h, _p(scene_data.scene), scene_data.scene.nbytes, _p(scene_data.camera), scene_data.camera.nbytes, _p(info)))
         self._after_update(scene_data)
-        return {k: info[k][0].item() for k in info.dtype.names}
+        return _fields(info)
 
     def _after_update(self, scene_data):
         self.scene_data = scene_data
@@ -366,22 +375,29 @@ class GPUVCM:
         """This context renders iterations first, first + stride, ... (iteration-interleaved multi-GPU runs)."""
         self._check(self.lib.etxb_set_iteration_stride(self.h, stride))
 
+    def _push_options(self):
+        self._check(self.lib.etxb_set_options(self.h, _p(self.options)))
+
+    def _converged(self, st):
+        """Whether every pixel has converged, which ends the run before scene.samples: never for the VCM."""
+        return False
+
     def run(self, first_iteration=0):
         """CPUVCM::run -> CPUVCMImpl::start: clears the film and arms iteration 0."""
-        self._check(self.lib.etxb_set_options(self.h, _p(self.options)))
+        self._push_options()
         self._check(self.lib.etxb_begin(self.h, first_iteration))
         self._running = True
         self._target_iterations = int(self.scene_data.scene["samples"][0])
 
     def update(self):
         """One pump of the integrator, non-blocking like CPUVCM::update (vcm_cpu.cxx:264-276): queues the next iteration once the previous one has
-        finished; stops at scene.samples like the reference."""
+        finished; stops at scene.samples like the reference, or earlier when _converged() says so."""
         if not self._running:
             return False
         st = self.status()
         if st["iteration_in_flight"]:
             return True
-        if st["completed_iterations"] >= self._target_iterations:
+        if self._converged(st) or (st["completed_iterations"] >= self._target_iterations):
             self._running = False
             return False
         self._check(self.lib.etxb_enqueue_iteration(self.h))
@@ -417,7 +433,7 @@ class GPUVCM:
     def status(self):
         st = np.zeros(1, dtype=S.STATUS)
         self._check(self.lib.etxb_poll(self.h, _p(st)))
-        return {k: st[k][0].item() for k in st.dtype.names}
+        return _fields(st)
 
     # -- results --------------------------------------------------------------------------------------
     def film(self, layer=S.FILM_RESULT, out=None):
@@ -439,7 +455,7 @@ class GPUVCM:
     def counters(self):
         c = np.zeros(1, dtype=S.COUNTERS)
         self._check(self.lib.etxb_get_counters(self.h, _p(c)))
-        return {k: int(c[k][0]) for k in c.dtype.names}
+        return _fields(c)
 
     def kernel_times(self):
         cap = 32
@@ -541,7 +557,7 @@ class GPUVCM:
         out = np.zeros(queries.shape[0], dtype=S.MERGE_RESULT)
         grid = np.zeros(1, dtype=S.MERGE_GRID)
         self._check(self.lib.etxb_debug_merge(self.h, _p(records), records.shape[0], _p(wl), _p(queries), queries.shape[0], _p(out), _p(grid)))
-        return out, {k: (grid[k][0].copy() if grid[k][0].ndim else grid[k][0].item()) for k in grid.dtype.names}
+        return out, _fields(grid)
 
 
 class GPUPathTracing(GPUVCM):
@@ -567,33 +583,18 @@ class GPUPathTracing(GPUVCM):
         """Scene::noise_threshold / radiance_clamp without a new upload."""
         self._check(self.lib.etxb_set_scene_settings(self.h, C.c_float(noise_threshold), C.c_float(radiance_clamp)))
 
-    def run(self, first_iteration=0):
-        """CPUPathTracing::run -> CPUPathTracingImpl::start (path_tracing.cxx:35-48): options, film.clear(ClearCameraData), first task."""
+    def _push_options(self):
+        """The path tracer's options, read by CPUPathTracingImpl::start (path_tracing.cxx:35-48)."""
         self._check(self.lib.etxb_pt_set_options(self.h, _p(self.pt_options)))
-        self._check(self.lib.etxb_begin(self.h, first_iteration))
-        self._running = True
-        self._target_iterations = int(self.scene_data.scene["samples"][0])
 
-    def update(self):
-        """CPUPathTracingImpl::update (path_tracing.cxx:85-110), non-blocking: an iteration that processed no pixel (all converged) ends the run."""
-        if not self._running:
-            return False
-        st = self.status()
-        if st["iteration_in_flight"]:
-            return True
-        if st["completed_iterations"] and (self.pt_status()["pixels_processed"] == 0):
-            self._running = False
-            return False
-        if st["completed_iterations"] >= self._target_iterations:
-            self._running = False
-            return False
-        self._check(self.lib.etxb_enqueue_iteration(self.h))
-        return True
+    def _converged(self, st):
+        """CPUPathTracingImpl::update (path_tracing.cxx:85-110): an iteration that processed no pixel (all converged) ends the run."""
+        return (st["completed_iterations"] > 0) and (self.pt_status()["pixels_processed"] == 0)
 
     def pt_status(self):
         st = np.zeros(1, dtype=S.PT_STATUS)
         self._check(self.lib.etxb_pt_get_status(self.h, _p(st)))
-        return {k: st[k][0].item() for k in st.dtype.names}
+        return _fields(st)
 
 
 class GPUVCMGroup:
@@ -603,11 +604,7 @@ class GPUVCMGroup:
     def __init__(self, scene_data, lanes=4, flavor="fast", device=0, max_light_vertices=0, profile=False):
         self.lib = load_library(flavor)
         self.h = C.c_void_p()
-        cfg = np.zeros(1, dtype=S.DEVICE_CONFIG)
-        cfg["device_index"] = device
-        cfg["max_light_vertices"] = max_light_vertices
-        cfg["flags"] = 1 if profile else 0
-        rc = self.lib.etxb_group_create(C.byref(self.h), _p(cfg), lanes)
+        rc = self.lib.etxb_group_create(C.byref(self.h), _p(_device_config(device, max_light_vertices, profile)), lanes)
         if rc != 0:
             raise EtxbError(rc, "etxb_group_create failed (no CUDA device? the module has no CPU fallback)")
         self.lanes = [GPUVCM(scene_data, flavor=flavor, _adopt=self.lib.etxb_group_lane(self.h, k)) for k in range(lanes)]
@@ -662,7 +659,7 @@ class GPUVCMGroup:
             g._after_update(scene_data)
         self.scene_data = scene_data
         self.width, self.height = self.lanes[0].width, self.lanes[0].height
-        return {k: info[k][0].item() for k in info.dtype.names}
+        return _fields(info)
 
     def comm_init(self, world, rank, comm_ids):
         """Pixel tiles over `world` processes with len(self.lanes) iterations in flight on each: collective; comm_ids = the (lanes + 1) x 128
@@ -714,7 +711,7 @@ class GPUVCMGroup:
     def status(self):
         st = np.zeros(1, dtype=S.STATUS)
         self._check(self.lib.etxb_group_poll(self.h, _p(st)))
-        return {k: st[k][0].item() for k in st.dtype.names}
+        return _fields(st)
 
     def film(self, layer=S.FILM_RESULT, out=None):
         if out is None:
