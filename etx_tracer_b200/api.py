@@ -128,6 +128,7 @@ def load_library(flavor="fast"):
     lib.etxb_debug_sampler.argtypes = [vp, vp, vp, u32, u32, vp, vp]
     lib.etxb_debug_math.argtypes = [vp, u32, vp, vp, u32, vp]
     lib.etxb_debug_closure_eval.argtypes = [vp, vp, u32, u32, vp]
+    lib.etxb_debug_bsdf_sample.argtypes = [vp, vp, u32, u32, vp]
     lib.etxb_debug_set_thresholds.argtypes = [vp, vp]
     lib.etxb_debug_get_branch_counts.argtypes = [vp, vp]
     lib.etxb_debug_merge.argtypes = [vp, vp, u32, vp, vp, u32, vp, vp]
@@ -526,6 +527,14 @@ class GPUVCM:
         queries = np.ascontiguousarray(queries, dtype=S.CLOSURE_QUERY)
         out = np.zeros((queries.shape[0], S.CLOSURE_STATS), dtype=np.float64)
         self._check(self.lib.etxb_debug_closure_eval(self.h, _p(queries), queries.shape[0], int(repetitions), _p(out)))
+        return out
+
+    def debug_bsdf_sample(self, queries, repetitions):
+        """bsdf_sample for S.SAMPLE_QUERY records on the uploaded scene, repetition r of each on the sampler (seed, r); returns
+        S.SAMPLE_RESULT records shaped (n, repetitions), laid out as etxb_debug_bsdf_sample documents (include/etx_b200.h)."""
+        queries = np.ascontiguousarray(queries, dtype=S.SAMPLE_QUERY)
+        out = np.zeros((queries.shape[0], int(repetitions)), dtype=S.SAMPLE_RESULT)
+        self._check(self.lib.etxb_debug_bsdf_sample(self.h, _p(queries), queries.shape[0], int(repetitions), _p(out)))
         return out
 
     def debug_thresholds(self, **fields):

@@ -364,6 +364,8 @@ DEV V3 visible_micronormal(V2 rnd, V3 wi, V2 alpha) {
     const float inv = 1.0f / sin_theta;
     cos_phi = wi_11.x * inv;
     sin_phi = wi_11.y * inv;
+  } else if (signbit(wi_11.x)) {
+    cos_phi = -1.0f;  // at normal incidence the reference rotates by atan2(+-0, -0) = +-pi: a negative zero x turns the slope round
   }
   V2 slope = {cos_phi * slope_11.x - sin_phi * slope_11.y, sin_phi * slope_11.x + cos_phi * slope_11.y};
 #endif
@@ -684,6 +686,11 @@ DEV float vmf_sigma_beckmann_expanded(float u, float m) {
   if (0.0f == m) return (u + fabsf(u)) / 2.0f;
   float m2 = m * m;
   if (1.0f == u) return 1.0f - 0.5f * m2;
+#if !(defined(ETXB_PARITY) && ETXB_PARITY)
+  // u = -1 (a sampled w_o exactly along n: the product build's m_pow rounds sqrt(u) of the largest samples up to 1) is the limit 0 of the
+  // expression below, which evaluates it as inf * 0
+  if (-1.0f == u) return 0.0f;
+#endif
   float expansion_term = -0.25f * m2 * (u + fabsf(u));
   float u2 = u * u;
   return ((m_exp(u2 / (m2 * (-1.0f + u2))) * m * sqrtf(1.0f - u2)) / sqrtf(kPi) + u * (1.0f + erf_buermann(u / (m * sqrtf(1.0f - u2))))) / 2.0f + expansion_term;

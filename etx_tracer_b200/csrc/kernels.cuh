@@ -1892,6 +1892,45 @@ __global__ void k_debug_closure(const __grid_constant__ DeviceScene sc, const et
   for (uint32_t k = 27; k < ETXB_CLOSURE_STATS; ++k) o[k] = 0.0;
 }
 
+// one thread per (etxb_sample_query, repetition): bsdf_sample on the sampler Smp::init(seed, r) with the fixed values a bounce pushes
+// (mode 0, kernels.cuh / dpt.cuh at every bsdf_sample call) or the query's own (mode 1); record layout in include/etx_b200.h
+template <bool SP>
+__global__ void k_debug_bsdf_sample(const __grid_constant__ DeviceScene sc, const etxb_sample_query* queries, uint32_t count, uint32_t reps, etxb_sample_result* out) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= count * reps) return;
+  const uint32_t i = t / reps, r = t % reps;
+  const etxb_sample_query& q = queries[i];
+  const V3 nrm = {q.nrm[0], q.nrm[1], q.nrm[2]}, tan = {q.tan[0], q.tan[1], q.tan[2]}, btn = {q.btn[0], q.btn[1], q.btn[2]};
+  const V3 w_i = {q.w_i[0], q.w_i[1], q.w_i[2]};
+  const BData d = {{0.0f, 0.0f, 0.0f}, nrm, tan, btn, {q.uv[0], q.uv[1]}, w_i, SP ? q.wavelength : -1.0f, q.path_source, q.medium};
+  Smp smp;
+  smp.init(q.seed, r);
+  etxb_sample_result& o = out[t];
+  o.seed_start = smp.seed;
+  if (q.mode == 0u) {
+    const V2 rnd_bsdf = smp.next_2d();
+    smp.next_2d();  // rnd_connection
+    const V2 rnd_support = smp.next_2d();
+    smp.push_fixed(rnd_bsdf.x, rnd_bsdf.y, rnd_support.x);
+  } else {
+    smp.push_fixed(q.fixed[0], q.fixed[1], q.fixed[2]);
+  }
+  const BSample<SP> s = bsdf_sample<SP>(sc, d, sc.materials[q.material], smp);
+  smp.pop_fixed();
+  const V3 w = s.weight.as_v3();
+  o.w_o[0] = s.w_o.x;
+  o.w_o[1] = s.w_o.y;
+  o.w_o[2] = s.w_o.z;
+  o.pdf = s.pdf;
+  o.weight[0] = w.x;
+  o.weight[1] = w.y;
+  o.weight[2] = w.z;
+  o.eta = s.eta;
+  o.properties = s.properties;
+  o.medium_index = s.medium_index;
+  o.seed_end = smp.seed;
+}
+
 // etxb_debug_merge: query i becomes path i of a one-bounce queue, staged in the columns the gather kernels read (hit record, ray
 // direction, throughput, MIS terms, sampler, depth, medium, wavelength), with the merge key k_camera_shade would give it.  Writes the
 // staged camera vertex's position and normal to pos_nrm[2 i], [2 i + 1], and i to queue slot i.

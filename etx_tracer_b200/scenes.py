@@ -130,8 +130,9 @@ class SceneData:
             m["scattering"]["spectrum_index"] = self.add_spectrum(spd_rgb_reflectance(kd))
         if ks is not None:
             m["reflectance"]["spectrum_index"] = self.add_spectrum(spd_rgb_reflectance(ks))
-        r2 = f32(roughness) * f32(roughness)  # "Pr" is squared by the loader (scene_representation.cxx:1731-1738)
-        m["roughness"]["value"][0][:2] = r2
+        # "Pr u" or "Pr u v", each axis squared by the loader (scene_representation.cxx:1731-1738); a scalar sets both axes
+        ru, rv = (roughness, roughness) if np.isscalar(roughness) else roughness
+        m["roughness"]["value"][0][:2] = (f32(ru) * f32(ru), f32(rv) * f32(rv))
         m["metalness"]["value"][0][:] = metalness
         m["transmission"]["value"][0][:] = transmission
         if emission is not None:
@@ -761,6 +762,10 @@ MATERIAL_KINDS = {
     "sss_refracted": dict(cls=S.MAT_PLASTIC, kd=[0.7, 0.8, 0.6], ks=[1.0, 1.0, 1.0], roughness=0.3, int_ior="plastic",
                           subsurface=dict(cls="random_walk", path="refracted", distances=[0.3, 0.6, 1.0], scale=0.1)),
     "sss_burley": dict(kd=[0.9, 0.5, 0.4], subsurface=dict(cls="burley", distances=[1.0, 0.3, 0.1], scale=0.08)),
+    # anisotropic roughness ("Pr u v"): the microsurface walk with alpha_x != alpha_y
+    "conductor_aniso": dict(cls=S.MAT_CONDUCTOR, ks=[1.0, 1.0, 1.0], roughness=(0.15, 0.6), int_ior="gold"),
+    "dielectric_aniso": dict(cls=S.MAT_DIELECTRIC, roughness=(0.5, 0.1), int_ior="glass"),
+    "plastic_aniso": dict(cls=S.MAT_PLASTIC, kd=[0.3, 0.5, 0.7], ks=[1.0, 1.0, 1.0], roughness=(0.2, 0.65), int_ior="plastic"),
 }
 
 

@@ -112,6 +112,15 @@ CLOSURE_QUERY = np.dtype([
     ("material", u4), ("path_source", u4), ("seed", u4), ("reserved", u4, 3),
 ])
 CLOSURE_STATS = 32
+# etxb_sample_query (96 B) and the per-sample record etxb_debug_bsdf_sample / oracle_bsdf_sample return (include/etx_b200.h)
+SAMPLE_QUERY = np.dtype([
+    ("nrm", f4, 3), ("tan", f4, 3), ("btn", f4, 3), ("w_i", f4, 3), ("uv", f4, 2), ("wavelength", f4),
+    ("material", u4), ("path_source", u4), ("seed", u4), ("medium", u4), ("mode", u4), ("fixed", f4, 3), ("reserved", u4),
+])
+SAMPLE_RESULT = np.dtype([("w_o", f4, 3), ("pdf", f4), ("weight", f4, 3), ("eta", f4), ("properties", u4), ("medium_index", u4),
+                          ("seed_start", u4), ("seed_end", u4)])
+SAMPLE_BOUNCE, SAMPLE_GIVEN = 0, 1
+BSDF_DIFFUSE, BSDF_REFLECTION, BSDF_TRANSMISSION, BSDF_MEDIUM_CHANGED, BSDF_DELTA = 1, 2, 4, 8, 16
 # etxb_debug_thresholds / etxb_debug_branch_counts (include/etx_b200.h): a threshold of 0 always takes the large-queue branch, NEVER never does
 DEBUG_THRESHOLDS = np.dtype([("merge_sort_min_queries", u4), ("merge_min_warps_per_sm", u4), ("tail_queue", u4), ("sort_queue_min", u4), ("merge_qpw", u4)])
 DEFAULT_THRESHOLDS = {"merge_sort_min_queries": 16384, "merge_min_warps_per_sm": 32, "tail_queue": 8192, "sort_queue_min": 1024, "merge_qpw": 0}
@@ -133,6 +142,7 @@ EXPECTED_SIZES = {
     "VERTEX": (VERTEX, 56), "TRIANGLE": (TRIANGLE, 32), "MATERIAL": (MATERIAL, 200), "EMITTER_PROFILE": (EMITTER_PROFILE, 48),
     "EMITTER": (EMITTER, 32), "SPECTRUM": (SPECTRUM, 3552), "DISTRIBUTION": (DISTRIBUTION, 32), "IMAGE": (IMAGE, 112),
     "MEDIUM": (MEDIUM, 80), "CAMERA": (CAMERA, 176), "SCENE": (SCENE, 528), "CLOSURE_QUERY": (CLOSURE_QUERY, 96),
+    "SAMPLE_QUERY": (SAMPLE_QUERY, 96), "SAMPLE_RESULT": (SAMPLE_RESULT, 48),
     "LIGHT_VERTEX_REC": (LIGHT_VERTEX_REC, 96), "MERGE_QUERY": (MERGE_QUERY, 64), "MERGE_RESULT": (MERGE_RESULT, 48), "MERGE_GRID": (MERGE_GRID, 64),
 }
 for _name, (_dt, _size) in EXPECTED_SIZES.items():

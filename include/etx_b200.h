@@ -510,6 +510,34 @@ typedef struct etxb_closure_query {
  * [24] the number of repetitions with a non-finite output, [25] with pdf < 0 or rev_pdf < 0, [26] with pdf == 0 but a non-zero func or bsdf. */
 #define ETXB_CLOSURE_STATS 32
 int etxb_debug_closure_eval(etxb_ctx* ctx, const etxb_closure_query* queries, uint32_t count, uint32_t repetitions, double* out);
+/* BSDF sampling query (dbsdf.cuh bsdf_sample, as every bounce of the light pass, the camera pass and the path tracer calls it) on the
+ * uploaded scene.  One query is 96 bytes: the shading frame as interpolated, w_i pointing AT the surface, uv, the wavelength (ignored in
+ * RGB scenes), the material index, the path source (1 = camera, 2 = light), a sampler seed, the current medium (what Boundary and Void
+ * return), the mode and three fixed values.  Repetition r starts from the sampler Smp::init(seed, r) (= the reference's Sampler(seed, r)):
+ *   mode 0 ("bounce")  draws rnd_bsdf, rnd_connection, rnd_support with next_2d() and pushes (rnd_bsdf.x, rnd_bsdf.y, rnd_support.x)
+ *                      as the fixed values, as a bounce does (vcm_shared.hxx:1013-1025)
+ *   mode 1 ("given")   pushes fixed[0..3) as they are
+ * then bsdf_sample and pop_fixed. */
+typedef struct etxb_sample_query {
+  float nrm[3], tan[3], btn[3];
+  float w_i[3];
+  float uv[2];
+  float wavelength;
+  uint32_t material, path_source, seed, medium, mode;
+  float fixed[3];
+  uint32_t reserved;
+} etxb_sample_query;
+/* One 48-byte record per (query, repetition), repetition-minor: w_o, pdf, weight (rgb; a spectral value fills all three), eta, properties
+ * (BSDFSample::Properties), medium_index, the sampler state Smp::init(seed, r) left and the state after pop_fixed (their distance in the
+ * stream is the number of draws the sample made). */
+typedef struct etxb_sample_result {
+  float w_o[3];
+  float pdf;
+  float weight[3];
+  float eta;
+  uint32_t properties, medium_index, seed_start, seed_end;
+} etxb_sample_result;
+int etxb_debug_bsdf_sample(etxb_ctx* ctx, const etxb_sample_query* queries, uint32_t count, uint32_t repetitions, etxb_sample_result* out);
 /* Queue sizes from which the light and camera passes take their large-queue branches.  A pass of a long queue runs the same paths as
  * one of a short queue, in another order; these let a small film take either branch.  Each field is a queue size: 0 = always the
  * large-queue branch, 0xffffffff = never.

@@ -46,6 +46,8 @@ def load(flavor="parity"):
     lib.oracle_bvh_info.argtypes = [vp, C.POINTER(u32), C.POINTER(u32)]
     if hasattr(lib, "oracle_bsdf_eval"):  # an oracle/_ref built before this export still serves every other test
         lib.oracle_bsdf_eval.argtypes = [vp, vp, u32, u32, u32, vp]
+    if hasattr(lib, "oracle_bsdf_sample"):
+        lib.oracle_bsdf_sample.argtypes = [vp, vp, u32, u32, u32, vp]
     if hasattr(lib, "oracle_merge"):
         lib.oracle_merge.argtypes = [vp, vp, u32, vp, vp, u32, u32, u32, vp, vp]
     lib.oracle_sampler.argtypes = [vp, vp, u32, u32, vp, vp]
@@ -72,6 +74,11 @@ def load(flavor="parity"):
 def has_bsdf_eval(flavor="parity"):
     """Whether the built oracle exports oracle_bsdf_eval (oracle/_ref is older than the export where the reference could not rebuild it)."""
     return hasattr(load(flavor), "oracle_bsdf_eval")
+
+
+def has_bsdf_sample(flavor="parity"):
+    """Whether the built oracle exports oracle_bsdf_sample."""
+    return hasattr(load(flavor), "oracle_bsdf_sample")
 
 
 def has_merge(flavor="parity"):
@@ -249,6 +256,14 @@ class Oracle:
         queries = np.ascontiguousarray(queries, dtype=self.S.CLOSURE_QUERY)
         out = np.zeros((queries.shape[0], self.S.CLOSURE_STATS), dtype=np.float64)
         self.lib.oracle_bsdf_eval(self.h, _p(queries), queries.shape[0], int(repetitions), int(threads or os.cpu_count() or 1), _p(out))
+        return out
+
+    def bsdf_sample(self, queries, repetitions, threads=None):
+        """The reference's bsdf::sample for S.SAMPLE_QUERY records, repetition r of each on Sampler(seed, r); S.SAMPLE_RESULT records
+        shaped (n, repetitions), in the layout of GPUVCM.debug_bsdf_sample."""
+        queries = np.ascontiguousarray(queries, dtype=self.S.SAMPLE_QUERY)
+        out = np.zeros((queries.shape[0], int(repetitions)), dtype=self.S.SAMPLE_RESULT)
+        self.lib.oracle_bsdf_sample(self.h, _p(queries), queries.shape[0], int(repetitions), int(threads or os.cpu_count() or 1), _p(out))
         return out
 
     def merge(self, records, light_wavelengths, queries, repetitions=1, threads=None):

@@ -1115,6 +1115,54 @@ void oracle_bsdf_eval(void* h, const etxb_closure_query* queries, uint32_t count
   });
 }
 
+// The reference's own bsdf::sample for etxb_sample_query records (include/etx_b200.h), with the fixed values a bounce pushes
+// (vcm_shared.hxx:1013-1027: rnd_bsdf, rnd_connection, rnd_support, push_fixed, sample, pop_fixed) in mode 0 or the query's own in
+// mode 1.  One etxb_sample_result per (query, repetition r), repetition r on Sampler(seed, r), as etxb_debug_bsdf_sample writes them.
+static_assert(sizeof(etxb_sample_query) == 96);
+static_assert(sizeof(etxb_sample_result) == 48);
+void oracle_bsdf_sample(void* h, const etxb_sample_query* queries, uint32_t count, uint32_t repetitions, uint32_t threads, etxb_sample_result* out) {
+  auto* o = static_cast<Oracle*>(h);
+  const Scene& scene = o->scene;
+  parallel_ranges(count * repetitions, threads, [&](uint32_t begin, uint32_t end, uint32_t, uint32_t) {
+    for (uint32_t t = begin; t < end; ++t) {
+      const etxb_sample_query& q = queries[t / repetitions];
+      Vertex v = {};
+      v.nrm = {q.nrm[0], q.nrm[1], q.nrm[2]};
+      v.tan = {q.tan[0], q.tan[1], q.tan[2]};
+      v.btn = {q.btn[0], q.btn[1], q.btn[2]};
+      v.tex = {q.uv[0], q.uv[1]};
+      const float3 w_i = {q.w_i[0], q.w_i[1], q.w_i[2]};
+      const SpectralQuery spect = scene.spectral() ? SpectralQuery{q.wavelength, SpectralQuery::Spectral} : SpectralQuery::sample();
+      const BSDFData data(spect, q.medium, static_cast<PathSource>(q.path_source), v, w_i);
+      Sampler smp(q.seed, t % repetitions);
+      etxb_sample_result& dst = out[t];
+      dst.seed_start = smp.seed;
+      if (q.mode == 0u) {
+        const float2 rnd_bsdf = smp.next_2d();
+        smp.next_2d();  // rnd_connection
+        const float2 rnd_support = smp.next_2d();
+        smp.push_fixed(rnd_bsdf.x, rnd_bsdf.y, rnd_support.x);
+      } else {
+        smp.push_fixed(q.fixed[0], q.fixed[1], q.fixed[2]);
+      }
+      const BSDFSample s = bsdf::sample(data, scene.materials[q.material], scene, smp);
+      smp.pop_fixed();
+      const float3 w = s.weight.spectral() ? float3{s.weight.value, s.weight.value, s.weight.value} : s.weight.integrated;
+      dst.w_o[0] = s.w_o.x;
+      dst.w_o[1] = s.w_o.y;
+      dst.w_o[2] = s.w_o.z;
+      dst.pdf = s.pdf;
+      dst.weight[0] = w.x;
+      dst.weight[1] = w.y;
+      dst.weight[2] = w.z;
+      dst.eta = s.eta;
+      dst.properties = s.properties;
+      dst.medium_index = s.medium_index;
+      dst.seed_end = smp.seed;
+    }
+  });
+}
+
 // The reference's own photon gather (VCMSpatialGridData::gather, vcm_shared.hxx:886-924) for etxb_debug_merge's inputs: the light-vertex
 // records (device layout, 96 B) become o.light_vertices and build_grid runs on them at the current iteration; each query becomes the
 // Intersection make_intersection builds for its hit (as oracle_trace does) and a VCMPathState, and is gathered `repetitions` times on
