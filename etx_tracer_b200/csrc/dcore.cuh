@@ -214,7 +214,14 @@ struct Smp {
   }
   DEV void init(uint32_t a, uint32_t b) {
     seed = random_seed(a, b);
-    fixed_u = fixed_v = fixed_w = 0.0f;
+    pop_fixed();
+  }
+  // a stream continued from a seed stored between kernels (fixed values are never stored: a path holds none between bounces)
+  DEV static Smp resume(uint32_t seed) {
+    Smp s;
+    s.seed = seed;
+    s.pop_fixed();
+    return s;
   }
   DEV float next() {
     seed = (seed ^ 61u) ^ (seed >> 16u);
@@ -237,6 +244,21 @@ struct Smp {
   DEV void pop_fixed() { fixed_u = fixed_v = fixed_w = 0.0f; }
   DEV bool has_fixed() const { return (sqr(fixed_u) + sqr(fixed_v) + sqr(fixed_w)) > kEpsilon; }
 };
+
+// Streams the product build derives from a camera vertex's seed, each past its first draw.  The vertex-connection stage and the closure
+// gather prepare the same vertex closure only because both take it from closure_prep_stream.
+// the closure preparation of the camera vertex (RGB thin-film wavelength jitter)
+DEV Smp closure_prep_stream(uint32_t seed) {
+  Smp s = Smp::resume(seed ^ 0x85ebca6bu);
+  s.next();
+  return s;
+}
+// the evaluation of one (camera vertex, light vertex or photon) pair; `ordinal` numbers the light vertex within its path, or the photon
+DEV Smp pair_stream(uint32_t seed, uint32_t ordinal) {
+  Smp s = Smp::resume(seed ^ ((ordinal + 1u) * 0x9E3779B1u));
+  s.next();
+  return s;
+}
 
 // ---- spectral value: one float in spectral mode, three in RGB mode (spectrum.hxx:242-374) --------------
 // SpectralResponse keeps {value, integrated}; only `value` is observable in spectral mode and only

@@ -72,6 +72,19 @@ DEV HitRec trace_closest(const DeviceScene& sc, V3 o, V3 d, float tmin, float tm
   return vis.best;
 }
 
+// The segment set-up of every shadow query (rt.cxx:468-490): false for a degenerate segment, whose squared length is at most kRayEpsilon
+// (it counts as unoccluded, :474-477); otherwise the unit direction from p0 and the distance to stop at, short of p1 by
+// max(kRayEpsilon, length * kRayEpsilon) so that the surface at p1 is not hit.
+DEV bool shadow_segment(V3 p0, V3 p1, V3& direction, float& t_max) {
+  direction = p1 - p0;
+  t_max = dot(direction, direction);
+  if (t_max <= kRayEpsilon) return false;
+  t_max = sqrtf(t_max);
+  direction /= t_max;
+  t_max -= fmaxf(kRayEpsilon, t_max * kRayEpsilon);
+  return true;
+}
+
 struct Crossing {
   uint32_t primitive_id;
   float u, v, t;
@@ -115,12 +128,9 @@ struct OcclusionVisitor {
   }
 };
 DEV bool trace_occluded(const DeviceScene& sc, V3 p0, V3 p1) {
-  V3 direction = p1 - p0;
-  float t_max = dot(direction, direction);
-  if (t_max <= kRayEpsilon) return false;
-  t_max = sqrtf(t_max);
-  direction /= t_max;
-  t_max -= fmaxf(kRayEpsilon, t_max * kRayEpsilon);
+  V3 direction;
+  float t_max;
+  if (!shadow_segment(p0, p1, direction, t_max)) return false;
   OcclusionVisitor vis{sc, false};
   DevNodeLoad nl{sc.bvh_nodes};
   DevTriLoad tl{sc.bvh_tris};
@@ -145,12 +155,9 @@ struct PlainShadowVisitor {
 // PLAIN: compile-time promise that the scene has no Boundary surfaces, media or subsurface materials (DeviceScene flags, checked by the host).
 template <bool SP, bool PLAIN = false>
 DEVN Spec<SP> trace_transmittance(const DeviceScene& sc, float wavelength, V3 p0, V3 p1, uint32_t medium_index, Smp& smp, TraverseStats* stats) {
-  V3 direction = p1 - p0;
-  float t_max = dot(direction, direction);
-  if (t_max <= kRayEpsilon) return Spec<SP>::make(1.0f);
-  t_max = sqrtf(t_max);
-  direction /= t_max;
-  t_max -= fmaxf(kRayEpsilon, t_max * kRayEpsilon);
+  V3 direction;
+  float t_max;
+  if (!shadow_segment(p0, p1, direction, t_max)) return Spec<SP>::make(1.0f);
   if constexpr (PLAIN) {
     // scenes without Boundary surfaces and media: the first candidate that passes the alpha test occludes — no crossing list, no media walk
     PlainShadowVisitor pvis{sc, smp, false};

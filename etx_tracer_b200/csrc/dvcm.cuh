@@ -949,6 +949,17 @@ DEV uint32_t grid_position_to_index(V3 pos, V3 bbox_min, float cell_size, uint32
   V3 m = vfloor((pos - bbox_min) / cell_size);
   return grid_cell_index(mask, static_cast<int32_t>(m.x), static_cast<int32_t>(m.y), static_cast<int32_t>(m.z));
 }
+// Cell `c` (0..7) of the eight a gather at `pos` visits (vcm_shared.hxx:895-916): the cell of `pos`, stepped along x / y / z where bit 0 / 1 / 2
+// of `c` is set, towards the neighbour on the nearer side.
+DEV uint32_t grid_gather_cell(const GridData& g, V3 pos, uint32_t c) {
+  V3 m = (pos - g.bbox_min) / g.cell_size;
+  V3 mf = vfloor(m);
+  V3 md = m - mf;
+  int32_t cx = static_cast<int32_t>(mf.x) + ((c & 1u) ? ((md.x < 0.5f) ? -1 : +1) : 0);
+  int32_t cy = static_cast<int32_t>(mf.y) + ((c & 2u) ? ((md.y < 0.5f) ? -1 : +1) : 0);
+  int32_t cz = static_cast<int32_t>(mf.z) + ((c & 4u) ? ((md.z < 0.5f) ? -1 : +1) : 0);
+  return grid_cell_index(g.hash_table_mask, cx, cy, cz);
+}
 
 template <bool SP>
 DEV V3 grid_gather(const DeviceScene& sc, const GridData& g, const VcmParams& it, const Isect& isect, PathState<SP>& state, uint32_t& candidates, uint32_t& accepts) {
@@ -957,13 +968,6 @@ DEV V3 grid_gather(const DeviceScene& sc, const GridData& g, const VcmParams& it
   V3 pos = isect.pos;
   if (!((pos.x >= g.bbox_min.x) && (pos.y >= g.bbox_min.y) && (pos.z >= g.bbox_min.z) && (pos.x <= g.bbox_max.x) && (pos.y <= g.bbox_max.y) && (pos.z <= g.bbox_max.z)))
     return merged;
-  V3 m = (pos - g.bbox_min) / g.cell_size;
-  V3 mf = vfloor(m);
-  V3 md = m - mf;
-  int32_t acx = static_cast<int32_t>(mf.x), acy = static_cast<int32_t>(mf.y), acz = static_cast<int32_t>(mf.z);
-  int32_t bcx = acx + ((md.x < 0.5f) ? -1 : +1);
-  int32_t bcy = acy + ((md.y < 0.5f) ? -1 : +1);
-  int32_t bcz = acz + ((md.z < 0.5f) ? -1 : +1);
 
   const etxb_material& mat = sc.materials[isect.material_index];
   BData camera_data = make_bdata(isect, isect.w_i, state.wavelength, state.medium_index, kPathCamera);
@@ -973,8 +977,7 @@ DEV V3 grid_gather(const DeviceScene& sc, const GridData& g, const VcmParams& it
 
 #pragma unroll 1
   for (uint32_t c = 0; c < 8; ++c) {
-    uint32_t cell = grid_cell_index(g.hash_table_mask, (c & 1u) ? bcx : acx, (c & 2u) ? bcy : acy, (c & 4u) ? bcz : acz);
-    uint2 range = __ldg(&g.cell_range[cell]);
+    uint2 range = __ldg(&g.cell_range[grid_gather_cell(g, pos, c)]);
     V3 cell_merged = {0.0f, 0.0f, 0.0f};
     for (uint32_t j = range.x; j < range.y; ++j) {
       float4 pd = __ldg(&g.pos_dvcm[j]);

@@ -156,4 +156,38 @@ DEV void wide_begin(WideWalk& w, V3 o, V3 d, float t0, float t1) {
   w.sp = 0;
 }
 
+// One ray through the whole tree (global memory, nothing staged); n_nodes / n_tris count the nodes and triangles it tested.
+template <class Visitor>
+DEV void wide_trace(const DeviceScene& sc, V3 o, V3 d, float tmin, float tmax, Visitor& visit, uint32_t& n_nodes, uint32_t& n_tris) {
+  const WideNodes nodes{nullptr, sc.wide_nodes, 0u};
+  WideWalk walk;
+  WideHit stack[kWideStackSize];
+  wide_begin(walk, o, d, tmin, tmax);
+  while (!wide_step(walk, stack, nodes, sc.bvh_tris, visit, n_nodes, n_tris)) {
+  }
+}
+
+// The candidate test of a closest-hit query (Raytracing::trace, rt.cxx:428-466): Void surfaces and alpha-rejected hits are skipped, any
+// other candidate becomes the closest hit so far.
+struct ClosestHitVisitor {
+  const DeviceScene& sc;
+  Smp* smp;
+  HitRec* best;
+  DEV int operator()(uint32_t triangle_index, float u, float v, float t) {
+    const etxb_material& mat = sc.materials[load_triangle_material(sc, triangle_index)];
+    if (mat.cls == ETXB_MAT_VOID) return kCandIgnore;
+    if (alpha_test_rejects(sc, mat, triangle_index, u, v, *smp)) return kCandIgnore;
+    *best = {u, v, t, triangle_index};
+    return kCandAccept;
+  }
+};
+
+// The closest hit of one ray (tri = kInvalidIndex: none), drawing from `smp` once per alpha-tested candidate.
+DEV HitRec trace_closest_wide(const DeviceScene& sc, V3 o, V3 d, float tmin, float tmax, Smp& smp, uint32_t& n_nodes, uint32_t& n_tris) {
+  HitRec best = {0.0f, 0.0f, 0.0f, kInvalidIndex};
+  ClosestHitVisitor visit{sc, &smp, &best};
+  wide_trace(sc, o, d, tmin, tmax, visit, n_nodes, n_tris);
+  return best;
+}
+
 }  // namespace etxb

@@ -170,8 +170,7 @@ DEV PathState<SP> load_state(const PathBuffers& b, uint32_t i) {
   s.d_vc = m.y;
   s.d_vm = m.z;
   s.eta = m.w;
-  s.sampler.seed = u.x;
-  s.sampler.fixed_u = s.sampler.fixed_v = s.sampler.fixed_w = 0.0f;
+  s.sampler = Smp::resume(u.x);
   s.total_path_depth = u.y;
   s.medium_index = u.z;
   s.flags = u.w;
@@ -220,9 +219,7 @@ __global__ void __launch_bounds__(256) k_trace_closest(const __grid_constant__ L
   uint32_t i = queue[q];
   float4 o = p.paths.ray_o[i], d = p.paths.ray_d[i];
   uint4 misc = p.paths.misc[i];
-  Smp smp;
-  smp.seed = misc.x;
-  smp.fixed_u = smp.fixed_v = smp.fixed_w = 0.0f;
+  Smp smp = Smp::resume(misc.x);
   STATS_DECL;
   HitRec h = trace_closest(p.scene, {o.x, o.y, o.z}, {d.x, d.y, d.z}, o.w, d.w, smp, stats);
   p.paths.hit[i] = make_float4(h.u, h.v, h.t, __uint_as_float(h.tri));
@@ -672,10 +669,7 @@ DEV void camera_emit_connections(const LaunchParams& p, uint32_t i, const Isect&
       *p.overflow = 1u;
     }
     ConnRec<SP>& rec = *conn_rec_at<SP>(p.paths.conn_rec, i);
-    Smp prep;  // the closure's own stream (RGB thin-film wavelength jitter), as in k_camera_merge_closure
-    prep.seed = state.sampler.seed ^ 0x85ebca6bu;
-    prep.fixed_u = prep.fixed_v = prep.fixed_w = 0.0f;
-    prep.next();
+    Smp prep = closure_prep_stream(state.sampler.seed);
     BData cam = make_bdata(isect, isect.w_i, state.wavelength, state.medium_index, kPathCamera);
     rec.closure = make_closure<SP>(sc, cam, isect.material_index, prep);
     rec.pos = isect.pos;
@@ -980,10 +974,7 @@ __global__ void __launch_bounds__(128, kBounceMinBlocksPerSm<PLAIN>) k_camera_co
     uint2 entry = conn_list[t];
     uint32_t i = entry.x;
     const ConnRec<SP>& cam = *conn_rec_at<SP>(p.paths.conn_rec, i);
-    Smp smp;
-    smp.seed = cam.seed ^ ((entry.y + 1u) * 0x9E3779B1u);
-    smp.fixed_u = smp.fixed_v = smp.fixed_w = 0.0f;
-    smp.next();
+    Smp smp = pair_stream(cam.seed, entry.y);
     LightVertexRec lv = load_light_vertex(p.lv_final + cam.lp_offset + entry.y);
     V3 target_position;
     Spec<SP> value;
@@ -1079,14 +1070,94 @@ __global__ void __launch_bounds__(128) k_camera_merge_serial(const __grid_consta
   counter_add(&p.counters->merge_accepts, accepts);
 }
 
-// Warp-cooperative Lambert gather (product build).  Input: the queue sorted by merge_query_key.  One query at a time is
-// broadcast to the warp; the eight cell ranges are concatenated into one virtual range that the 32 lanes sweep with coalesced
-// 16-B position loads; photons inside the radius are compacted (ballot + prefix) into a per-warp shared list and finished 32 at
-// a time with all lanes busy (normal / path-length / cosine tests, MIS weight, kernel); partial sums meet in a shuffle reduction.
 constexpr uint32_t kMergeWarpsPerBlock = 8;
 constexpr uint32_t kMergeListSize = 64;
 
-// Lambert camera vertices only: the BSDF value is independent of the photon direction and the sampler is not used.
+// The sweep both warp gathers share: the photons of the eight cells around `bpos`, the position of the query broadcast from lane `src`, that lie
+// inside the radius are appended to the warp's pair list (kMergeListSize entries per column: photon, squared distance, d_vcm, and with SRC the
+// query's lane).  Whenever 32 pairs are listed, finish(32) consumes the first 32 and the rest moves to the front.  `n_list` (warp-uniform) carries
+// over between calls; the caller consumes what is left.
+template <bool SRC, class Finish>
+DEV void merge_sweep(const GridData& g, V3 bpos, uint32_t src, uint32_t* s_idx, float* s_d2, float* s_dvcm, uint32_t* s_src, uint32_t& n_list,
+                     uint32_t& candidates, Finish& finish) {
+  constexpr uint32_t kFull = 0xffffffffu;
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t lane_lt = (1u << lane) - 1u;
+  // lanes 0..7 fetch the ranges of the eight cells, then an 8-wide exclusive scan of the counts concatenates them into one virtual range
+  // (prefetching the next query's ranges and the next 32 candidate positions was measured: no gain, the sweep is L2-bandwidth bound)
+  uint32_t my_begin = 0, my_cnt = 0;
+  if (lane < 8u) {
+    uint2 r = __ldg(&g.cell_range[grid_gather_cell(g, bpos, lane)]);
+    my_begin = r.x;
+    my_cnt = r.y - r.x;
+  }
+  uint32_t incl = my_cnt;
+#pragma unroll
+  for (uint32_t o = 1; o < 8u; o <<= 1) {
+    uint32_t v = __shfl_up_sync(kFull, incl, o);
+    if (lane >= o) incl += v;
+  }
+  uint32_t my_excl = incl - my_cnt;
+  const uint32_t total = __shfl_sync(kFull, incl, 7);
+  uint32_t e1 = __shfl_sync(kFull, my_excl, 1), e2 = __shfl_sync(kFull, my_excl, 2), e3 = __shfl_sync(kFull, my_excl, 3), e4 = __shfl_sync(kFull, my_excl, 4),
+           e5 = __shfl_sync(kFull, my_excl, 5), e6 = __shfl_sync(kFull, my_excl, 6), e7 = __shfl_sync(kFull, my_excl, 7);
+  // the 32 lanes sweep the virtual range with coalesced 16-B position loads; photons inside the radius are compacted (ballot + prefix)
+  for (uint32_t base = 0; base < total; base += 32u) {
+    uint32_t k = base + lane;
+    bool valid = k < total;
+    uint32_t c = uint32_t(k >= e1) + uint32_t(k >= e2) + uint32_t(k >= e3) + uint32_t(k >= e4) + uint32_t(k >= e5) + uint32_t(k >= e6) + uint32_t(k >= e7);
+    uint32_t cb = __shfl_sync(kFull, my_begin, c);
+    uint32_t ce = __shfl_sync(kFull, my_excl, c);
+    uint32_t j = cb + (k - ce);
+    bool inside = false;
+    float distance_squared = 0.0f, dvcm = 0.0f;
+    if (valid) {
+      float4 pd = __ldg(&g.pos_dvcm[j]);
+      V3 d = V3{pd.x, pd.y, pd.z} - bpos;
+      distance_squared = dot(d, d);
+      dvcm = pd.w;
+      inside = !(distance_squared > g.radius_squared);
+      candidates += 1;
+    }
+    uint32_t bal = __ballot_sync(kFull, inside);
+    if (inside) {
+      uint32_t slot = n_list + __popc(bal & lane_lt);
+      s_idx[slot] = j;
+      s_d2[slot] = distance_squared;
+      s_dvcm[slot] = dvcm;
+      if constexpr (SRC) s_src[slot] = src;
+    }
+    n_list += __popc(bal);
+    __syncwarp();
+    if (n_list >= 32u) {
+      finish(32u);
+      __syncwarp();
+      uint32_t rest = n_list - 32u;  // < 32: move the tail to the front
+      uint32_t tj = 0, ts = 0;
+      float td = 0.0f, tv = 0.0f;
+      if (lane < rest) {
+        tj = s_idx[32u + lane];
+        td = s_d2[32u + lane];
+        tv = s_dvcm[32u + lane];
+        if constexpr (SRC) ts = s_src[32u + lane];
+      }
+      __syncwarp();
+      if (lane < rest) {
+        s_idx[lane] = tj;
+        s_d2[lane] = td;
+        s_dvcm[lane] = tv;
+        if constexpr (SRC) s_src[lane] = ts;
+      }
+      n_list = rest;
+      __syncwarp();
+    }
+  }
+}
+
+// Warp-cooperative Lambert gather (product build).  Input: the queue sorted by merge_query_key.  The queries of a warp are broadcast one at a
+// time; their pairs are finished 32 at a time with all lanes busy (normal / path-length / cosine tests, MIS weight, kernel), and the partial sums
+// of a query meet in a shuffle reduction.  Lambert camera vertices only: the BSDF value is independent of the photon direction and the sampler is
+// not used.
 template <bool SP>
 __global__ void __launch_bounds__(kMergeWarpsPerBlock * 32) k_camera_merge_coop(const __grid_constant__ LaunchParams p, const uint32_t* sorted_ids, const uint32_t* sorted_keys, const uint32_t* count_in,
                                                                                 uint32_t queries_per_warp) {
@@ -1096,7 +1167,6 @@ __global__ void __launch_bounds__(kMergeWarpsPerBlock * 32) k_camera_merge_coop(
   const DeviceScene& sc = p.scene;
   const GridData& g = p.grid;
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-  const uint32_t lane_lt = (1u << lane) - 1u;
   // A warp works through its queries one after the other, so a query's latency is paid `queries_per_warp` times per warp: 32 when the
   // queue is long (every lane brings one query), fewer when it is short (the tail of the pass), so that the queries spread over more warps.
   uint32_t q = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * queries_per_warp + lane;
@@ -1144,32 +1214,6 @@ __global__ void __launch_bounds__(kMergeWarpsPerBlock * 32) k_camera_merge_coop(
     float b_dvm = __shfl_sync(0xffffffffu, q_dvm, src);
     float b_rev_cos = __shfl_sync(0xffffffffu, q_rev_cos, src);
     uint32_t b_depth = __shfl_sync(0xffffffffu, q_depth, src);
-    // the eight cells (vcm_shared.hxx:895-916): lanes 0..7 fetch their ranges, then an 8-wide exclusive scan of the counts
-    // (prefetching the next query's ranges and the next 32 candidate positions was measured: no gain, the sweep is L2-bandwidth bound)
-    uint32_t my_begin = 0, my_cnt = 0;
-    if (lane < 8u) {
-      V3 m = (bpos - g.bbox_min) / g.cell_size;
-      V3 mf = vfloor(m);
-      V3 md = m - mf;
-      int32_t acx = static_cast<int32_t>(mf.x), acy = static_cast<int32_t>(mf.y), acz = static_cast<int32_t>(mf.z);
-      int32_t cx = (lane & 1u) ? acx + ((md.x < 0.5f) ? -1 : +1) : acx;
-      int32_t cy = (lane & 2u) ? acy + ((md.y < 0.5f) ? -1 : +1) : acy;
-      int32_t cz = (lane & 4u) ? acz + ((md.z < 0.5f) ? -1 : +1) : acz;
-      uint2 r = __ldg(&g.cell_range[grid_cell_index(g.hash_table_mask, cx, cy, cz)]);
-      my_begin = r.x;
-      my_cnt = r.y - r.x;
-    }
-    uint32_t incl = my_cnt;
-#pragma unroll
-    for (uint32_t o = 1; o < 8u; o <<= 1) {
-      uint32_t v = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += v;
-    }
-    uint32_t my_excl = incl - my_cnt;
-    const uint32_t total = __shfl_sync(0xffffffffu, incl, 7);
-    uint32_t e1 = __shfl_sync(0xffffffffu, my_excl, 1), e2 = __shfl_sync(0xffffffffu, my_excl, 2), e3 = __shfl_sync(0xffffffffu, my_excl, 3),
-             e4 = __shfl_sync(0xffffffffu, my_excl, 4), e5 = __shfl_sync(0xffffffffu, my_excl, 5), e6 = __shfl_sync(0xffffffffu, my_excl, 6),
-             e7 = __shfl_sync(0xffffffffu, my_excl, 7);
     float wx = 0.0f, wy = 0.0f, wz = 0.0f;  // per-lane partial sums
     uint32_t n_list = 0;                    // warp-uniform fill of the shared list
 
@@ -1202,54 +1246,7 @@ __global__ void __launch_bounds__(kMergeWarpsPerBlock * 32) k_camera_merge_coop(
         }
       }
     };
-
-    for (uint32_t base = 0; base < total; base += 32u) {
-      uint32_t k = base + lane;
-      bool valid = k < total;
-      uint32_t c = uint32_t(k >= e1) + uint32_t(k >= e2) + uint32_t(k >= e3) + uint32_t(k >= e4) + uint32_t(k >= e5) + uint32_t(k >= e6) + uint32_t(k >= e7);
-      uint32_t cb = __shfl_sync(0xffffffffu, my_begin, c);
-      uint32_t ce = __shfl_sync(0xffffffffu, my_excl, c);
-      uint32_t j = cb + (k - ce);
-      bool inside = false;
-      float distance_squared = 0.0f, dvcm = 0.0f;
-      if (valid) {
-        float4 pd = __ldg(&g.pos_dvcm[j]);
-        V3 d = V3{pd.x, pd.y, pd.z} - bpos;
-        distance_squared = dot(d, d);
-        dvcm = pd.w;
-        inside = !(distance_squared > g.radius_squared);
-        candidates += 1;
-      }
-      uint32_t bal = __ballot_sync(0xffffffffu, inside);
-      if (inside) {
-        uint32_t slot = n_list + __popc(bal & lane_lt);
-        s_idx[warp][slot] = j;
-        s_d2[warp][slot] = distance_squared;
-        s_dvcm[warp][slot] = dvcm;
-      }
-      n_list += __popc(bal);
-      __syncwarp();
-      if (n_list >= 32u) {
-        finish(32u);
-        __syncwarp();
-        uint32_t rest = n_list - 32u;  // < 32: move the tail to the front
-        uint32_t tj = 0;
-        float td = 0.0f, tv = 0.0f;
-        if (lane < rest) {
-          tj = s_idx[warp][32u + lane];
-          td = s_d2[warp][32u + lane];
-          tv = s_dvcm[warp][32u + lane];
-        }
-        __syncwarp();
-        if (lane < rest) {
-          s_idx[warp][lane] = tj;
-          s_d2[warp][lane] = td;
-          s_dvcm[warp][lane] = tv;
-        }
-        n_list = rest;
-        __syncwarp();
-      }
-    }
+    merge_sweep<false>(g, bpos, src, s_idx[warp], s_d2[warp], s_dvcm[warp], nullptr, n_list, candidates, finish);
     if (n_list) finish(n_list);
     __syncwarp();
 #pragma unroll
@@ -1298,7 +1295,6 @@ __global__ void __launch_bounds__(kClosureWarpsPerBlock * 32, kMinBlocksPerSm) k
   const DeviceScene& sc = p.scene;
   const GridData& g = p.grid;
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-  const uint32_t lane_lt = (1u << lane) - 1u;
   uint32_t q = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * queries_per_warp + lane;
   uint32_t merge_queries = 0, candidates = 0, accepts = 0;
   bool active = (lane < queries_per_warp) && (q < *count_in) && (sorted_keys[q] != 0xffffffffu);
@@ -1324,10 +1320,7 @@ __global__ void __launch_bounds__(kClosureWarpsPerBlock * 32, kMinBlocksPerSm) k
       aux.seed = state.sampler.seed;
       state.sampler.next();  // the path's own stream moves on by one draw per query
       p.paths.misc[i].x = state.sampler.seed;
-      Smp prep;  // the closure's own stream (RGB thin-film wavelength jitter)
-      prep.seed = aux.seed ^ 0x85ebca6bu;
-      prep.fixed_u = prep.fixed_v = prep.fixed_w = 0.0f;
-      prep.next();
+      Smp prep = closure_prep_stream(aux.seed);
       BData cam = make_bdata(isect, isect.w_i, state.wavelength, state.medium_index, kPathCamera);
       s_cl[warp][lane] = make_closure<SP>(sc, cam, isect.material_index, prep);
       s_aux[warp][lane] = aux;
@@ -1354,10 +1347,7 @@ __global__ void __launch_bounds__(kClosureWarpsPerBlock * 32, kMinBlocksPerSm) k
       bool ok = !(__float_as_uint(wl.w) + aux.depth + 1 > sc.max_path_length);
       ok = ok && !(dot(c.nrm, V3{nd.x, nd.y, nd.z}) <= kEpsilon);
       if (ok) {
-        Smp lane_smp;
-        lane_smp.seed = aux.seed ^ ((j + 1u) * 0x9E3779B1u);
-        lane_smp.fixed_u = lane_smp.fixed_v = lane_smp.fixed_w = 0.0f;
-        lane_smp.next();
+        Smp lane_smp = pair_stream(aux.seed, j);
         CEval<SP> e = closure_evaluate<SP>(sc, c, V3{-wl.x, -wl.y, -wl.z}, lane_smp);
         if (e.valid()) {
           float4 lt = __ldg(&g.thr_rgb[j]);
@@ -1380,80 +1370,7 @@ __global__ void __launch_bounds__(kClosureWarpsPerBlock * 32, kMinBlocksPerSm) k
     uint32_t src = __ffs(pending) - 1u;
     pending &= pending - 1u;
     V3 bpos = {__shfl_sync(kFull, qpos.x, src), __shfl_sync(kFull, qpos.y, src), __shfl_sync(kFull, qpos.z, src)};
-    // the eight cells (vcm_shared.hxx:895-916): lanes 0..7 fetch their ranges, then an 8-wide exclusive scan of the counts
-    uint32_t my_begin = 0, my_cnt = 0;
-    if (lane < 8u) {
-      V3 m = (bpos - g.bbox_min) / g.cell_size;
-      V3 mf = vfloor(m);
-      V3 md = m - mf;
-      int32_t acx = static_cast<int32_t>(mf.x), acy = static_cast<int32_t>(mf.y), acz = static_cast<int32_t>(mf.z);
-      int32_t cx = (lane & 1u) ? acx + ((md.x < 0.5f) ? -1 : +1) : acx;
-      int32_t cy = (lane & 2u) ? acy + ((md.y < 0.5f) ? -1 : +1) : acy;
-      int32_t cz = (lane & 4u) ? acz + ((md.z < 0.5f) ? -1 : +1) : acz;
-      uint2 r = __ldg(&g.cell_range[grid_cell_index(g.hash_table_mask, cx, cy, cz)]);
-      my_begin = r.x;
-      my_cnt = r.y - r.x;
-    }
-    uint32_t incl = my_cnt;
-#pragma unroll
-    for (uint32_t o = 1; o < 8u; o <<= 1) {
-      uint32_t v = __shfl_up_sync(kFull, incl, o);
-      if (lane >= o) incl += v;
-    }
-    uint32_t my_excl = incl - my_cnt;
-    const uint32_t total = __shfl_sync(kFull, incl, 7);
-    uint32_t e1 = __shfl_sync(kFull, my_excl, 1), e2 = __shfl_sync(kFull, my_excl, 2), e3 = __shfl_sync(kFull, my_excl, 3), e4 = __shfl_sync(kFull, my_excl, 4),
-             e5 = __shfl_sync(kFull, my_excl, 5), e6 = __shfl_sync(kFull, my_excl, 6), e7 = __shfl_sync(kFull, my_excl, 7);
-    for (uint32_t base = 0; base < total; base += 32u) {
-      uint32_t k = base + lane;
-      bool valid = k < total;
-      uint32_t c = uint32_t(k >= e1) + uint32_t(k >= e2) + uint32_t(k >= e3) + uint32_t(k >= e4) + uint32_t(k >= e5) + uint32_t(k >= e6) + uint32_t(k >= e7);
-      uint32_t cb = __shfl_sync(kFull, my_begin, c);
-      uint32_t ce = __shfl_sync(kFull, my_excl, c);
-      uint32_t j = cb + (k - ce);
-      bool inside = false;
-      float distance_squared = 0.0f, dvcm = 0.0f;
-      if (valid) {
-        float4 pd = __ldg(&g.pos_dvcm[j]);
-        V3 d = V3{pd.x, pd.y, pd.z} - bpos;
-        distance_squared = dot(d, d);
-        dvcm = pd.w;
-        inside = !(distance_squared > g.radius_squared);
-        candidates += 1;
-      }
-      uint32_t bal = __ballot_sync(kFull, inside);
-      if (inside) {
-        uint32_t slot = n_list + __popc(bal & lane_lt);
-        s_idx[warp][slot] = j;
-        s_d2[warp][slot] = distance_squared;
-        s_dvcm[warp][slot] = dvcm;
-        s_src[warp][slot] = src;
-      }
-      n_list += __popc(bal);
-      __syncwarp();
-      if (n_list >= 32u) {
-        finish(32u);
-        __syncwarp();
-        uint32_t rest = n_list - 32u;  // < 32: move the tail to the front
-        uint32_t tj = 0, ts = 0;
-        float td = 0.0f, tv = 0.0f;
-        if (lane < rest) {
-          tj = s_idx[warp][32u + lane];
-          td = s_d2[warp][32u + lane];
-          tv = s_dvcm[warp][32u + lane];
-          ts = s_src[warp][32u + lane];
-        }
-        __syncwarp();
-        if (lane < rest) {
-          s_idx[warp][lane] = tj;
-          s_d2[warp][lane] = td;
-          s_dvcm[warp][lane] = tv;
-          s_src[warp][lane] = ts;
-        }
-        n_list = rest;
-        __syncwarp();
-      }
-    }
+    merge_sweep<true>(g, bpos, src, s_idx[warp], s_d2[warp], s_dvcm[warp], s_src[warp], n_list, candidates, finish);
   }
   if (n_list) finish(n_list);
   __syncwarp();
@@ -1472,21 +1389,6 @@ __global__ void __launch_bounds__(kClosureWarpsPerBlock * 32, kMinBlocksPerSm) k
 // staging their own copy took 128 KB away from the L1 that caches the rest of the tree: ncu, L1 hit rate 64 % -> 46 %, and the kernel got slower).
 constexpr uint32_t kTraversalBlock = 1024u;
 
-// The candidate test of a closest-hit query (Raytracing::trace, rt.cxx:428-466) for the tree walks of dtrav.cuh / dwide.cuh: Void surfaces and
-// alpha-rejected hits are skipped, any other candidate becomes the closest hit so far.
-struct ClosestHitVisitor {
-  const DeviceScene& sc;
-  Smp* smp;
-  HitRec* best;
-  DEV int operator()(uint32_t triangle_index, float u, float v, float t) {
-    const etxb_material& mat = sc.materials[load_triangle_material(sc, triangle_index)];
-    if (mat.cls == ETXB_MAT_VOID) return kCandIgnore;
-    if (alpha_test_rejects(sc, mat, triangle_index, u, v, *smp)) return kCandIgnore;
-    *best = {u, v, t, triangle_index};
-    return kCandAccept;
-  }
-};
-
 // Closest hit through the 4-wide quantised tree (dwide.cuh), one ray per thread: the product build's kernel for scenes with stochastic BSDFs.
 __global__ void __launch_bounds__(256) k_trace_closest_wide(const __grid_constant__ LaunchParams p, const uint32_t* queue, const uint32_t* queue_count, uint32_t* material_keys,
                                                             uint32_t key_limit) {
@@ -1497,18 +1399,9 @@ __global__ void __launch_bounds__(256) k_trace_closest_wide(const __grid_constan
   }
   uint32_t i = queue[q];
   float4 o = p.paths.ray_o[i], d = p.paths.ray_d[i];
-  Smp smp;
-  smp.seed = p.paths.misc[i].x;
-  smp.fixed_u = smp.fixed_v = smp.fixed_w = 0.0f;
-  HitRec best = {0.0f, 0.0f, 0.0f, kInvalidIndex};
-  ClosestHitVisitor visit{p.scene, &smp, &best};
-  const WideNodes nodes{nullptr, p.scene.wide_nodes, 0u};
-  WideWalk walk;
-  WideHit stack[kWideStackSize];
+  Smp smp = Smp::resume(p.paths.misc[i].x);
   uint32_t n_nodes = 0, n_tris = 0;
-  wide_begin(walk, {o.x, o.y, o.z}, {d.x, d.y, d.z}, o.w, d.w);
-  while (!wide_step(walk, stack, nodes, p.scene.bvh_tris, visit, n_nodes, n_tris)) {
-  }
+  const HitRec best = trace_closest_wide(p.scene, {o.x, o.y, o.z}, {d.x, d.y, d.z}, o.w, d.w, smp, n_nodes, n_tris);
   p.paths.hit[i] = make_float4(best.u, best.v, best.t, __uint_as_float(best.tri));
   p.paths.misc[i].x = smp.seed;
   if (material_keys != nullptr) material_keys[q] = queue_sort_key(p.scene, best.tri);
@@ -1564,14 +1457,11 @@ __global__ void __launch_bounds__(kTraversalBlock) k_shadow_resolve(const __grid
       k = next;
       float4 a = p.shadow_p0[k], b = p.shadow_p1[k];
       target = reinterpret_cast<const uint32_t*>(p.shadow_p1 + k)[3];  // raw bits (see ShadowBatch::push_rgb)
-      V3 direction = V3{b.x, b.y, b.z} - V3{a.x, a.y, a.z};
-      float t_max = dot(direction, direction);
-      if (t_max <= kRayEpsilon) {
-        contribute(k, target);  // a degenerate segment is unoccluded (rt.cxx:474-477)
+      V3 direction;
+      float t_max;
+      if (!shadow_segment({a.x, a.y, a.z}, {b.x, b.y, b.z}, direction, t_max)) {
+        contribute(k, target);  // a degenerate segment is unoccluded
       } else {
-        t_max = sqrtf(t_max);
-        direction /= t_max;
-        t_max -= fmaxf(kRayEpsilon, t_max * kRayEpsilon);
         if constexpr (WIDE) {
           wide_begin(wide_walk, {a.x, a.y, a.z}, direction, kRayEpsilon, t_max);
         } else {
@@ -1732,39 +1622,17 @@ __global__ void __launch_bounds__(256) k_film_resolve(const __grid_constant__ Fi
 // ---------------------------------------------------------------------------------------------------------------------
 // debug / known-answer kernels
 // ---------------------------------------------------------------------------------------------------------------------
-__global__ void k_debug_trace(const __grid_constant__ DeviceScene sc, const float* rays, uint32_t* seeds, uint32_t count, float* hits_uv_t, uint32_t* hits_tri) {
+// closest hits of rays (origin, tmin, direction, tmax: 8 floats each), as k_trace_closest finds them; through the 4-wide quantised tree, as
+// k_trace_closest_wide finds them, when `wide` (product build, scenes that have one)
+__global__ void k_debug_trace(const __grid_constant__ DeviceScene sc, const float* rays, uint32_t* seeds, uint32_t count, uint32_t wide, float* hits_uv_t,
+                              uint32_t* hits_tri) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= count) return;
   const float* r = rays + size_t(i) * 8;
-  Smp smp;
-  smp.seed = seeds[i];
-  smp.fixed_u = smp.fixed_v = smp.fixed_w = 0.0f;
-  HitRec h = trace_closest(sc, {r[0], r[1], r[2]}, {r[4], r[5], r[6]}, r[3], r[7], smp, nullptr);
-  seeds[i] = smp.seed;
-  hits_tri[i] = h.tri;
-  bool hit = h.tri != kInvalidIndex;
-  hits_uv_t[size_t(i) * 3 + 0] = hit ? h.u : 0.0f;
-  hits_uv_t[size_t(i) * 3 + 1] = hit ? h.v : 0.0f;
-  hits_uv_t[size_t(i) * 3 + 2] = hit ? h.t : 0.0f;
-}
-
-// the same query through the 4-wide quantised tree (product build, scenes that have one): the walk k_trace_closest_wide runs (dwide.cuh)
-__global__ void k_debug_trace_wide(const __grid_constant__ DeviceScene sc, const float* rays, uint32_t* seeds, uint32_t count, float* hits_uv_t, uint32_t* hits_tri) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= count) return;
-  const float* r = rays + size_t(i) * 8;
-  Smp smp;
-  smp.seed = seeds[i];
-  smp.fixed_u = smp.fixed_v = smp.fixed_w = 0.0f;
-  HitRec h = {0.0f, 0.0f, 0.0f, kInvalidIndex};
-  ClosestHitVisitor visit{sc, &smp, &h};
-  const WideNodes nodes{nullptr, sc.wide_nodes, 0u};
-  WideWalk walk;
-  WideHit stack[kWideStackSize];
+  const V3 o = {r[0], r[1], r[2]}, d = {r[4], r[5], r[6]};
+  Smp smp = Smp::resume(seeds[i]);
   uint32_t n_nodes = 0, n_tris = 0;
-  wide_begin(walk, {r[0], r[1], r[2]}, {r[4], r[5], r[6]}, r[3], r[7]);
-  while (!wide_step(walk, stack, nodes, sc.bvh_tris, visit, n_nodes, n_tris)) {
-  }
+  const HitRec h = wide ? trace_closest_wide(sc, o, d, r[3], r[7], smp, n_nodes, n_tris) : trace_closest(sc, o, d, r[3], r[7], smp, nullptr);
   seeds[i] = smp.seed;
   hits_tri[i] = h.tri;
   bool hit = h.tri != kInvalidIndex;
@@ -1784,23 +1652,15 @@ __global__ void k_debug_occluded(const __grid_constant__ DeviceScene sc, const f
     occluded[i] = trace_occluded(sc, p0, p1) ? 1u : 0u;
     return;
   }
-  V3 direction = p1 - p0;
-  float t_max = dot(direction, direction);
-  if (t_max <= kRayEpsilon) {
-    occluded[i] = 0u;  // a degenerate segment is unoccluded (rt.cxx:474-477)
+  V3 direction;
+  float t_max;
+  if (!shadow_segment(p0, p1, direction, t_max)) {
+    occluded[i] = 0u;  // a degenerate segment is unoccluded
     return;
   }
-  t_max = sqrtf(t_max);
-  direction /= t_max;
-  t_max -= fmaxf(kRayEpsilon, t_max * kRayEpsilon);
   OcclusionVisitor visit{sc, false};
-  const WideNodes nodes{nullptr, sc.wide_nodes, 0u};
-  WideWalk walk;
-  WideHit stack[kWideStackSize];
   uint32_t n_nodes = 0, n_tris = 0;
-  wide_begin(walk, p0, direction, kRayEpsilon, t_max);
-  while (!wide_step(walk, stack, nodes, sc.bvh_tris, visit, n_nodes, n_tris)) {
-  }
+  wide_trace(sc, p0, direction, kRayEpsilon, t_max, visit, n_nodes, n_tris);
   occluded[i] = visit.occluded ? 1u : 0u;
 }
 

@@ -49,8 +49,7 @@ DEV PtState<SP> pt_load(const PathBuffers& b, uint32_t i) {
   s.sampled_bsdf_pdf = t.w;
   s.accumulated = Spec<SP>::make3({a.x, a.y, a.z});
   s.eta = b.mis[i].x;
-  s.smp.seed = u.x;
-  s.smp.fixed_u = s.smp.fixed_v = s.smp.fixed_w = 0.0f;
+  s.smp = Smp::resume(u.x);
   s.path_length = u.y;
   s.medium = u.z;
   s.mis_weight = (u.w & 1u) != 0u;

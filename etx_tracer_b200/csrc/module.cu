@@ -55,7 +55,7 @@ enum KernelId : uint32_t {
   K_QUEUE_SORT,
   K_CAMERA_MERGE_SORT,
   K_CAMERA_MERGE,
-  K_CAMERA_MERGE_SERIAL,
+  K_CAMERA_MERGE_GENERIC,
   K_CAMERA_CONTINUE,
   K_FILM_COMMIT,
   K_COMM_LIGHT_IMAGE,
@@ -782,7 +782,7 @@ int run_grid_build(etxb_ctx* ctx, const LightVertexRec* records, uint32_t count)
 template <bool SP>
 int launch_merge(etxb_ctx* ctx, const LaunchParams& p, const uint32_t* q, const uint32_t* count, uint32_t active) {
 #if defined(ETXB_PARITY) && ETXB_PARITY
-  LaunchTimer t(ctx, K_CAMERA_MERGE_SERIAL);
+  LaunchTimer t(ctx, K_CAMERA_MERGE_GENERIC);
   k_camera_merge_serial<SP><<<blocks_for(active, 128), 128, 0, ctx->stream>>>(p, q, count);
   ctx->branch_counts.merge_launches[0] += 1;
 #else
@@ -811,7 +811,7 @@ int launch_merge(etxb_ctx* ctx, const LaunchParams& p, const uint32_t* q, const 
     k_camera_merge_coop<SP><<<merge_blocks, kMergeWarpsPerBlock * 32, 0, ctx->stream>>>(p, ids, keys, count, qpw);
   }
   if (ctx->has_stochastic_merge) {
-    LaunchTimer t(ctx, K_CAMERA_MERGE_SERIAL);
+    LaunchTimer t(ctx, K_CAMERA_MERGE_GENERIC);
     const uint32_t closure_blocks = blocks_for(blocks_for(active, qpw), kClosureWarpsPerBlock);
     k_camera_merge_closure<SP><<<closure_blocks, kClosureWarpsPerBlock * 32, 0, ctx->stream>>>(p, ids, keys, count, qpw);
   }
@@ -2433,11 +2433,8 @@ int etxb_debug_trace(etxb_ctx* ctx, const float* rays, uint32_t* seeds, uint32_t
   if (int rc = upload(ctx, d_seeds, seeds, count)) return rc;
   CUDA_OK(ctx, d_uvt.alloc(size_t(count) * 3));
   CUDA_OK(ctx, d_tri.alloc(count));
-  if (ctx->debug_trace_wide && (ctx->dscene.wide_nodes != nullptr)) {
-    k_debug_trace_wide<<<blocks_for(count, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_rays.ptr, d_seeds.ptr, count, d_uvt.ptr, d_tri.ptr);
-  } else {
-    k_debug_trace<<<blocks_for(count, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_rays.ptr, d_seeds.ptr, count, d_uvt.ptr, d_tri.ptr);
-  }
+  const uint32_t wide = (ctx->debug_trace_wide && (ctx->dscene.wide_nodes != nullptr)) ? 1u : 0u;
+  k_debug_trace<<<blocks_for(count, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_rays.ptr, d_seeds.ptr, count, wide, d_uvt.ptr, d_tri.ptr);
   ctx->kernel_launches += 1;
   CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
   CUDA_OK(ctx, cudaMemcpy(seeds, d_seeds.ptr, size_t(count) * 4, cudaMemcpyDeviceToHost));

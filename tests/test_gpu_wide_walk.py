@@ -1,8 +1,9 @@
 """The product build's walk of the 4-wide quantised tree (dwide.cuh) against an independent answer: seeded closest-hit and occlusion queries on
 BASELINE config 3's million-triangle room, every ray against EVERY triangle in float64 (no BVH, no shared code).  Closest hits go through
-etxb_debug_trace (k_debug_trace_wide), occlusion queries through etxb_debug_occluded (k_debug_occluded), both running wide_step, the walk of
-k_trace_closest_wide and k_shadow_resolve<true>.  Rays include axis-aligned directions and directions with one zero component, where the
-reciprocal guard of wide_begin matters; the occlusion queries also run through the BVH2 walks of both builds."""
+etxb_debug_trace (k_debug_trace with `wide`), which calls trace_closest_wide as k_trace_closest_wide does; occlusion queries go through
+etxb_debug_occluded (k_debug_occluded), which sets its segments up with shadow_segment as k_shadow_resolve does and walks them with wide_step,
+the walk of k_shadow_resolve<true>.  Rays include axis-aligned directions and directions with one zero component, where the reciprocal guard
+of wide_begin matters; the occlusion queries also run through the BVH2 walks of both builds."""
 import ctypes as C
 
 import numpy as np
