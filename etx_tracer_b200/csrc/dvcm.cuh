@@ -220,11 +220,10 @@ DEV EmitterSample<SP> sample_emission(const DeviceScene& sc, float wavelength, S
     float pdf_image = 0.0f;
     F4v image_value;
     V2 uv = image_sample(img, smp.next_2d(), pdf_image, image_value);
-    if (pdf_image == 0.0f) {
-      r.pdf_dir = 0.0f;
-      r.triangle_index = kInvalidIndex;
-      r.is_delta = false;
-      r.is_distant = true;
+    if (pdf_image == 0.0f) {  // the reference returns a default EmitterSample (:272-274); its caller stops at pdf_dir == 0
+      r.pdf_sample = r.pdf_dir = 0.0f;
+      r.emitter_index = r.triangle_index = kInvalidIndex;
+      r.is_delta = r.is_distant = false;
       r.origin = r.normal = r.direction = {0.0f, 0.0f, 0.0f};
       return r;
     }
@@ -298,7 +297,7 @@ DEV EmitterSample<SP> sample_emitter(const DeviceScene& sc, float wavelength, ui
   r.emitter_index = emitter_index;
   r.triangle_index = em_inst.triangle_index;
   r.is_delta = em_inst.cls == kEmitterDirectional;
-  r.is_distant = em_inst.cls != kEmitterArea;
+  r.is_distant = false;  // the reference's sample_emitter leaves it at its default (:216-224); no connection reads it
   return r;
 }
 

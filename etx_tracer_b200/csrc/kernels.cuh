@@ -1791,6 +1791,59 @@ __global__ void k_debug_bsdf_sample(const __grid_constant__ DeviceScene sc, cons
   o.seed_end = smp.seed;
 }
 
+// one thread per (etxb_emitter_query, repetition): the emitter routines of dvcm.cuh as the passes call them; ops and record layout in
+// include/etx_b200.h
+static_assert(sizeof(etxb_emitter_query) == 80u && sizeof(etxb_emitter_result) == 104u, "etxb_emitter_query / etxb_emitter_result layout");
+template <bool SP>
+__global__ void k_debug_emitter(const __grid_constant__ DeviceScene sc, const etxb_emitter_query* queries, uint32_t count, uint32_t reps, etxb_emitter_result* out) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= count * reps) return;
+  const uint32_t i = t / reps, r = t % reps;
+  const etxb_emitter_query& q = queries[i];
+  const float wavelength = SP ? q.wavelength : -1.0f;
+  const V3 source = {q.source[0], q.source[1], q.source[2]};
+  etxb_emitter_result o = {};
+  EmitterSample<SP> s = {};
+  s.value = Spec<SP>::make(0.0f);
+  s.emitter_index = s.triangle_index = s.medium_index = kInvalidIndex;
+  if (q.op == ETXB_EMITTER_SELECT) {
+    s.emitter_index = distribution_sample(sc.emitter_dist, sc.emitter_count + 1u, q.rnd[0]);
+    s.pdf_sample = emitter_discrete_pdf(sc, sc.emitters[s.emitter_index]);
+  } else if (q.op == ETXB_EMITTER_SAMPLE_IN) {
+    s = sample_emitter<SP>(sc, wavelength, q.emitter, {q.rnd[0], q.rnd[1]}, source);
+  } else if (q.op == ETXB_EMITTER_EMISSION) {
+    Smp smp;
+    smp.init(q.seed, r);
+    o.seed_start = smp.seed;
+    s = sample_emission<SP>(sc, wavelength, smp);
+    o.seed_end = smp.seed;
+  } else {
+    const V3 target = {q.target[0], q.target[1], q.target[2]}, direction = {q.direction[0], q.direction[1], q.direction[2]};
+    s.emitter_index = q.emitter;
+    s.value = emitter_get_radiance<SP>(sc, sc.emitters[q.emitter], wavelength, source, target, direction, {q.uv[0], q.uv[1]}, q.directly_visible != 0u, s.pdf_area,
+      s.pdf_dir, s.pdf_dir_out);
+  }
+  const auto put = [](float* dst, V3 a) {
+    dst[0] = a.x;
+    dst[1] = a.y;
+    dst[2] = a.z;
+  };
+  put(o.value, s.value.as_v3());
+  put(o.origin, s.origin);
+  put(o.normal, s.normal);
+  put(o.direction, s.direction);
+  put(o.barycentric, s.barycentric);
+  o.pdf_sample = s.pdf_sample;
+  o.pdf_area = s.pdf_area;
+  o.pdf_dir = s.pdf_dir;
+  o.pdf_dir_out = s.pdf_dir_out;
+  o.emitter_index = s.emitter_index;
+  o.triangle_index = s.triangle_index;
+  o.medium_index = s.medium_index;
+  o.flags = (s.is_delta ? 1u : 0u) | (s.is_distant ? 2u : 0u);
+  out[t] = o;
+}
+
 // etxb_debug_merge: query i becomes path i of a one-bounce queue, staged in the columns the gather kernels read (hit record, ray
 // direction, throughput, MIS terms, sampler, depth, medium, wavelength), with the merge key k_camera_shade would give it.  Writes the
 // staged camera vertex's position and normal to pos_nrm[2 i], [2 i + 1], and i to queue slot i.

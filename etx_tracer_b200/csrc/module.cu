@@ -2553,6 +2553,36 @@ int etxb_debug_bsdf_sample(etxb_ctx* ctx, const etxb_sample_query* queries, uint
   return ETXB_OK;
 }
 
+// Test hook: the emitter routines of dvcm.cuh, query by query and repetition by repetition (layout and ops in include/etx_b200.h)
+int etxb_debug_emitter(etxb_ctx* ctx, const etxb_emitter_query* queries, uint32_t count, uint32_t repetitions, etxb_emitter_result* out) {
+  if (!ctx || !queries || !out || (repetitions == 0)) return ETXB_ERR_INVALID_ARGUMENT;
+  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
+  if (count == 0) return ETXB_OK;
+  if (uint64_t(count) * repetitions > 0x7fffffffull) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "%u queries x %u repetitions exceed 2^31 samples", count, repetitions);
+  if (ctx->emitters.count == 0) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "the scene has no emitter");
+  for (uint32_t i = 0; i < count; ++i) {
+    if (queries[i].op > ETXB_EMITTER_RADIANCE) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "emitter query %u: op must be 0 to 3", i);
+    const bool indexed = (queries[i].op == ETXB_EMITTER_SAMPLE_IN) || (queries[i].op == ETXB_EMITTER_RADIANCE);
+    if (indexed && (queries[i].emitter >= ctx->emitters.count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "emitter query %u: emitter index out of range", i);
+  }
+  cudaSetDevice(ctx->device);
+  const uint32_t total = count * repetitions;
+  DevBuf<etxb_emitter_query> d_queries;
+  DevBuf<etxb_emitter_result> d_out;
+  if (int rc = upload(ctx, d_queries, queries, count)) return rc;
+  CUDA_OK(ctx, d_out.alloc(total));
+  if (ctx->spectral) {
+    k_debug_emitter<true><<<blocks_for(total, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
+  } else {
+    k_debug_emitter<false><<<blocks_for(total, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
+  }
+  ctx->kernel_launches += 1;
+  CUDA_OK(ctx, cudaGetLastError());
+  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+  CUDA_OK(ctx, cudaMemcpy(out, d_out.ptr, d_out.bytes(), cudaMemcpyDeviceToHost));
+  return ETXB_OK;
+}
+
 // Test hook: the queue sizes from which the passes take their large-queue branches (NULL = the defaults), and what ran since etxb_begin
 int etxb_debug_set_thresholds(etxb_ctx* ctx, const etxb_debug_thresholds* thresholds) {
   if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;

@@ -188,6 +188,7 @@ class SceneData:
         img["format"] = 2 if u8 else 1
         img["data_size"] = store.nbytes if u8 else px.nbytes
         keep = [px, store]
+        table = None
         if build_table:
             # Image::read at texel centres = mean of the 2x2 neighbourhood (image.hxx:173-186)
             xs1 = (np.arange(w) + 1) % w if repeat else np.minimum(np.arange(w) + 1, w - 1)
@@ -224,6 +225,7 @@ class SceneData:
                 row_values[y] = f32(lum[y].astype(np.float64).sum()) * f32(1.0 if uniform_table else math.sin(v * math.pi))
             ey, total_y = build(row_values)
             keep += [rows, ey]
+            table = (np.stack(keep[2:2 + h]), ey)
             img["x_distributions"]["a"] = rows.ctypes.data
             img["x_distributions"]["count"] = h
             img["y_distribution"]["values"]["a"] = ey.ctypes.data
@@ -237,6 +239,9 @@ class SceneData:
             self._image_px = {}
         self._images.append(img)
         self._image_px[len(self._images) - 1] = px  # the pixels as Image::pixel() returns them (float4)
+        if not hasattr(self, "_image_tables"):
+            self._image_tables = {}
+        self._image_tables[len(self._images) - 1] = table  # (h, w + 1) row entries and the h + 1 row-selection entries, or None
         return len(self._images) - 1
 
     def image_evaluate(self, index, uv):
@@ -303,14 +308,15 @@ class SceneData:
             self._distant_emitters = []
         self._distant_emitters.append((p, e))
 
-    def add_directional_emitter(self, direction, rgb, angular_size_deg=0.0):
-        """et::dir (finite angular size allowed); equivalent_disk_size / angular_size_cosine as build_emitters_distribution (:2463-2466)."""
+    def add_directional_emitter(self, direction, rgb, angular_size_deg=0.0, image_index=S.INVALID):
+        """et::dir (finite angular size allowed, optionally an image over its disk); equivalent_disk_size / angular_size_cosine as
+        build_emitters_distribution (:2463-2466)."""
         d = np.asarray(direction, dtype=f32)
         d = (d / f32(math.sqrt(float(np.dot(d, d))))).astype(f32)
         ang = f32(math.radians(angular_size_deg))
         p = np.zeros(1, dtype=S.EMITTER_PROFILE)
         p["emission"]["spectrum_index"] = self.add_spectrum(spd_rgb_luminance(rgb))
-        p["emission"]["image_index"] = S.INVALID
+        p["emission"]["image_index"] = image_index
         p["direction"][0] = d
         p["cls"] = S.EMITTER_DIRECTIONAL
         p["angular_size"] = ang

@@ -120,6 +120,14 @@ SAMPLE_QUERY = np.dtype([
 SAMPLE_RESULT = np.dtype([("w_o", f4, 3), ("pdf", f4), ("weight", f4, 3), ("eta", f4), ("properties", u4), ("medium_index", u4),
                           ("seed_start", u4), ("seed_end", u4)])
 SAMPLE_BOUNCE, SAMPLE_GIVEN = 0, 1
+# etxb_emitter_query (80 B) and the per-sample record etxb_debug_emitter / oracle_emitter return (include/etx_b200.h)
+EMITTER_QUERY = np.dtype([("op", u4), ("emitter", u4), ("seed", u4), ("directly_visible", u4), ("rnd", f4, 2), ("wavelength", f4),
+                          ("source", f4, 3), ("target", f4, 3), ("direction", f4, 3), ("uv", f4, 2), ("reserved", u4, 2)])
+EMITTER_RESULT = np.dtype([("value", f4, 3), ("origin", f4, 3), ("normal", f4, 3), ("direction", f4, 3), ("barycentric", f4, 3),
+                           ("pdf_sample", f4), ("pdf_area", f4), ("pdf_dir", f4), ("pdf_dir_out", f4), ("emitter_index", u4), ("triangle_index", u4),
+                           ("medium_index", u4), ("flags", u4), ("seed_start", u4), ("seed_end", u4), ("reserved", u4)])
+EMITTER_SELECT, EMITTER_SAMPLE_IN, EMITTER_EMISSION, EMITTER_RADIANCE = 0, 1, 2, 3
+EMITTER_FLAG_DELTA, EMITTER_FLAG_DISTANT = 1, 2
 BSDF_DIFFUSE, BSDF_REFLECTION, BSDF_TRANSMISSION, BSDF_MEDIUM_CHANGED, BSDF_DELTA = 1, 2, 4, 8, 16
 # etxb_debug_thresholds / etxb_debug_branch_counts (include/etx_b200.h): a threshold of 0 always takes the large-queue branch, NEVER never does
 DEBUG_THRESHOLDS = np.dtype([("merge_sort_min_queries", u4), ("merge_min_warps_per_sm", u4), ("tail_queue", u4), ("sort_queue_min", u4), ("merge_qpw", u4)])
@@ -143,6 +151,7 @@ EXPECTED_SIZES = {
     "EMITTER": (EMITTER, 32), "SPECTRUM": (SPECTRUM, 3552), "DISTRIBUTION": (DISTRIBUTION, 32), "IMAGE": (IMAGE, 112),
     "MEDIUM": (MEDIUM, 80), "CAMERA": (CAMERA, 176), "SCENE": (SCENE, 528), "CLOSURE_QUERY": (CLOSURE_QUERY, 96),
     "SAMPLE_QUERY": (SAMPLE_QUERY, 96), "SAMPLE_RESULT": (SAMPLE_RESULT, 48),
+    "EMITTER_QUERY": (EMITTER_QUERY, 80), "EMITTER_RESULT": (EMITTER_RESULT, 104),
     "LIGHT_VERTEX_REC": (LIGHT_VERTEX_REC, 96), "MERGE_QUERY": (MERGE_QUERY, 64), "MERGE_RESULT": (MERGE_RESULT, 48), "MERGE_GRID": (MERGE_GRID, 64),
 }
 for _name, (_dt, _size) in EXPECTED_SIZES.items():

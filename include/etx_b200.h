@@ -538,6 +538,38 @@ typedef struct etxb_sample_result {
   uint32_t properties, medium_index, seed_start, seed_end;
 } etxb_sample_result;
 int etxb_debug_bsdf_sample(etxb_ctx* ctx, const etxb_sample_query* queries, uint32_t count, uint32_t repetitions, etxb_sample_result* out);
+/* Emitter query (dvcm.cuh: the emitter selection, sample_emitter, sample_emission and emitter_get_radiance, as the light pass, the camera
+ * pass and the path tracer call them) on the uploaded scene.  One query is 80 bytes: the op, an emitter index, a sampler seed,
+ * directly_visible (0 / 1), a 2-D random number, the wavelength (ignored in RGB scenes), a source and a target position, a direction and a
+ * uv.  The ops:
+ *   0 select     distribution_sample(emitter_dist, emitter_count + 1, rnd[0]): emitter_index and emitter_discrete_pdf as pdf_sample
+ *   1 sample_in  sample_emitter(emitter, rnd, from_point = source): next-event estimation
+ *   2 emission   sample_emission on the sampler Smp::init(seed, r) of repetition r: the start of a light path
+ *   3 radiance   emitter_get_radiance(emitter, source, target, direction, uv, directly_visible): value and pdf_area, pdf_dir, pdf_dir_out
+ * Ops 0, 1 and 3 ignore the seed and return the same record for every repetition; op 0 ignores the emitter index. */
+typedef struct etxb_emitter_query {
+  uint32_t op, emitter, seed, directly_visible;
+  float rnd[2];
+  float wavelength;
+  float source[3], target[3], direction[3];
+  float uv[2];
+  uint32_t reserved[2];
+} etxb_emitter_query;
+#define ETXB_EMITTER_SELECT 0u
+#define ETXB_EMITTER_SAMPLE_IN 1u
+#define ETXB_EMITTER_EMISSION 2u
+#define ETXB_EMITTER_RADIANCE 3u
+/* One 104-byte record per (query, repetition), repetition-minor: every field of the device EmitterSample (the value, rgb; a spectral value
+ * fills all three), flags (bit 0 is_delta, bit 1 is_distant), and for op 2 the sampler state Smp::init(seed, r) left and the state after
+ * sample_emission (0 for the other ops).  Op 0 fills emitter_index and pdf_sample, op 3 value, the three pdfs and emitter_index; in
+ * both, triangle_index and medium_index are 0xffffffff (kInvalidIndex) and the other fields 0. */
+typedef struct etxb_emitter_result {
+  float value[3];
+  float origin[3], normal[3], direction[3], barycentric[3];
+  float pdf_sample, pdf_area, pdf_dir, pdf_dir_out;
+  uint32_t emitter_index, triangle_index, medium_index, flags, seed_start, seed_end, reserved;
+} etxb_emitter_result;
+int etxb_debug_emitter(etxb_ctx* ctx, const etxb_emitter_query* queries, uint32_t count, uint32_t repetitions, etxb_emitter_result* out);
 /* Queue sizes from which the light and camera passes take their large-queue branches.  A pass of a long queue runs the same paths as
  * one of a short queue, in another order; these let a small film take either branch.  Each field is a queue size: 0 = always the
  * large-queue branch, 0xffffffff = never.

@@ -48,6 +48,8 @@ def load(flavor="parity"):
         lib.oracle_bsdf_eval.argtypes = [vp, vp, u32, u32, u32, vp]
     if hasattr(lib, "oracle_bsdf_sample"):
         lib.oracle_bsdf_sample.argtypes = [vp, vp, u32, u32, u32, vp]
+    if hasattr(lib, "oracle_emitter"):
+        lib.oracle_emitter.argtypes = [vp, vp, u32, u32, u32, vp]
     if hasattr(lib, "oracle_merge"):
         lib.oracle_merge.argtypes = [vp, vp, u32, vp, vp, u32, u32, u32, vp, vp]
     lib.oracle_sampler.argtypes = [vp, vp, u32, u32, vp, vp]
@@ -79,6 +81,11 @@ def has_bsdf_eval(flavor="parity"):
 def has_bsdf_sample(flavor="parity"):
     """Whether the built oracle exports oracle_bsdf_sample."""
     return hasattr(load(flavor), "oracle_bsdf_sample")
+
+
+def has_emitter(flavor="parity"):
+    """Whether the built oracle exports oracle_emitter."""
+    return hasattr(load(flavor), "oracle_emitter")
 
 
 def has_merge(flavor="parity"):
@@ -264,6 +271,14 @@ class Oracle:
         queries = np.ascontiguousarray(queries, dtype=self.S.SAMPLE_QUERY)
         out = np.zeros((queries.shape[0], int(repetitions)), dtype=self.S.SAMPLE_RESULT)
         self.lib.oracle_bsdf_sample(self.h, _p(queries), queries.shape[0], int(repetitions), int(threads or os.cpu_count() or 1), _p(out))
+        return out
+
+    def emitter(self, queries, repetitions=1, threads=None):
+        """The reference's emitter routines for S.EMITTER_QUERY records, repetition r of each emission query on Sampler(seed, r); S.EMITTER_RESULT
+        records shaped (n, repetitions), in the layout of GPUVCM.debug_emitter."""
+        queries = np.ascontiguousarray(queries, dtype=self.S.EMITTER_QUERY)
+        out = np.zeros((queries.shape[0], int(repetitions)), dtype=self.S.EMITTER_RESULT)
+        self.lib.oracle_emitter(self.h, _p(queries), queries.shape[0], int(repetitions), int(threads or os.cpu_count() or 1), _p(out))
         return out
 
     def merge(self, records, light_wavelengths, queries, repetitions=1, threads=None):

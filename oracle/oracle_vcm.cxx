@@ -1163,6 +1163,66 @@ void oracle_bsdf_sample(void* h, const etxb_sample_query* queries, uint32_t coun
   });
 }
 
+// The reference's own emitter routines (scene_emitters.hxx) for etxb_emitter_query records (include/etx_b200.h): sample_emitter_index and
+// emitter_discrete_pdf (op 0), sample_emitter (op 1), sample_emission on Sampler(seed, r) (op 2), emitter_get_radiance with the
+// EmitterRadianceQuery the query describes (op 3).  One etxb_emitter_result per (query, repetition r), as etxb_debug_emitter writes them.
+static_assert(sizeof(etxb_emitter_query) == 80);
+static_assert(sizeof(etxb_emitter_result) == 104);
+void oracle_emitter(void* h, const etxb_emitter_query* queries, uint32_t count, uint32_t repetitions, uint32_t threads, etxb_emitter_result* out) {
+  auto* o = static_cast<Oracle*>(h);
+  const Scene& scene = o->scene;
+  parallel_ranges(count * repetitions, threads, [&](uint32_t begin, uint32_t end, uint32_t, uint32_t) {
+    for (uint32_t t = begin; t < end; ++t) {
+      const etxb_emitter_query& q = queries[t / repetitions];
+      const SpectralQuery spect = scene.spectral() ? SpectralQuery{q.wavelength, SpectralQuery::Spectral} : SpectralQuery::sample();
+      const float3 source = {q.source[0], q.source[1], q.source[2]};
+      etxb_emitter_result dst = {};
+      EmitterSample s = {};
+      if (q.op == ETXB_EMITTER_SELECT) {
+        s.emitter_index = sample_emitter_index(scene, q.rnd[0]);
+        s.pdf_sample = emitter_discrete_pdf(scene.emitter_instances[s.emitter_index], scene.emitters_distribution);
+      } else if (q.op == ETXB_EMITTER_SAMPLE_IN) {
+        s = sample_emitter(spect, q.emitter, {q.rnd[0], q.rnd[1]}, source, scene);
+      } else if (q.op == ETXB_EMITTER_EMISSION) {
+        Sampler smp(q.seed, t % repetitions);
+        dst.seed_start = smp.seed;
+        s = sample_emission(scene, spect, smp);
+        dst.seed_end = smp.seed;
+      } else {
+        EmitterRadianceQuery rq = {
+          .source_position = source,
+          .target_position = {q.target[0], q.target[1], q.target[2]},
+          .direction = {q.direction[0], q.direction[1], q.direction[2]},
+          .uv = {q.uv[0], q.uv[1]},
+          .directly_visible = q.directly_visible != 0u,
+        };
+        s.emitter_index = q.emitter;
+        s.value = emitter_get_radiance(scene.emitter_instances[q.emitter], spect, rq, s.pdf_area, s.pdf_dir, s.pdf_dir_out, scene);
+      }
+      const float3 v = s.value.spectral() ? float3{s.value.value, s.value.value, s.value.value} : s.value.integrated;
+      const auto put = [](float* d, const float3& a) {
+        d[0] = a.x;
+        d[1] = a.y;
+        d[2] = a.z;
+      };
+      put(dst.value, v);
+      put(dst.origin, s.origin);
+      put(dst.normal, s.normal);
+      put(dst.direction, s.direction);
+      put(dst.barycentric, s.barycentric);
+      dst.pdf_sample = s.pdf_sample;
+      dst.pdf_area = s.pdf_area;
+      dst.pdf_dir = s.pdf_dir;
+      dst.pdf_dir_out = s.pdf_dir_out;
+      dst.emitter_index = s.emitter_index;
+      dst.triangle_index = s.triangle_index;
+      dst.medium_index = s.medium_index;
+      dst.flags = (s.is_delta ? 1u : 0u) | (s.is_distant ? 2u : 0u);
+      out[t] = dst;
+    }
+  });
+}
+
 // The reference's own photon gather (VCMSpatialGridData::gather, vcm_shared.hxx:886-924) for etxb_debug_merge's inputs: the light-vertex
 // records (device layout, 96 B) become o.light_vertices and build_grid runs on them at the current iteration; each query becomes the
 // Intersection make_intersection builds for its hit (as oracle_trace does) and a VCMPathState, and is gathered `repetitions` times on
