@@ -92,6 +92,7 @@ def load_library(flavor="fast"):
     lib.etxb_group_comm_reduce_film.argtypes = [vp, u32, vp, u64]
     lib.etxb_group_comm_init_replicas.argtypes = [vp, u32, u32, vp, u64]
     lib.etxb_group_reserve_split_lane.argtypes = [vp]
+    lib.etxb_debug_group_plan.argtypes = [u32, u32, u32, u32, C.c_int, vp, u32, vp, u32]
     lib.etxb_set_integrator.argtypes = [vp, u32]
     lib.etxb_pt_options_default.argtypes = [vp]
     lib.etxb_pt_options_default.restype = None
@@ -616,8 +617,9 @@ class GPUPathTracing(GPUVCM):
 
 
 class GPUVCMGroup:
-    """Several iterations in flight on one device (etxb_group): `lanes` contexts, one host thread each inside the module, pulling
-    iteration indices from a shared counter.  Same Integrator-style surface as GPUVCM: run / enqueue / wait / status / film."""
+    """Several iterations in flight on one device (etxb_group): `lanes` contexts, one host thread each inside the module, each popping
+    iteration indices from its lane's queue, which enqueue fills (on one GPU all lanes share one queue, so a free lane takes the next index).
+    Same Integrator-style surface as GPUVCM: run / enqueue / wait / status / film."""
 
     def __init__(self, scene_data, lanes=4, flavor="fast", device=0, max_light_vertices=0, profile=False):
         self.lib = load_library(flavor)

@@ -283,8 +283,8 @@ struct etxb_ctx {
 };
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Iterations in flight (etxb_group): L contexts on one device, one host thread each, pulling iteration indices from a shared
-// counter.  VCM iterations are independent (vcm_cpu.cxx:95-113: the index only sets the merge radius and the sampler seeds), and
+// Iterations in flight (etxb_group): L contexts on one device, one host thread each, pulling iteration indices from per-lane
+// queues (WorkPlan).  VCM iterations are independent (vcm_cpu.cxx:95-113: the index only sets the merge radius and the sampler seeds), and
 // the bounce loop of one iteration ends in a long latency-bound tail (a few thousand paths, ~50 bounces); with several iterations in
 // flight that tail overlaps the full-width head of another iteration.  The film is the mean of the lanes' films weighted by the
 // iterations each lane finished — the same set of iterations, hence the same estimate, as one context running them in sequence.
@@ -340,13 +340,37 @@ __global__ void __launch_bounds__(256) k_film_finish_mean(const float4* sum, flo
 }
 }  // extern "C"
 
+// Which lane renders which iteration of an etxb_group.  etxb_group_enqueue deals the new ordinals into queues (plan_enqueue, the one place
+// that reads the mode); lane l pops queues[lane_queue[l]], whatever the mode.
+//   local     one GPU: every lane reads queue 0, which holds the ordinals in order, so a free lane takes the next one
+//   tiles     etxb_group_comm_init, world >= 2: lane l reads queue l, which holds the ordinals l, l + L, l + 2L, ... on EVERY rank (lane l of every
+//             rank shares a communicator; one shared queue would pair different iterations across ranks)
+//   replicas  etxb_group_comm_init_replicas, world >= 2: replica_plan deals the job's ordinals; whole frames go to queue 0, which every lane but
+//             the split lane reads, and camera-split parts to the split lane's own queue
+// The split lane reads its own queue in every mode, which only the replica mode fills; tile mode and a split lane refuse each other.
+struct WorkItem {
+  uint32_t ordinal;      // of the iteration within the job
+  uint32_t part, parts;  // parts == 1: the whole frame; else the camera pass of part `part` (tile % parts == part), light pass in full
+};
+enum class GroupMode : uint32_t { local = 0, tiles = 1, replicas = 2 };  // the values etxb_debug_group_plan takes
+struct WorkPlan {
+  GroupMode mode = GroupMode::local;
+  uint32_t world = 1, rank = 0;
+  uint32_t enqueued = 0;                     // iterations enqueued since etxb_group_begin: the next ordinal
+  uint32_t split_lane = 0xffffffffu;         // the lane reserved for camera-split iterations (etxb_group_reserve_split_lane), or none
+  uint32_t split_part = 0, split_parts = 0;  // the (part, parts) that lane's film is made of; 0 parts = not used yet
+  std::vector<std::deque<WorkItem>> queues;  // one per lane
+  std::vector<uint32_t> lane_queue;
+};
+
 struct etxb_group {
   std::vector<etxb_ctx*> lanes;
   std::vector<std::thread> workers;
   std::mutex m;
   std::condition_variable cv_work, cv_idle;
   uint32_t first_iteration = 0, stride = 1, taken = 0;  // the k-th iteration handed out renders index first + k * stride
-  uint32_t pending = 0, in_flight = 0;
+  uint32_t in_flight = 0;
+  WorkPlan plan;
   bool quit = false;
   int error = ETXB_OK;
   std::string error_text;
@@ -355,21 +379,6 @@ struct etxb_group {
   double last_iteration_seconds = 0.0;
   DevBuf<float4> combined;
   int device = 0;
-  // pixel-tile sharding over several processes (etxb_group_comm_init): every lane has its own communicator, and the k-th iteration of lane l is
-  // the ordinal l + k * lanes on EVERY rank (the shared counter of the single-GPU mode would pair different iterations across ranks)
-  bool sharded = false;
-  struct ReplicaItem {
-    uint32_t index;        // ordinal of the iteration within the job
-    uint32_t part, parts;  // parts == 1: the whole frame; else the camera pass of part `part` (tile % parts == part), light pass in full
-  };
-  std::deque<ReplicaItem> whole_queue, split_queue;
-  uint32_t split_lane = 0xffffffffu;  // replicas: the lane reserved for camera-split iterations (etxb_group_reserve_split_lane), or none
-  uint32_t split_part = 0, split_parts = 0;  // the (part, parts) that lane's film is made of; 0 parts = not used yet
-  bool replicas = false;             // etxb_group_comm_init_replicas: whole-frame iterations dealt to the ranks (global index j -> rank j % world), one film reduce
-  uint32_t job_enqueued = 0;         // replicas: iterations enqueued for the whole job
-  uint32_t world = 1, rank = 0;
-  uint32_t enqueued_total = 0;
-  std::vector<uint32_t> lane_next;
   ncclComm_t reduce_comm = nullptr;  // the frame reduce has its own communicator: the lanes' ones are busy with iterations in flight
   cudaStream_t stream = nullptr;
   DevBuf<float4> combined_light, reduced;
@@ -443,6 +452,23 @@ int fail(etxb_ctx* ctx, int code, const char* fmt, ...) {
     ncclResult_t res__ = (call);                                                                                           \
     if (res__ != ncclSuccess) return fail(ctx, ETXB_ERR_CUDA, "%s failed: %s (%s:%d)", #call, nccl_api()->GetErrorString(res__), __FILE__, __LINE__); \
   } while (0)
+
+// Joins rank `rank` of a `world`-rank communicator on the current device; `id` holds the ncclUniqueId rank 0 made.  Collective.
+int comm_init_rank(etxb_ctx* ctx, ncclComm_t* comm, uint32_t world, uint32_t rank, const void* id) {
+  NcclApi* n = nccl_api();
+  if (!n) return fail(ctx, ETXB_ERR_NOT_READY, "libnccl.so.2 could not be loaded");
+  ncclUniqueId uid;
+  memcpy(&uid, id, sizeof(uid));
+  NCCL_OK(ctx, n->CommInitRank(comm, int(world), uid, int(rank)));
+  return ETXB_OK;
+}
+
+// A stream at the device's highest priority, so that its few blocks do not queue behind the lanes' large kernels
+cudaError_t create_priority_stream(cudaStream_t* stream) {
+  int prio_low = 0, prio_high = 0;
+  if (cudaError_t err = cudaDeviceGetStreamPriorityRange(&prio_low, &prio_high)) return err;
+  return cudaStreamCreateWithPriority(stream, cudaStreamNonBlocking, prio_high);
+}
 
 template <class T>
 int upload(etxb_ctx* ctx, DevBuf<T>& buf, const T* host, size_t n) {
@@ -1706,9 +1732,9 @@ int debug_merge(etxb_ctx* ctx, uint32_t record_count, const etxb_merge_query* d_
 // behind the others (20 iterations on 8 ranks: 3, 3, 3, 3, 2, 2, 2, 2): with a split lane those R iterations are split instead, each over
 // P = world / R ranks by camera tile — every part traces the whole light pass itself (same photon map, no exchange) and the camera pass of its
 // tiles; the parts meet in the frame reduce.  A split lane's film is made of ONE (part, parts) geometry: a later round that would need another
-// one is dealt as whole frames.  Returns the parts of this round's split (0: none).
-uint32_t replica_plan(uint32_t world, uint32_t rank, uint32_t base, uint32_t iterations, bool split_lane, uint32_t have_part, uint32_t have_parts,
-                             std::vector<etxb_group::ReplicaItem>& out) {
+// parts count is dealt as whole frames (with the count fixed, a rank's part is always rank % parts).  Returns the parts of this round's split
+// (0: none).
+uint32_t replica_plan(uint32_t world, uint32_t rank, uint32_t base, uint32_t iterations, bool split_lane, uint32_t have_parts, std::vector<WorkItem>& out) {
   uint32_t whole = iterations, rest = 0, parts = 1;
   if ((iterations >= world) && split_lane) {
     rest = iterations % world;
@@ -1722,25 +1748,39 @@ uint32_t replica_plan(uint32_t world, uint32_t rank, uint32_t base, uint32_t ite
   for (uint32_t j = base; j < base + whole; ++j)
     if ((j % world) == rank) out.push_back({j, 0u, 1u});
   for (uint32_t r = 0; r < rest; ++r) {
-    if ((rank / parts) != r) continue;
-    const uint32_t part = rank % parts;
-    if ((have_parts != 0u) && (have_part != part)) continue;  // cannot happen while `parts` stays the same: a rank's part is rank % parts
-    out.push_back({base + whole + r, part, parts});
+    if ((rank / parts) == r) out.push_back({base + whole + r, rank % parts, parts});
   }
   return rest ? parts : 0u;
 }
 
-bool group_has_work(const etxb_group* grp, uint32_t lane) {
-  if (grp->replicas) return (lane == grp->split_lane) ? !grp->split_queue.empty() : !grp->whole_queue.empty();
-  if (lane == grp->split_lane) return false;
-  return grp->sharded ? (grp->lane_next[lane] < grp->enqueued_total) : (grp->pending > 0);
+// The planner: deals the ordinals enqueued .. enqueued + iterations - 1 into the queues and routes every lane to its queue (see WorkPlan).
+void plan_enqueue(WorkPlan& p, uint32_t iterations) {
+  const uint32_t lanes = uint32_t(p.queues.size());
+  const bool tiles = p.mode == GroupMode::tiles;
+  for (uint32_t l = 0; l < lanes; ++l) p.lane_queue[l] = (tiles || (l == p.split_lane)) ? l : 0u;
+  if (p.mode == GroupMode::replicas) {
+    std::vector<WorkItem> items;
+    uint32_t parts_used = replica_plan(p.world, p.rank, p.enqueued, iterations, p.split_lane != 0xffffffffu, p.split_parts, items);
+    for (const WorkItem& it : items) {
+      if (it.parts > 1u) p.split_part = it.part;
+      p.queues[(it.parts > 1u) ? p.split_lane : 0u].push_back(it);
+    }
+    if (parts_used) p.split_parts = parts_used;  // every rank records the split geometry, also those that got no part of this round
+  } else {
+    for (uint32_t k = p.enqueued; k < p.enqueued + iterations; ++k) p.queues[tiles ? (k % lanes) : 0u].push_back({k, 0u, 1u});
+  }
+  p.enqueued += iterations;
 }
+void plan_clear(WorkPlan& p) {
+  for (auto& q : p.queues) q.clear();
+  p.enqueued = 0;
+}
+
+bool group_has_work(const etxb_group* grp, uint32_t lane) { return !grp->plan.queues[grp->plan.lane_queue[lane]].empty(); }
 bool group_idle(const etxb_group* grp) {
   if (grp->in_flight > 0) return false;
-  if (grp->replicas) return grp->whole_queue.empty() && grp->split_queue.empty();
-  if (!grp->sharded) return grp->pending == 0;
-  for (uint32_t next : grp->lane_next)
-    if (next < grp->enqueued_total) return false;
+  for (const auto& q : grp->plan.queues)
+    if (!q.empty()) return false;
   return true;
 }
 
@@ -1751,26 +1791,14 @@ void group_worker(etxb_group* grp, uint32_t lane) {
   for (;;) {
     grp->cv_work.wait(lock, [&] { return grp->quit || group_has_work(grp, lane); });
     if (grp->quit) return;
-    uint32_t ordinal = 0;
-    etxb_group::ReplicaItem item = {0u, 0u, 1u};
-    if (grp->replicas) {
-      auto& queue = (lane == grp->split_lane) ? grp->split_queue : grp->whole_queue;
-      item = queue.front();
-      queue.pop_front();
-      ordinal = item.index;
-      grp->taken = std::max(grp->taken, ordinal + 1u);
-    } else if (grp->sharded) {
-      ordinal = grp->lane_next[lane];
-      grp->lane_next[lane] += uint32_t(grp->lanes.size());
-      grp->taken = std::max(grp->taken, ordinal + 1u);
-    } else {
-      ordinal = grp->taken++;
-      grp->pending -= 1;
-    }
-    uint32_t iteration = grp->first_iteration + ordinal * grp->stride;
+    auto& queue = grp->plan.queues[grp->plan.lane_queue[lane]];
+    const WorkItem item = queue.front();
+    queue.pop_front();
+    grp->taken = std::max(grp->taken, item.ordinal + 1u);
+    uint32_t iteration = grp->first_iteration + item.ordinal * grp->stride;
     grp->in_flight += 1;
     lock.unlock();
-    if (grp->replicas && (lane == grp->split_lane)) {
+    if (item.parts > 1u) {
       // this lane renders the camera pass of its part only; the light pass (and so the photon map) in full
       ctx->rank = item.part;
       ctx->world = item.parts;
@@ -1784,16 +1812,21 @@ void group_worker(etxb_group* grp, uint32_t lane) {
     if ((rc != ETXB_OK) && (grp->error == ETXB_OK)) {
       grp->error = rc;
       grp->error_text = etxb_last_error(ctx);
-      grp->pending = 0;
-      grp->whole_queue.clear();
-      grp->split_queue.clear();
-      for (auto& next : grp->lane_next) next = 0xffffffffu;
+      plan_clear(grp->plan);
     }
     if (group_idle(grp)) {
       grp->busy_seconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - grp->busy_since).count();
       grp->cv_idle.notify_all();
     }
   }
+}
+
+// A call the group refuses in its present state: the reason goes to etxb_group_last_error and to lane 0's etxb_last_error
+int group_refuse(etxb_group* grp, const char* why) {
+  fail(grp->lanes[0], ETXB_ERR_INVALID_ARGUMENT, "%s", why);
+  std::lock_guard<std::mutex> lock(grp->m);
+  grp->error_text = why;
+  return ETXB_ERR_INVALID_ARGUMENT;
 }
 
 int group_combine_into(etxb_group* grp, uint32_t layer, DevBuf<float4>& target, uint32_t* completed, bool raw = false) {
@@ -1814,7 +1847,7 @@ int group_combine_into(etxb_group* grp, uint32_t layer, DevBuf<float4>& target, 
     f.weight[l] = raw ? float(grp->lanes[l]->completed) : (total ? float(double(grp->lanes[l]->completed) / double(total)) : 0.0f);
     f.weight_light[l] = f.weight[l];
     f.weight_count[l] = f.weight[l];
-    if (raw && (l == grp->split_lane) && (grp->split_part != 0u)) {
+    if (raw && (l == grp->plan.split_lane) && (grp->plan.split_part != 0u)) {
       // a camera-split lane that is not part 0: its camera tiles count, its (complete, redundant) light image and its iteration count do not
       f.weight_light[l] = 0.0f;
       f.weight_count[l] = 0.0f;
@@ -2168,19 +2201,13 @@ int etxb_comm_unique_id(void* out_id, uint64_t bytes) {
 
 int etxb_comm_init(etxb_ctx* ctx, uint32_t world, uint32_t rank, const void* id, uint64_t bytes) {
   if (!ctx || !id || (bytes < sizeof(ncclUniqueId)) || (world == 0u) || (rank >= world)) return ETXB_ERR_INVALID_ARGUMENT;
-  NcclApi* n = nccl_api();
-  if (!n) return fail(ctx, ETXB_ERR_NOT_READY, "libnccl.so.2 could not be loaded");
   if (ctx->comm != nullptr) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "the context already has a communicator");
   cudaSetDevice(ctx->device);
-  ncclUniqueId uid;
-  memcpy(&uid, id, sizeof(uid));
-  NCCL_OK(ctx, n->CommInitRank(&ctx->comm, int(world), uid, int(rank)));
+  if (int rc = comm_init_rank(ctx, &ctx->comm, world, rank, id)) return rc;
   ctx->rank = rank;
   ctx->world = world;
   CUDA_OK(ctx, ctx->comm_counts.alloc(world));
-  int prio_low = 0, prio_high = 0;
-  CUDA_OK(ctx, cudaDeviceGetStreamPriorityRange(&prio_low, &prio_high));
-  CUDA_OK(ctx, cudaStreamCreateWithPriority(&ctx->comm_stream, cudaStreamNonBlocking, prio_high));
+  CUDA_OK(ctx, create_priority_stream(&ctx->comm_stream));
   CUDA_OK(ctx, cudaEventCreateWithFlags(&ctx->comm_ev_in, cudaEventDisableTiming));
   CUDA_OK(ctx, cudaEventCreateWithFlags(&ctx->comm_ev_out, cudaEventDisableTiming));
   return ETXB_OK;
@@ -2679,14 +2706,10 @@ int etxb_group_create(etxb_group** out, const etxb_device_config* cfg, uint32_t 
     }
     grp->lanes.push_back(ctx);
   }
-  grp->lane_next.assign(lanes, 0u);
+  grp->plan.queues.resize(lanes);
+  grp->plan.lane_queue.assign(lanes, 0u);
   cudaSetDevice(grp->device);
-  {
-    // the frame combine / reduce must not queue behind the lanes' kernels: highest priority
-    int prio_low = 0, prio_high = 0;
-    cudaDeviceGetStreamPriorityRange(&prio_low, &prio_high);
-    cudaStreamCreateWithPriority(&grp->stream, cudaStreamNonBlocking, prio_high);
-  }
+  create_priority_stream(&grp->stream);  // the frame combine / reduce
   for (uint32_t l = 0; l < lanes; ++l) grp->workers.emplace_back(group_worker, grp, l);
   *out = grp;
   return ETXB_OK;
@@ -2697,7 +2720,6 @@ void etxb_group_destroy(etxb_group* grp) {
   {
     std::lock_guard<std::mutex> lock(grp->m);
     grp->quit = true;
-    grp->pending = 0;
   }
   grp->cv_work.notify_all();
   for (auto& w : grp->workers) w.join();
@@ -2729,12 +2751,8 @@ int etxb_group_begin(etxb_group* grp, uint32_t first_iteration) {
   std::lock_guard<std::mutex> lock(grp->m);
   grp->first_iteration = first_iteration;
   grp->taken = 0;
-  grp->enqueued_total = 0;
-  grp->job_enqueued = 0;
-  grp->whole_queue.clear();
-  grp->split_queue.clear();
-  grp->split_part = grp->split_parts = 0;
-  for (uint32_t l = 0; l < grp->lane_next.size(); ++l) grp->lane_next[l] = l;
+  plan_clear(grp->plan);
+  grp->plan.split_part = grp->plan.split_parts = 0;
   grp->busy_seconds = 0.0;
   grp->error = ETXB_OK;
   grp->error_text.clear();
@@ -2751,7 +2769,7 @@ int etxb_group_update_scene(etxb_group* grp, const void* scene_blob, uint64_t sc
     grp->error_text = etxb_last_error(first);
     return rc;
   };
-  bool comm = grp->sharded || grp->replicas;
+  bool comm = grp->plan.mode != GroupMode::local;
   for (auto* c : grp->lanes) comm = comm || (c->comm != nullptr);
   if (comm) return refuse(fail(first, ETXB_ERR_UNSUPPORTED, "etxb_group_update_scene: a group with communicators takes a new scene through etxb_upload_scene on each lane"));
   if (int rc = check_scene_args(first, scene_bytes, camera_bytes)) return refuse(rc);
@@ -2799,28 +2817,7 @@ int etxb_group_enqueue(etxb_group* grp, uint32_t iterations) {
     if (grp->error != ETXB_OK) return grp->error;
     if (iterations == 0) return ETXB_OK;
     if (group_idle(grp)) grp->busy_since = std::chrono::steady_clock::now();
-    if (grp->sharded) {
-      grp->enqueued_total += iterations;
-    } else if (grp->replicas) {
-      // `iterations` more of the JOB's iterations.  Whole frames are dealt round-robin (the job's j-th iteration on rank j % world).  What is left
-      // when the count is not a multiple of the ranks would leave some ranks a whole iteration behind the others (20 iterations on 8 ranks: 3, 3, 3, 3,
-      // 2, 2, 2, 2): those R iterations are split instead, each over P = world / R ranks by camera tile — every part traces the whole light pass itself
-      // (same photon map, no exchange) and the camera pass of its tiles; the parts meet in the frame reduce.
-      std::vector<etxb_group::ReplicaItem> items;
-      uint32_t parts_used = replica_plan(grp->world, grp->rank, grp->job_enqueued, iterations, grp->split_lane != 0xffffffffu, grp->split_part, grp->split_parts, items);
-      for (const auto& it : items) {
-        if (it.parts == 1u) {
-          grp->whole_queue.push_back(it);
-        } else {
-          grp->split_part = it.part;
-          grp->split_queue.push_back(it);
-        }
-      }
-      if (parts_used) grp->split_parts = parts_used;  // every rank records the split geometry, also those that got no part of this round
-      grp->job_enqueued += iterations;
-    } else {
-      grp->pending += iterations;
-    }
+    plan_enqueue(grp->plan, iterations);
   }
   grp->cv_work.notify_all();
   return ETXB_OK;
@@ -2833,7 +2830,7 @@ int etxb_group_poll(etxb_group* grp, etxb_status* status) {
   for (size_t l = 0; l < grp->lanes.size(); ++l) {
     etxb_ctx* c = grp->lanes[l];
     // a camera-split iteration is finished by several ranks: it counts where part 0 ran
-    if (!((l == grp->split_lane) && (grp->split_part != 0u))) status->completed_iterations += c->completed;
+    if (!((l == grp->plan.split_lane) && (grp->plan.split_part != 0u))) status->completed_iterations += c->completed;
     status->light_vertices = std::max(status->light_vertices, c->last_light_vertices);
     status->overflow |= c->overflow_flag;
   }
@@ -2854,13 +2851,13 @@ int etxb_group_combine(etxb_group* grp, uint32_t layer, void** device_ptr, uint6
 }
 
 // Pixel tiles over several processes, `lanes` iterations in flight on each: ids = (lanes + 1) NCCL unique ids of 128 bytes, the same on every
-// rank (lane l of every rank forms communicator l; the last one carries the frame reduce).  Collective.
+// rank (lane l of every rank forms communicator l; the last one carries the frame reduce).  Collective.  Refused, before any NCCL call and so
+// alike on every rank, on a group that already has a communicator or, for world >= 2, a split lane.
 int etxb_group_comm_init(etxb_group* grp, uint32_t world, uint32_t rank, const void* ids, uint32_t id_count) {
   if (!grp || !ids || (world == 0u) || (rank >= world) || (id_count != grp->lanes.size() + 1u)) return ETXB_ERR_INVALID_ARGUMENT;
   if (int rc = etxb_group_wait(grp)) return rc;
-  NcclApi* n = nccl_api();
-  etxb_ctx* first = grp->lanes[0];
-  if (!n) return fail(first, ETXB_ERR_NOT_READY, "libnccl.so.2 could not be loaded");
+  if (grp->reduce_comm != nullptr) return group_refuse(grp, "etxb_group_comm_init: the group already has a communicator");
+  if ((world > 1u) && (grp->plan.split_lane != 0xffffffffu)) return group_refuse(grp, "etxb_group_comm_init: pixel tiles and a split lane exclude each other");
   const uint8_t* bytes = static_cast<const uint8_t*>(ids);
   for (size_t l = 0; l < grp->lanes.size(); ++l) {
     if (int rc = etxb_comm_init(grp->lanes[l], world, rank, bytes + l * sizeof(ncclUniqueId), sizeof(ncclUniqueId))) {
@@ -2869,63 +2866,66 @@ int etxb_group_comm_init(etxb_group* grp, uint32_t world, uint32_t rank, const v
     }
   }
   cudaSetDevice(grp->device);
-  ncclUniqueId uid;
-  memcpy(&uid, bytes + grp->lanes.size() * sizeof(ncclUniqueId), sizeof(uid));
-  NCCL_OK(first, n->CommInitRank(&grp->reduce_comm, int(world), uid, int(rank)));
+  if (int rc = comm_init_rank(grp->lanes[0], &grp->reduce_comm, world, rank, bytes + grp->lanes.size() * sizeof(ncclUniqueId))) return rc;
   std::lock_guard<std::mutex> lock(grp->m);
-  grp->sharded = world > 1u;
-  grp->world = world;
-  grp->rank = rank;
-  for (uint32_t l = 0; l < grp->lane_next.size(); ++l) grp->lane_next[l] = l;
-  grp->enqueued_total = 0;
+  grp->plan.mode = (world > 1u) ? GroupMode::tiles : GroupMode::local;
+  grp->plan.world = world;
+  grp->plan.rank = rank;
+  grp->plan.enqueued = 0;
   return ETXB_OK;
 }
 
-// Test hook (no device needed): what rank `rank` of `world` takes of an etxb_group_enqueue(iterations) in replica mode — triples (ordinal, part,
-// parts) into out; returns their number.
-int etxb_debug_replica_plan(uint32_t world, uint32_t rank, uint32_t base, uint32_t iterations, int split_lane, uint32_t* out_triples, uint32_t capacity) {
-  if ((world == 0u) || (rank >= world) || !out_triples) return ETXB_ERR_INVALID_ARGUMENT;
-  std::vector<etxb_group::ReplicaItem> items;
-  replica_plan(world, rank, base, iterations, split_lane != 0, 0u, 0u, items);
+// Test hook (no device needed): the queues of a `lanes`-lane group in `mode` (0 local, 1 tiles, 2 replicas) on rank `rank` of `world`, with its
+// last lane reserved for camera-split iterations if `split_lane`, after etxb_group_enqueue(enqueues[0]), ..., (enqueues[count - 1]) — quads
+// (queue, ordinal, part, parts) into out, queue by queue in the order the lanes pop them; returns their number.
+int etxb_debug_group_plan(uint32_t mode, uint32_t lanes, uint32_t world, uint32_t rank, int split_lane, const uint32_t* enqueues, uint32_t count,
+                          uint32_t* out_quads, uint32_t capacity) {
+  if ((mode > uint32_t(GroupMode::replicas)) || (lanes == 0u) || (lanes > kMaxLanes) || (world == 0u) || (rank >= world) || (!enqueues && count) || !out_quads)
+    return ETXB_ERR_INVALID_ARGUMENT;
+  if (split_lane && ((lanes < 2u) || (GroupMode(mode) == GroupMode::tiles))) return ETXB_ERR_INVALID_ARGUMENT;
+  WorkPlan p;
+  p.mode = GroupMode(mode);
+  p.world = world;
+  p.rank = rank;
+  p.queues.resize(lanes);
+  p.lane_queue.assign(lanes, 0u);
+  if (split_lane) p.split_lane = lanes - 1u;
+  for (uint32_t i = 0; i < count; ++i) plan_enqueue(p, enqueues[i]);
   uint32_t n = 0;
-  for (const auto& it : items) {
-    if (n >= capacity) break;
-    out_triples[n * 3u + 0u] = it.index;
-    out_triples[n * 3u + 1u] = it.part;
-    out_triples[n * 3u + 2u] = it.parts;
-    n += 1u;
-  }
+  for (uint32_t q = 0; q < lanes; ++q)
+    for (const WorkItem& it : p.queues[q]) {
+      if (n >= capacity) return int(n);
+      uint32_t* o = out_quads + 4u * n++;
+      o[0] = q, o[1] = it.ordinal, o[2] = it.part, o[3] = it.parts;
+    }
   return int(n);
 }
 
-// Replica mode: reserves the group's LAST lane for camera-split iterations (see etxb_group_enqueue); it takes no whole-frame iterations.  Call
-// before etxb_group_comm_init_replicas; needs at least two lanes.
+// Replica mode: reserves the group's LAST lane for camera-split iterations (see replica_plan); it takes no whole-frame iterations.  Call before
+// etxb_group_comm_init_replicas; needs at least two lanes, and is refused on a group in tile mode.
 int etxb_group_reserve_split_lane(etxb_group* grp) {
   if (!grp || (grp->lanes.size() < 2u)) return ETXB_ERR_INVALID_ARGUMENT;
   if (int rc = etxb_group_wait(grp)) return rc;
+  if (grp->plan.mode == GroupMode::tiles) return group_refuse(grp, "etxb_group_reserve_split_lane: pixel tiles and a split lane exclude each other");
   std::lock_guard<std::mutex> lock(grp->m);
-  grp->split_lane = uint32_t(grp->lanes.size()) - 1u;
+  grp->plan.split_lane = uint32_t(grp->lanes.size()) - 1u;
   return ETXB_OK;
 }
 
 // The other way to split a K-iteration render over the ranks: whole-frame iterations, the job's j-th iteration on rank j % world (each rank's
 // lanes take that rank's share in order).  No collective inside an iteration; one ncclReduce of the (count-weighted) films per frame.  id = one
-// NCCL unique id.  Collective.
+// NCCL unique id.  Collective.  Refused, before any NCCL call, on a group that already has a communicator.
 int etxb_group_comm_init_replicas(etxb_group* grp, uint32_t world, uint32_t rank, const void* id, uint64_t bytes) {
   if (!grp || !id || (bytes < sizeof(ncclUniqueId)) || (world == 0u) || (rank >= world)) return ETXB_ERR_INVALID_ARGUMENT;
   if (int rc = etxb_group_wait(grp)) return rc;
-  NcclApi* n = nccl_api();
-  etxb_ctx* first = grp->lanes[0];
-  if (!n) return fail(first, ETXB_ERR_NOT_READY, "libnccl.so.2 could not be loaded");
+  if (grp->reduce_comm != nullptr) return group_refuse(grp, "etxb_group_comm_init_replicas: the group already has a communicator");
   cudaSetDevice(grp->device);
-  ncclUniqueId uid;
-  memcpy(&uid, id, sizeof(uid));
-  NCCL_OK(first, n->CommInitRank(&grp->reduce_comm, int(world), uid, int(rank)));
+  if (int rc = comm_init_rank(grp->lanes[0], &grp->reduce_comm, world, rank, id)) return rc;
   std::lock_guard<std::mutex> lock(grp->m);
-  grp->replicas = world > 1u;
-  grp->world = world;
-  grp->rank = rank;
-  grp->job_enqueued = 0;
+  grp->plan.mode = (world > 1u) ? GroupMode::replicas : GroupMode::local;
+  grp->plan.world = world;
+  grp->plan.rank = rank;
+  grp->plan.enqueued = 0;
   return ETXB_OK;
 }
 
@@ -2933,17 +2933,17 @@ int etxb_group_comm_init_replicas(etxb_group* grp, uint32_t world, uint32_t rank
 // the same weights on every rank, the lane -> iteration map is fixed), the camera tiles are summed on rank 0, Result = max(0, camera + light).
 int etxb_group_comm_reduce_film(etxb_group* grp, uint32_t layer, float* dst_rgba, uint64_t dst_bytes) {
   if (!grp || (layer > ETXB_FILM_LIGHT)) return ETXB_ERR_INVALID_ARGUMENT;
-  if (!grp->sharded && !grp->replicas) return etxb_group_read_film(grp, layer, dst_rgba, dst_bytes);
+  if (grp->plan.mode == GroupMode::local) return etxb_group_read_film(grp, layer, dst_rgba, dst_bytes);
   NcclApi* n = nccl_api();
   etxb_ctx* first = grp->lanes[0];
   const size_t px = first->path_count;
   cudaSetDevice(grp->device);
-  if (grp->replicas) {
+  if (grp->plan.mode == GroupMode::replicas) {
     // every rank: sum over its lanes of (iterations finished x mean film), .w = iterations; rank 0 divides the reduced sum by the reduced count
     if (int rc = group_combine_into(grp, layer, grp->combined, nullptr, true)) return rc;
     if (grp->reduced.count < px) CUDA_OK(first, grp->reduced.alloc(px));
     NCCL_OK(first, n->Reduce(grp->combined.ptr, grp->reduced.ptr, px * 4u, ncclFloat, ncclSum, 0, grp->reduce_comm, grp->stream));
-    if (grp->rank != 0u) {
+    if (grp->plan.rank != 0u) {
       CUDA_OK(first, cudaStreamSynchronize(grp->stream));
       return ETXB_OK;
     }
@@ -2958,7 +2958,7 @@ int etxb_group_comm_reduce_film(etxb_group* grp, uint32_t layer, float* dst_rgba
     if (grp->reduced.count < px) CUDA_OK(first, grp->reduced.alloc(px));
     NCCL_OK(first, n->Reduce(grp->combined.ptr, grp->reduced.ptr, px * 4u, ncclFloat, ncclSum, 0, grp->reduce_comm, grp->stream));
   }
-  if (grp->rank != 0u) {
+  if (grp->plan.rank != 0u) {
     CUDA_OK(first, cudaStreamSynchronize(grp->stream));
     return ETXB_OK;
   }

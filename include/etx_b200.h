@@ -628,8 +628,8 @@ int etxb_debug_merge(etxb_ctx* ctx, const void* records, uint32_t record_count, 
 /* ---- several iterations in flight on one device -----------------------------------------------------------------------
  * The reference runs ONE iteration at a time and spreads its paths over the CPU's threads (vcm_cpu.cxx:115-171, TaskScheduler).
  * A GPU wavefront iteration ends in a long, latency-bound tail (few paths, ~50 more bounces); an etxb_group keeps `lanes`
- * independent contexts on one device, one host thread each, pulling iteration indices from a shared counter, so that tail overlaps
- * other iterations.  Uploads/options go to every lane (etxb_group_lane); the film is the mean of the lanes' films weighted by the
+ * independent contexts on one device, one host thread each, pulling iteration indices from per-lane queues that etxb_group_enqueue
+ * fills, so that tail overlaps other iterations.  Uploads/options go to every lane (etxb_group_lane); the film is the mean of the lanes' films weighted by the
  * iterations each finished — the same set of iterations as a single context running them in order.
  * Replaces the run()/update() pump of CPUVCM (vcm_cpu.cxx:247-276) for throughput rendering. */
 typedef struct etxb_group etxb_group;
@@ -665,18 +665,23 @@ int etxb_comm_world(const etxb_ctx* ctx, uint32_t* world, uint32_t* rank);
 /* Collective: sums the disjoint camera tiles on rank 0 (ncclReduce of the float4 film); dst_rgba is written on rank 0 only. */
 int etxb_comm_reduce_film(etxb_ctx* ctx, uint32_t layer, float* dst_rgba, uint64_t dst_bytes);
 /* The same with several iterations in flight per GPU: ids = (lanes + 1) x ETXB_COMM_ID_BYTES (one communicator per lane + one for the frame
- * reduce); lane l renders the iteration ordinals l, l + lanes, ... on every rank. */
+ * reduce); lane l renders the iteration ordinals l, l + lanes, ... on every rank.  ETXB_ERR_INVALID_ARGUMENT, before any collective, on a group
+ * that already has a communicator (from either init) or, for world >= 2, a split lane. */
 int etxb_group_comm_init(etxb_group* group, uint32_t world, uint32_t rank, const void* ids, uint32_t id_count); /* collective */
 /* Whole-frame iterations dealt to the ranks instead (the job's j-th iteration on rank j % world; etxb_group_enqueue then counts iterations of the
- * JOB): no collective inside an iteration, one count-weighted ncclReduce of the films per frame.  id = one ETXB_COMM_ID_BYTES id. */
+ * JOB): no collective inside an iteration, one count-weighted ncclReduce of the films per frame.  id = one ETXB_COMM_ID_BYTES id.
+ * ETXB_ERR_INVALID_ARGUMENT, before any collective, on a group that already has a communicator. */
 int etxb_group_comm_init_replicas(etxb_group* group, uint32_t world, uint32_t rank, const void* id, uint64_t bytes); /* collective */
 /* Optional, before etxb_group_comm_init_replicas: reserves the group's LAST lane for camera-split iterations.  When an etxb_group_enqueue(n >= world)
  * is not a multiple of the ranks, its last n % world iterations are then split over world / (n % world) ranks each: every part traces the whole
  * light pass itself (same photon map, no exchange) and the camera pass of its pixel tiles, and the parts meet in etxb_group_comm_reduce_film —
- * instead of leaving some ranks one whole iteration behind the others. */
+ * instead of leaving some ranks one whole iteration behind the others.  ETXB_ERR_INVALID_ARGUMENT on a group in pixel-tile mode. */
 int etxb_group_reserve_split_lane(etxb_group* group);
-/* Test hook (needs no device): the (ordinal, part, parts) triples rank `rank` of `world` takes of etxb_group_enqueue(iterations) in replica mode. */
-int etxb_debug_replica_plan(uint32_t world, uint32_t rank, uint32_t base, uint32_t iterations, int split_lane, uint32_t* out_triples, uint32_t capacity);
+/* Test hook (needs no device): the queues a `lanes`-lane group on rank `rank` of `world` holds after etxb_group_begin and one
+ * etxb_group_enqueue(enqueues[i]) per entry, in `mode` 0 (one GPU), 1 (pixel tiles) or 2 (replicas), with its last lane reserved for camera-split
+ * iterations if `split_lane`: (queue, ordinal, part, parts) quads, queue by queue in the order the lanes pop them; returns their number. */
+int etxb_debug_group_plan(uint32_t mode, uint32_t lanes, uint32_t world, uint32_t rank, int split_lane, const uint32_t* enqueues, uint32_t count,
+                          uint32_t* out_quads, uint32_t capacity);
 int etxb_group_comm_reduce_film(etxb_group* group, uint32_t layer, float* dst_rgba, uint64_t dst_bytes);        /* collective, both modes */
 
 #ifdef __cplusplus

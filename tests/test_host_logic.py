@@ -143,26 +143,40 @@ def test_bench_algorithmic_bytes_follow_the_survey_formula():
     assert total == sum(once.values())
 
 
-def test_replica_mode_deals_every_iteration_exactly_once():
-    """etxb_group_enqueue in replica mode (module.cu replica_plan, through the device-free test hook): whole frames round-robin; with a split lane
-    the n % world left-over iterations are split over world / (n % world) ranks each by camera tile.  Whatever (world, n): every ordinal is
-    rendered exactly once — by one rank as a whole frame, or by `parts` ranks holding the parts 0 .. parts - 1 — and no rank carries more than
-    ceil(n / world) units of work."""
-    import ctypes as C
+GROUP_LOCAL, GROUP_TILES, GROUP_REPLICAS = 0, 1, 2  # etxb_debug_group_plan's modes
+
+
+def _group_plan(lib, mode, lanes, world, rank, split, enqueues):
+    """The (queue, ordinal, part, parts) rows a group's work plan holds after these successive etxb_group_enqueue counts."""
+    counts = np.array(enqueues, dtype=np.uint32)
+    cap = int(counts.sum()) + 1
+    out = np.zeros((cap, 4), dtype=np.uint32)
+    k = lib.etxb_debug_group_plan(mode, lanes, world, rank, split, counts.ctypes.data_as(ctypes.c_void_p), len(counts), out.ctypes.data_as(ctypes.c_void_p), cap)
+    assert 0 <= k < cap, k
+    return out[:k].astype(np.int64)
+
+
+def test_work_plan_deals_every_iteration_exactly_once():
+    """etxb_group_enqueue's work plan (module.cu plan_enqueue, through the device-free test hook etxb_debug_group_plan).
+    Replica mode: whole frames round-robin; with a split lane the n % world left-over iterations are split over world / (n % world) ranks each by
+    camera tile.  Whatever (world, n): every ordinal is rendered exactly once — by one rank as a whole frame, or by `parts` ranks holding the
+    parts 0 .. parts - 1 — and no rank carries more than ceil(n / world) units of work.  Whole frames wait in queue 0, split parts in the split
+    lane's own queue.  Over several enqueues the split lane's film keeps one (part, parts) geometry.
+    One GPU: a single queue holding each ordinal once, in order.  Pixel tiles: queue l holds exactly the ordinals = l (mod lanes)."""
     from etx_tracer_b200 import api
     lib = api.load_library("fast")
-    lib.etxb_debug_replica_plan.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.c_void_p, C.c_uint32]
-    buf = np.zeros(3 * 256, dtype=np.uint32)
+    base, lanes = 840, 2  # a first enqueue every world 1..8 divides: dealt as whole frames, it leaves no split geometry behind
     for world in range(1, 9):
         for n in range(1, 41):
             for split in (0, 1):
                 whole, parts_seen, load = {}, {}, [0.0] * world
                 for rank in range(world):
-                    k = lib.etxb_debug_replica_plan(world, rank, 100, n, split, buf.ctypes.data_as(C.c_void_p), 256)
-                    assert k >= 0
-                    for i in range(k):
-                        j, part, parts = (int(v) for v in buf[i * 3:i * 3 + 3])
-                        assert 100 <= j < 100 + n
+                    rows = _group_plan(lib, GROUP_REPLICAS, lanes, world, rank, split, [base, n])
+                    first = rows[rows[:, 1] < base]
+                    assert len(first) == base // world and np.all(first[:, 0] == 0) and np.all(first[:, 3] == 1) and np.all(first[:, 1] % world == rank)
+                    for q, j, part, parts in rows[rows[:, 1] >= base]:
+                        assert base <= j < base + n
+                        assert q == (lanes - 1 if parts > 1 else 0)
                         if parts == 1:
                             whole[j] = whole.get(j, 0) + 1
                             load[rank] += 1.0
@@ -170,7 +184,7 @@ def test_replica_mode_deals_every_iteration_exactly_once():
                             assert split and n >= world and parts == world // (n % world) and parts >= 2
                             parts_seen.setdefault(j, []).append(part)
                             load[rank] += 1.0 / parts
-                for j in range(100, 100 + n):
+                for j in range(base, base + n):
                     if j in whole:
                         assert whole[j] == 1 and j not in parts_seen, (world, n, split, j)
                     else:
@@ -179,3 +193,44 @@ def test_replica_mode_deals_every_iteration_exactly_once():
                 assert max(load) <= -(-n // world) + 1e-9
                 if split and n >= world and n % world and world // (n % world) >= 2:
                     assert max(load) < -(-n // world)  # the point of the split: nobody a whole iteration behind
+
+    # replicas over two enqueues: a round is split only with the parts count of every earlier split round (one geometry per split lane's
+    # film), and a rank that took no part of the first split still takes its part of a later one
+    for world in range(2, 9):
+        for rounds in [(a, b) for a in range(1, 21) for b in range(1, 21)]:
+            done, geometry = {}, {}
+            for rank in range(world):
+                for q, j, part, parts in _group_plan(lib, GROUP_REPLICAS, 3, world, rank, 1, rounds):
+                    assert q == (2 if parts > 1 else 0)
+                    done.setdefault(j, []).append((part, parts))
+                    if parts > 1:
+                        geometry.setdefault(rank, set()).add((part, parts))
+            assert all(len(g) == 1 for g in geometry.values()), (world, rounds, geometry)
+            have, start, want = 0, 0, {}
+            for n in rounds:
+                rest = n % world if n >= world else 0
+                parts = world // rest if rest else 1
+                if parts >= 2 and have in (0, parts):
+                    have = parts
+                    want.update({j: parts for j in range(start + n - rest, start + n)})
+                start += n
+            assert sorted(done) == list(range(start))
+            for j, got in done.items():
+                assert sorted(got) == ([(p, want[j]) for p in range(want[j])] if j in want else [(0, 1)]), (world, rounds, j, got)
+
+    # one GPU: one queue, each ordinal once and in order; a reserved split lane's own queue stays empty
+    for lanes in range(1, 9):
+        for split in ((0, 1) if lanes >= 2 else (0,)):
+            assert _group_plan(lib, GROUP_LOCAL, lanes, 1, 0, split, [3, 5, 1, 7]).tolist() == [[0, j, 0, 1] for j in range(16)]
+
+    # pixel tiles: queue l holds exactly the ordinals = l (mod lanes), in order, on every rank, across enqueues
+    for lanes in range(1, 9):
+        total = 16 + lanes
+        for rank in (0, 1):
+            rows = _group_plan(lib, GROUP_TILES, lanes, 2, rank, 0, [3, 5, 1, 7, lanes])
+            assert len(rows) == total
+            for l in range(lanes):
+                assert rows[rows[:, 0] == l].tolist() == [[l, j, 0, 1] for j in range(l, total, lanes)]
+    out = np.zeros(4, dtype=np.uint32)
+    one = np.ones(1, dtype=np.uint32)
+    assert lib.etxb_debug_group_plan(GROUP_TILES, 2, 2, 0, 1, one.ctypes.data_as(ctypes.c_void_p), 1, out.ctypes.data_as(ctypes.c_void_p), 1) < 0
