@@ -103,6 +103,8 @@ def load_library(flavor="fast"):
     lib.etxb_set_partition.argtypes = [vp, u32, u32]
     lib.etxb_set_iteration_stride.argtypes = [vp, u32]
     lib.etxb_begin.argtypes = [vp, u32]
+    lib.etxb_set_film_pixel_size.argtypes = [vp, u32]
+    lib.etxb_group_set_film_pixel_size.argtypes = [vp, u32]
     lib.etxb_enqueue_iteration.argtypes = [vp]
     lib.etxb_enqueue_light_pass.argtypes = [vp]
     lib.etxb_enqueue_grid_build.argtypes = [vp, vp, u64]
@@ -373,6 +375,12 @@ class GPUVCM:
             out = np.zeros((self.height, self.width, 4), dtype=np.float32)
         self._check(self.lib.etxb_comm_reduce_film(self.h, layer, _p(out) if r.value == 0 else None, out.nbytes if r.value == 0 else 0))
         return out if r.value == 0 else None
+
+    def set_film_pixel_size(self, size):
+        """Film::set_pixel_size: the coarse preview the application renders while the camera moves (8), and full resolution (1).  Clamped to
+        [1, 1024]; takes effect at the next run() or update_scene().  At size s an iteration traces ceil(W / s) x ceil(H / s) paths and every
+        s x s block of the film takes its path's value; the film stays W x H."""
+        self._check(self.lib.etxb_set_film_pixel_size(self.h, size))
 
     def set_iteration_stride(self, stride):
         """This context renders iterations first, first + stride, ... (iteration-interleaved multi-GPU runs)."""
@@ -659,6 +667,10 @@ class GPUVCMGroup:
             if integrator == S.INTEGRATOR_PT:
                 g._check(self.lib.etxb_pt_set_options(g.h, _p(pt_options if pt_options is not None else S.default_pt_options())))
                 g._check(self.lib.etxb_set_scene_settings(g.h, C.c_float(0.0), C.c_float(float(self.scene_data.scene["radiance_clamp"][0]))))
+
+    def set_film_pixel_size(self, size):
+        """GPUVCM.set_film_pixel_size for every lane (etxb_group_set_film_pixel_size): applied by the next run() or update_scene()."""
+        self._check(self.lib.etxb_group_set_film_pixel_size(self.h, size))
 
     def set_options(self):
         """Pushes self.options (the Integrator options) to every lane."""

@@ -55,8 +55,10 @@ struct DeviceCounters {
 struct FilmBuffers {
   float4* camera;           // running mean over iterations (y-flipped storage like film.cxx:189)
   float4* light;            // running mean
-  float4* light_iteration;  // per-iteration splats
+  float4* light_iteration;  // per-iteration splats; at pixel size > 1 indexed by coarse cell (splat_prepare), expanded by k_film_commit_light
   uint32_t width, height;
+  uint32_t pixel_size;      // Film::pixel_size (1 = every pixel is a path's own)
+  uint32_t dims_x, dims_y;  // Film::dimensions(): ceil(width / pixel_size) x ceil(height / pixel_size)
 };
 
 struct LaunchParams {
@@ -75,7 +77,7 @@ struct LaunchParams {
   uint32_t* sampler_end_light;   // debug taps (ETXB_BUF_LIGHT_SAMPLER / CAMERA_SAMPLER)
   uint32_t* sampler_end_camera;
   float4* camera_value;          // ETXB_BUF_CAMERA_GATHERED
-  uint32_t path_count;           // N = W*H
+  uint32_t path_count;           // paths of the iteration: Film::pixel_count() = dims_x * dims_y (W * H at pixel size 1)
   uint32_t rank, world;          // pixel-tile partition
   uint32_t light_world;          // the light pass's partition: `world` (tiles over NCCL: every rank traces its own pixels' light paths) or 1 (a camera-split
                                  //    iteration: every part traces ALL light paths itself — the same photon map everywhere, nothing to exchange)
@@ -135,6 +137,17 @@ DEV void queue_push(uint32_t* queue, uint32_t* queue_count, bool alive, uint32_t
   if (lane == leader) base = atomicAdd(queue_count, __popc(ballot));
   base = __shfl_sync(mask, base, leader);
   if (alive) queue[base + __popc(ballot & ((1u << lane) - 1u))] = id;
+}
+
+// Film::active_pixel (film.cxx:434-461): the film pixel (x + y * width, unflipped) path i samples in `iteration` — its own at pixel size 1,
+// else a pixel of its block, origin offset by pm::preview_offset (portable_math.h) and clamped to the film
+DEV uint32_t film_path_pixel(const FilmBuffers& f, uint32_t i, uint32_t iteration) {
+  if (f.pixel_size == 1u) return i;
+  uint32_t dx = 0, dy = 0;
+  pm::preview_offset(i, iteration, f.pixel_size, dx, dy);
+  const uint32_t x = umin((i % f.dims_x) * f.pixel_size + dx, f.width - 1u);
+  const uint32_t y = umin((i / f.dims_x) * f.pixel_size + dy, f.height - 1u);
+  return x + y * f.width;
 }
 
 DEV bool pixel_owned(const LaunchParams& p, uint32_t index, bool light_pass = false) {
@@ -236,17 +249,18 @@ __global__ void __launch_bounds__(256) k_trace_closest(const __grid_constant__ L
 }
 
 // Film::atomic_add_light_iteration (film.cxx:147-171) of one light-tracing contribution (vcm_cpu.cxx:147-154), in two halves: value -> RGB and
-// pixel (false: below the driver's cut or off the film), then the three float atomics
+// pixel (false: below the driver's cut or off the film), then the three float atomics.  The pixel is a cell of Film::dimensions() (x * s >= W
+// exactly when x >= dims_x); at pixel size s > 1 k_film_commit_light spreads the cell over its s x s block as the reference's clamped loop does.
 template <bool SP>
 DEV bool splat_prepare(const LaunchParams& p, Spec<SP> value, V2 uv, float wavelength, V3& rgb, uint32_t& pixel, uint32_t& counted) {
   rgb = spec_to_rgb<SP>(p.scene, value, wavelength) / sampling_pdf<SP>(wavelength);
   if (!(dot(rgb, rgb) > kEpsilon)) return false;
   counted = 1u;
   V2 uv01 = uv * 0.5f + 0.5f;
-  uint32_t x = static_cast<uint32_t>(uv01.x * float(p.film.width));
-  uint32_t y = static_cast<uint32_t>(uv01.y * float(p.film.height));
-  if ((x >= p.film.width) || (y >= p.film.height)) return false;
-  pixel = x + (p.film.height - 1u - y) * p.film.width;
+  uint32_t x = static_cast<uint32_t>(uv01.x * float(p.film.dims_x));
+  uint32_t y = static_cast<uint32_t>(uv01.y * float(p.film.dims_y));
+  if ((x >= p.film.dims_x) || (y >= p.film.dims_y)) return false;
+  pixel = x + (p.film.dims_y - 1u - y) * p.film.dims_x;
   return true;
 }
 DEV void splat_add(const LaunchParams& p, uint32_t pixel, V3 rgb) {
@@ -563,7 +577,8 @@ __global__ void __launch_bounds__(128) k_camera_begin(const __grid_constant__ La
   if (i < p.path_count) {
     alive = pixel_owned(p, i);
     if (alive) {
-      uint32_t px = i % p.film.width, py = i / p.film.width;
+      const uint32_t pixel = film_path_pixel(p.film, i, p.vcm.iteration);
+      uint32_t px = pixel % p.film.width, py = pixel / p.film.width;
       PathState<SP> s = generate_camera_state<SP>(p.scene, p.vcm, px, py, i, p.paths.wavelength[i]);
       p.paths.wavelength[i] = s.wavelength;
       store_state<SP>(p.paths, i, s);
@@ -735,7 +750,8 @@ __global__ void __launch_bounds__(128, kBounceMinBlocksPerSm<PLAIN>) k_camera_sh
         rnd_connection = state.sampler.next_2d();
         rnd_support = state.sampler.next_2d();
         if (p.vcm.blue_noise && (state.total_path_depth == 1) && (p.vcm.iteration < 256u)) {
-          uint32_t px = i % p.film.width, py = i / p.film.width;
+          const uint32_t pixel = film_path_pixel(p.film, i, p.vcm.iteration);
+          uint32_t px = pixel % p.film.width, py = pixel / p.film.width;
           rnd_bsdf = sample_blue_noise(sc, px, py, p.vcm.iteration, 0);
           rnd_connection = sample_blue_noise(sc, px, py, p.vcm.iteration, 2);
           rnd_support = sample_blue_noise(sc, px, py, p.vcm.iteration, 4);
@@ -1576,21 +1592,24 @@ __global__ void __launch_bounds__(128) k_camera_continue(const __grid_constant__
     if (alive) {
       store_state<SP>(p.paths, i, state);
     } else {
-      // vcm_cpu.cxx:195-198 + Film::accumulate_camera_image (film.cxx:173-230, camera layer)
+      // vcm_cpu.cxx:195-198 + Film::accumulate_camera_image (film.cxx:173-230, camera layer); at pixel size > 1 k_film_fill_blocks fills
+      // the path's block from camera_value
       float4 g = p.paths.gathered[i], mg = p.paths.merged[i];
       V3 merged = {mg.x, mg.y, mg.z};
       merged *= p.vcm.vm_normalization;
       merged += spec_to_rgb<SP>(sc, Spec<SP>::make3({g.x, g.y, g.z}) / sampling_pdf<SP>(state.wavelength), state.wavelength);
-      uint32_t px = i % p.film.width, py = i / p.film.width;
-      uint32_t fi = px + (p.film.height - 1u - py) * p.film.width;
-      float4 old = p.film.camera[fi];
-      V3 result = merged;
-      if (p.camera_sample_index != 0u) {
-        double ds = double(p.camera_sample_index);
-        float t = float(ds / (ds + 1.0));
-        result = {lerpf(merged.x, old.x, t), lerpf(merged.y, old.y, t), lerpf(merged.z, old.z, t)};
+      if (p.film.pixel_size == 1u) {
+        uint32_t px = i % p.film.width, py = i / p.film.width;
+        uint32_t fi = px + (p.film.height - 1u - py) * p.film.width;
+        float4 old = p.film.camera[fi];
+        V3 result = merged;
+        if (p.camera_sample_index != 0u) {
+          double ds = double(p.camera_sample_index);
+          float t = float(ds / (ds + 1.0));
+          result = {lerpf(merged.x, old.x, t), lerpf(merged.y, old.y, t), lerpf(merged.z, old.z, t)};
+        }
+        p.film.camera[fi] = make_float4(result.x, result.y, result.z, 1.0f);
       }
-      p.film.camera[fi] = make_float4(result.x, result.y, result.z, 1.0f);
       p.sampler_end_camera[i] = state.sampler.seed;
       p.camera_value[i] = make_float4(merged.x, merged.y, merged.z, 0.0f);
     }
@@ -1601,15 +1620,29 @@ __global__ void __launch_bounds__(128) k_camera_continue(const __grid_constant__
 // ---------------------------------------------------------------------------------------------------------------------
 // film (film.cxx:332-343, 381-418)
 // ---------------------------------------------------------------------------------------------------------------------
+// At pixel size s > 1 the splats sit in coarse cells (splat_prepare): the reference adds a splat to the s x s pixels of the cell's block with
+// coordinates clamped to the film, so the last column / row of a partial block receives it once per clamped position.  Pixel i takes its
+// cell's sum times that count; the host clears the cells after this kernel.
 __global__ void __launch_bounds__(256) k_film_commit_light(const __grid_constant__ FilmBuffers film, uint32_t iteration_index) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= film.width * film.height) return;
   float t = float(double(iteration_index) / double(iteration_index + 1u));
-  float4 s = film.light_iteration[i], d = film.light[i];
+  float4 s, d = film.light[i];
+  if (film.pixel_size == 1u) {
+    s = film.light_iteration[i];
+    film.light_iteration[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+  } else {
+    const uint32_t n = film.pixel_size, px = i % film.width, py = film.height - 1u - i / film.width;
+    const uint32_t bx = px / n, by = py / n;
+    const uint32_t mx = (px == film.width - 1u) ? (bx * n + n - px) : 1u;
+    const uint32_t my = (py == film.height - 1u) ? (by * n + n - py) : 1u;
+    const float k = float(mx * my);
+    float4 c = film.light_iteration[bx + (film.dims_y - 1u - by) * film.dims_x];
+    s = make_float4(c.x * k, c.y * k, c.z * k, 0.0f);
+  }
   V3 sv = {s.x, s.y, s.z}, dv = {d.x, d.y, d.z};
   V3 r = (t == 0.0f) ? sv : lerp3(sv, dv, t);
   film.light[i] = make_float4(r.x, r.y, r.z, 1.0f);
-  film.light_iteration[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
 }
 
 __global__ void __launch_bounds__(256) k_film_resolve(const __grid_constant__ FilmBuffers film, float4* out) {

@@ -59,21 +59,23 @@ DEV PtState<SP> pt_load(const PathBuffers& b, uint32_t i) {
   return s;
 }
 
+// storage index (y-flipped) of film pixel i = x + y * width
 DEV uint32_t pt_film_index(const FilmBuffers& film, uint32_t i) {
   uint32_t px = i % film.width, py = i / film.width;
   return px + (film.height - 1u - py) * film.width;
 }
 
-// make_ray_payload for every active pixel (path_tracing.cxx:57-62; Film::active_pixel with pixel_size == 1: a converged pixel is skipped)
+// make_ray_payload for every active pixel (path_tracing.cxx:57-62; Film::active_pixel: a path whose pixel has converged is skipped)
 template <bool SP>
 __global__ void __launch_bounds__(128) k_pt_begin(const __grid_constant__ LaunchParams p, const __grid_constant__ PtParams pt, const __grid_constant__ PtFilm pf, uint32_t* queue,
                                                   uint32_t* queue_count) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   bool alive = false;
   if (i < p.path_count) {
-    alive = pixel_owned(p, i) && ((pf.info[pt_film_index(p.film, i)] & kPtConverged) == 0u);
+    const uint32_t pixel = film_path_pixel(p.film, i, pt.iteration);
+    alive = pixel_owned(p, pixel) && ((pf.info[pt_film_index(p.film, pixel)] & kPtConverged) == 0u);
     if (alive) {
-      PtState<SP> s = pt_make_payload<SP>(p.scene, pt, i % p.film.width, i / p.film.width, i);
+      PtState<SP> s = pt_make_payload<SP>(p.scene, pt, pixel % p.film.width, pixel / p.film.width, i);
       p.paths.wavelength[i] = s.wavelength;
       pt_store<SP>(p.paths, i, s);
       p.paths.bs_weight_pdf[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
@@ -132,7 +134,8 @@ __global__ void __launch_bounds__(128, kBounceMinBlocksPerSm<PLAIN>) k_pt_shade(
         deferred = &batch;
       }
       const bool first = s.path_length == 1u;
-      alive = pt_handle_hit_ray<SP, PLAIN>(sc, pt, isect, i % p.film.width, i / p.film.width, s, stats, shadow_rays, deferred);
+      const uint32_t pixel = film_path_pixel(p.film, i, pt.iteration);
+      alive = pt_handle_hit_ray<SP, PLAIN>(sc, pt, isect, pixel % p.film.width, pixel / p.film.width, s, stats, shadow_rays, deferred);
       if (first) {
         V3 a = s.view_albedo.as_v3();
         p.paths.bs_weight_pdf[i] = make_float4(a.x, a.y, a.z, 0.0f);
@@ -155,14 +158,16 @@ __global__ void __launch_bounds__(128, kBounceMinBlocksPerSm<PLAIN>) k_pt_shade(
 
 // The end of execute_range's loop body (path_tracing.cxx:68-81) + Film::accumulate_camera_image (film.cxx:173-230) for every pixel that was
 // active in this iteration: colour, normal and albedo running means, the every-other-sample mean the noise estimate compares against, the
-// per-pixel sample counter.
+// per-pixel sample counter.  At pixel size > 1 the path leaves colour (camera_value), albedo (bs_weight_pdf) and normal (bs_wo_eta) for
+// k_film_fill_blocks.
 template <bool SP>
 __global__ void __launch_bounds__(256) k_pt_accumulate(const __grid_constant__ LaunchParams p, const __grid_constant__ PtParams pt, const __grid_constant__ PtFilm pf) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= p.path_count) return;
-  const uint32_t fi = pt_film_index(p.film, i);
+  const uint32_t pixel = film_path_pixel(p.film, i, pt.iteration);
+  const uint32_t fi = pt_film_index(p.film, pixel);
   const uint32_t info = pf.info[fi];
-  if (!pixel_owned(p, i) || (info & kPtConverged)) return;
+  if (!pixel_owned(p, pixel) || (info & kPtConverged)) return;
   const float wavelength = p.paths.wavelength[i];
   float4 acc = p.paths.gathered[i], alb = p.paths.bs_weight_pdf[i], nrm = p.paths.bs_wo_eta[i];
   const float pdf = sampling_pdf<SP>(wavelength);
@@ -172,6 +177,11 @@ __global__ void __launch_bounds__(256) k_pt_accumulate(const __grid_constant__ L
   if ((pt.radiance_clamp > 0.0f) && (p.paths.misc[i].y > 1u)) {
     float lum = luminance(color);
     if (lum > pt.radiance_clamp) color *= pt.radiance_clamp / lum;
+  }
+  if (p.film.pixel_size != 1u) {
+    p.paths.bs_weight_pdf[i] = make_float4(albedo.x, albedo.y, albedo.z, 0.0f);
+    p.camera_value[i] = make_float4(color.x, color.y, color.z, 0.0f);
+    return;
   }
   const uint32_t sample_index = info & kPtCountMask;
   float4 c_old = p.film.camera[fi], n_old = pf.normals[fi], a_old = pf.albedo[fi], v_old = pf.adaptive[fi];
@@ -194,6 +204,52 @@ __global__ void __launch_bounds__(256) k_pt_accumulate(const __grid_constant__ L
   pf.adaptive[fi] = make_float4(v.x, v.y, v.z, 1.0f);
   pf.info[fi] = (info & ~kPtCountMask) | ((sample_index + 1u) & kPtCountMask);
   p.camera_value[i] = make_float4(color.x, color.y, color.z, 0.0f);
+}
+
+// Film::accumulate_camera_image at pixel size s > 1 (film.cxx:173-230): the reference loops over the block of the path's pixel, clipped to
+// the film; here every film pixel reads its block's path and lerps with its own sample count — coalesced writes, the same cost for any s.
+// VCM: the camera layer, every block every iteration.  PT: also normal, albedo, the every-other-sample mean and the count, for the blocks
+// whose path ran (its chosen pixel had not converged; the other pixels of the block are not tested, as in the reference).
+template <bool PT>
+__global__ void __launch_bounds__(256) k_film_fill_blocks(const __grid_constant__ LaunchParams p, const __grid_constant__ PtFilm pf, uint32_t iteration) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  const FilmBuffers& film = p.film;
+  if (i >= film.width * film.height) return;
+  const uint32_t px = i % film.width, py = film.height - 1u - i / film.width;
+  const uint32_t path = (px / film.pixel_size) + (py / film.pixel_size) * film.dims_x;
+  uint32_t sample_index = p.camera_sample_index, info = 0u;
+  if constexpr (PT) {
+    if (pf.info[pt_film_index(film, film_path_pixel(film, path, iteration))] & kPtConverged) return;
+    info = pf.info[i];
+    sample_index = info & kPtCountMask;
+  }
+  const float4 cv = p.camera_value[path];
+  const V3 color = {cv.x, cv.y, cv.z};
+  const float4 c_old = film.camera[i];
+  V3 c = color;
+  double ds = double(sample_index);
+  float t = float(ds / (ds + 1.0));
+  if (sample_index != 0u) c = {lerpf(color.x, c_old.x, t), lerpf(color.y, c_old.y, t), lerpf(color.z, c_old.z, t)};
+  film.camera[i] = make_float4(c.x, c.y, c.z, 1.0f);
+  if constexpr (PT) {
+    const float4 nrm = p.paths.bs_wo_eta[path], alb = p.paths.bs_weight_pdf[path];
+    const V3 normal = {nrm.x, nrm.y, nrm.z}, albedo = {alb.x, alb.y, alb.z};
+    const float4 n_old = pf.normals[i], a_old = pf.albedo[i], v_old = pf.adaptive[i];
+    V3 n = normal, a = albedo, v = color;
+    if (sample_index != 0u) {
+      n = {lerpf(normal.x, n_old.x, t), lerpf(normal.y, n_old.y, t), lerpf(normal.z, n_old.z, t)};
+      a = {lerpf(albedo.x, a_old.x, t), lerpf(albedo.y, a_old.y, t), lerpf(albedo.z, a_old.z, t)};
+      v = {v_old.x, v_old.y, v_old.z};
+      if ((sample_index % 2u) == 0u) {
+        t = float(ds / (ds + 2.0));
+        v = {lerpf(color.x, v_old.x, t), lerpf(color.y, v_old.y, t), lerpf(color.z, v_old.z, t)};
+      }
+    }
+    pf.normals[i] = make_float4(n.x, n.y, n.z, 1.0f);
+    pf.albedo[i] = make_float4(a.x, a.y, a.z, 1.0f);
+    pf.adaptive[i] = make_float4(v.x, v.y, v.z, 1.0f);
+    pf.info[i] = (info & ~kPtCountMask) | ((sample_index + 1u) & kPtCountMask);
+  }
 }
 
 // Film::estimate_noise_levels (film.cxx:233-330), first pass: error level of every pixel that has not converged, the convergence decision, and

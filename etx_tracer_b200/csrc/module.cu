@@ -200,8 +200,10 @@ struct etxb_ctx {
   double bvh_build_seconds = 0.0;
   SceneHashes hashes;
 
-  // per-path state + queues
-  uint32_t width = 0, height = 0, path_count = 0;
+  // per-path state + queues.  path_count = W * H sizes the film and every path-indexed buffer; launch_count = Film::pixel_count() is the
+  // number of paths an iteration traces: W * H at pixel size 1, ceil(W / s) * ceil(H / s) in the coarse preview
+  uint32_t width = 0, height = 0, path_count = 0, launch_count = 0;
+  uint32_t pixel_size = 1, target_pixel_size = 1;  // Film::pixel_size, and the one etxb_set_film_pixel_size stored for the next etxb_begin
   DevBuf<float4> ray_o, ray_d, thr, mis, hit, gathered, merged, camera_value, bs_weight_pdf, bs_wo_eta;
   DevBuf<uint4> misc;
   DevBuf<uint2> bs_props;
@@ -527,12 +529,16 @@ uint32_t next_pow2(uint64_t v) {
   return uint32_t(v);
 }
 
+// Film::dimensions() (film.cxx:373-379)
+uint32_t film_dims_x(const etxb_ctx* ctx) { return (ctx->width + ctx->pixel_size - 1u) / ctx->pixel_size; }
+uint32_t film_dims_y(const etxb_ctx* ctx) { return (ctx->height + ctx->pixel_size - 1u) / ctx->pixel_size; }
+
 LaunchParams make_params(etxb_ctx* ctx) {
   LaunchParams p = {};
   p.scene = ctx->dscene;
   p.paths = {ctx->ray_o.ptr, ctx->ray_d.ptr, ctx->thr.ptr, ctx->mis.ptr, ctx->misc.ptr, ctx->hit.ptr, ctx->gathered.ptr, ctx->merged.ptr, ctx->wavelength.ptr,
     ctx->lv_count.ptr, ctx->bs_weight_pdf.ptr, ctx->bs_wo_eta.ptr, ctx->bs_props.ptr, ctx->merge_key.ptr, ctx->conn_rec.ptr};
-  p.film = {ctx->film_camera.ptr, ctx->film_light.ptr, ctx->film_light_iteration.ptr, ctx->width, ctx->height};
+  p.film = {ctx->film_camera.ptr, ctx->film_light.ptr, ctx->film_light_iteration.ptr, ctx->width, ctx->height, ctx->pixel_size, film_dims_x(ctx), film_dims_y(ctx)};
   p.grid = ctx->grid;
   p.lv_tmp = ctx->lv_tmp.ptr;
   p.lv_final = ctx->lv_final.ptr;
@@ -544,7 +550,7 @@ LaunchParams make_params(etxb_ctx* ctx) {
   p.sampler_end_light = ctx->sampler_end_light.ptr;
   p.sampler_end_camera = ctx->sampler_end_camera.ptr;
   p.camera_value = ctx->camera_value.ptr;
-  p.path_count = ctx->path_count;
+  p.path_count = ctx->launch_count;
   p.rank = ctx->rank;
   p.world = ctx->world;
   p.light_world = ctx->light_full ? 1u : ctx->world;
@@ -572,7 +578,8 @@ LaunchParams make_params(etxb_ctx* ctx) {
 #else
   p.connect_stage = ctx->has_stochastic_merge ? 1u : 0u;
 #endif
-  // start_next_iteration (vcm_cpu.cxx:95-113)
+  // start_next_iteration (vcm_cpu.cxx:95-113): the radius from dimensions() * pixel_size() (wider than the film when a side is not a multiple
+  // of the pixel size), eta_vcm from pixel_count()
   VcmParams& v = p.vcm;
   v.options = ctx->options.options;
   v.kernel = ctx->options.kernel;
@@ -580,12 +587,12 @@ LaunchParams make_params(etxb_ctx* ctx) {
   v.iteration = ctx->iteration;
   float used_radius = ctx->options.initial_radius;
   if (used_radius == 0.0f) {
-    uint32_t max_dim = std::max(ctx->width, ctx->height);
+    uint32_t max_dim = std::max(film_dims_x(ctx) * ctx->pixel_size, film_dims_y(ctx) * ctx->pixel_size);
     used_radius = 5.0f * ctx->dscene.bounding_sphere_radius / float(max_dim);
   }
   float radius_scale = 1.0f / (1.0f + float(ctx->iteration) / float(ctx->options.radius_decay));
   v.current_radius = used_radius * radius_scale;
-  float eta_vcm = kPi * (v.current_radius * v.current_radius) * float(ctx->path_count);
+  float eta_vcm = kPi * (v.current_radius * v.current_radius) * float(ctx->launch_count);
   v.vc_weight = 1.0f / eta_vcm;
   v.vm_weight = (ctx->options.options & ETXB_VCM_ENABLE_MERGING) ? eta_vcm : 0.0f;
   v.vm_normalization = 1.0f / eta_vcm;
@@ -692,7 +699,7 @@ int run_light_pass(etxb_ctx* ctx) {
   auto begin = [&](uint32_t* queue, uint32_t* count) -> int {
     CUDA_OK(ctx, cudaMemsetAsync(ctx->lv_tmp_count.ptr, 0, 4, ctx->stream));
     LaunchTimer t(ctx, K_LIGHT_BEGIN);
-    k_light_begin<SP><<<blocks_for(ctx->path_count, 128), 128, 0, ctx->stream>>>(p, queue, count);
+    k_light_begin<SP><<<blocks_for(ctx->launch_count, 128), 128, 0, ctx->stream>>>(p, queue, count);
     return ETXB_OK;
   };
   auto bounce = [&](const uint32_t* q, const uint32_t* count, uint32_t* next_queue, uint32_t* next_count, uint32_t active) -> int {
@@ -720,7 +727,7 @@ int run_light_pass(etxb_ctx* ctx) {
   {
     LaunchTimer t(ctx, K_LV_SCAN);
     size_t temp_bytes = ctx->cub_temp.bytes();
-    CUDA_OK(ctx, cub::DeviceScan::ExclusiveSum(ctx->cub_temp.ptr, temp_bytes, ctx->lv_count.ptr, ctx->lp_offset.ptr, int(ctx->path_count), ctx->stream));
+    CUDA_OK(ctx, cub::DeviceScan::ExclusiveSum(ctx->cub_temp.ptr, temp_bytes, ctx->lv_count.ptr, ctx->lp_offset.ptr, int(ctx->launch_count), ctx->stream));
   }
   if (total > 0) {
     LaunchTimer t(ctx, K_LV_REORDER);
@@ -745,6 +752,7 @@ int run_grid_build(etxb_ctx* ctx, const LightVertexRec* records, uint32_t count)
     // which always starts at 0; after etxb_begin(ctx, k != 0) or with interleaved iterations the absolute index would scale the first
     // commit by 1/(k+1) against a cleared film)
     k_film_commit_light<<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(p.film, ctx->completed);
+    if (ctx->pixel_size != 1u) CUDA_OK(ctx, cudaMemsetAsync(ctx->film_light_iteration.ptr, 0, size_t(ctx->launch_count) * 16u, ctx->stream));
   }
   bool merging = (ctx->options.options & ETXB_VCM_ENABLE_MERGING) && (ctx->options.options & ETXB_VCM_MERGE_VERTICES);
   if (!merging || (count == 0)) return ETXB_OK;
@@ -852,7 +860,7 @@ int run_camera_pass(etxb_ctx* ctx) {
   const bool merging = (ctx->options.options & ETXB_VCM_ENABLE_MERGING) && (ctx->options.options & ETXB_VCM_MERGE_VERTICES);
   auto begin = [&](uint32_t* queue, uint32_t* count) -> int {
     LaunchTimer t(ctx, K_CAMERA_BEGIN);
-    k_camera_begin<SP><<<blocks_for(ctx->path_count, 128), 128, 0, ctx->stream>>>(p, queue, count);
+    k_camera_begin<SP><<<blocks_for(ctx->launch_count, 128), 128, 0, ctx->stream>>>(p, queue, count);
     return ETXB_OK;
   };
   auto bounce = [&](const uint32_t* q, const uint32_t* count, uint32_t* next_queue, uint32_t* next_count, uint32_t active) -> int {
@@ -915,7 +923,13 @@ int run_camera_pass(etxb_ctx* ctx) {
     k_camera_continue<SP><<<blocks_for(active, 128), 128, 0, ctx->stream>>>(p, q, count, next_queue, next_count);
     return ETXB_OK;
   };
-  return run_bounces(ctx, p, K_TRACE_CAMERA, begin, bounce);
+  if (int rc = run_bounces(ctx, p, K_TRACE_CAMERA, begin, bounce)) return rc;
+  if (ctx->pixel_size != 1u) {
+    LaunchTimer t(ctx, K_CAMERA_CONTINUE);
+    k_film_fill_blocks<false><<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(p, PtFilm{}, ctx->iteration);
+  }
+  CUDA_OK(ctx, cudaGetLastError());
+  return ETXB_OK;
 }
 
 // Pixel-tile sharding (SURVEY 8(e), north star): between the light pass and the grid build of an iteration the ranks exchange what is global —
@@ -1068,7 +1082,7 @@ int run_pt_iteration(etxb_ctx* ctx) {
   PtFilm pf = make_pt_film(ctx);
   auto begin = [&](uint32_t* queue, uint32_t* count) -> int {
     LaunchTimer t(ctx, K_PT_BEGIN);
-    k_pt_begin<SP><<<blocks_for(ctx->path_count, 128), 128, 0, ctx->stream>>>(p, pt, pf, queue, count);
+    k_pt_begin<SP><<<blocks_for(ctx->launch_count, 128), 128, 0, ctx->stream>>>(p, pt, pf, queue, count);
     return ETXB_OK;
   };
   auto bounce = [&](const uint32_t* q, const uint32_t* count, uint32_t* next_queue, uint32_t* next_count, uint32_t active) -> int {
@@ -1086,7 +1100,8 @@ int run_pt_iteration(etxb_ctx* ctx) {
   if (int rc = run_bounces(ctx, p, K_TRACE_CAMERA, begin, bounce, &ctx->pt_pixels_processed)) return rc;
   {
     LaunchTimer t(ctx, K_PT_ACCUMULATE);
-    k_pt_accumulate<SP><<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(p, pt, pf);
+    k_pt_accumulate<SP><<<blocks_for(ctx->launch_count, 256), 256, 0, ctx->stream>>>(p, pt, pf);
+    if (ctx->pixel_size != 1u) k_film_fill_blocks<true><<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(p, pf, ctx->iteration);
   }
   if (int rc = pt_estimate_noise_levels(ctx, ctx->iteration)) return rc;
   CUDA_OK(ctx, cudaGetLastError());
@@ -1822,11 +1837,11 @@ void group_worker(etxb_group* grp, uint32_t lane) {
 }
 
 // A call the group refuses in its present state: the reason goes to etxb_group_last_error and to lane 0's etxb_last_error
-int group_refuse(etxb_group* grp, const char* why) {
-  fail(grp->lanes[0], ETXB_ERR_INVALID_ARGUMENT, "%s", why);
+int group_refuse(etxb_group* grp, const char* why, int code = ETXB_ERR_INVALID_ARGUMENT) {
+  fail(grp->lanes[0], code, "%s", why);
   std::lock_guard<std::mutex> lock(grp->m);
   grp->error_text = why;
-  return ETXB_ERR_INVALID_ARGUMENT;
+  return code;
 }
 
 int group_combine_into(etxb_group* grp, uint32_t layer, DevBuf<float4>& target, uint32_t* completed, bool raw = false) {
@@ -2033,6 +2048,7 @@ int etxb_set_options(etxb_ctx* ctx, const etxb_vcm_options* opt) {
 
 int etxb_set_partition(etxb_ctx* ctx, uint32_t rank, uint32_t world) {
   if (!ctx || world == 0 || rank >= world) return ETXB_ERR_INVALID_ARGUMENT;
+  if ((world > 1u) && (ctx->target_pixel_size > 1u)) return fail(ctx, ETXB_ERR_UNSUPPORTED, "etxb_set_partition: pixel tiles and a film pixel size above 1 exclude each other");
   ctx->rank = rank;
   ctx->world = world;
   return ETXB_OK;
@@ -2048,6 +2064,15 @@ int etxb_set_next_iteration(etxb_ctx* ctx, uint32_t iteration) {
   if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;
   ctx->iteration = iteration;
   ctx->iteration_stride = 0;  // externally driven: no auto-advance, the film mean counts this context's own iterations
+  return ETXB_OK;
+}
+
+int etxb_set_film_pixel_size(etxb_ctx* ctx, uint32_t size) {
+  if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;
+  size = std::min(std::max(size, 1u), 1024u);  // Film::set_pixel_size (film.cxx:483-485)
+  if ((size > 1u) && ((ctx->comm != nullptr) || (ctx->world > 1u)))
+    return fail(ctx, ETXB_ERR_UNSUPPORTED, "etxb_set_film_pixel_size: pixel tiles index film pixels; the coarse preview renders on one GPU");
+  ctx->target_pixel_size = size;
   return ETXB_OK;
 }
 
@@ -2069,8 +2094,11 @@ int etxb_begin(etxb_ctx* ctx, uint32_t first_iteration) {
     DevBuf<float4>* layers[] = {&ctx->film_normals, &ctx->film_albedo, &ctx->film_adaptive};
     for (auto* b : layers) CUDA_OK(ctx, cudaMemsetAsync(b->ptr, 0, n * 16, ctx->stream));
   }
+  // Film::clear applies the stored pixel size (film.cxx:365)
+  ctx->pixel_size = ctx->target_pixel_size;
+  ctx->launch_count = film_dims_x(ctx) * film_dims_y(ctx);
   ctx->pt_pixels_processed = 0;
-  ctx->pt_active_pixels = ctx->path_count;
+  ctx->pt_active_pixels = ctx->launch_count;
   ctx->pt_noise_level = 0.0f;
   CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
   ctx->iteration = first_iteration;
@@ -2202,6 +2230,7 @@ int etxb_comm_unique_id(void* out_id, uint64_t bytes) {
 int etxb_comm_init(etxb_ctx* ctx, uint32_t world, uint32_t rank, const void* id, uint64_t bytes) {
   if (!ctx || !id || (bytes < sizeof(ncclUniqueId)) || (world == 0u) || (rank >= world)) return ETXB_ERR_INVALID_ARGUMENT;
   if (ctx->comm != nullptr) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "the context already has a communicator");
+  if (ctx->target_pixel_size > 1u) return fail(ctx, ETXB_ERR_UNSUPPORTED, "etxb_comm_init: the coarse preview (film pixel size above 1) renders on one GPU");
   cudaSetDevice(ctx->device);
   if (int rc = comm_init_rank(ctx, &ctx->comm, world, rank, id)) return rc;
   ctx->rank = rank;
@@ -2759,6 +2788,21 @@ int etxb_group_begin(etxb_group* grp, uint32_t first_iteration) {
   return ETXB_OK;
 }
 
+int etxb_group_set_film_pixel_size(etxb_group* grp, uint32_t size) {
+  if (!grp) return ETXB_ERR_INVALID_ARGUMENT;
+  if ((size > 1u) && ((grp->plan.mode != GroupMode::local) || (grp->reduce_comm != nullptr)))
+    return group_refuse(grp, "etxb_group_set_film_pixel_size: a group with communicators renders film pixels in tiles or parts; the coarse preview renders on one GPU", ETXB_ERR_UNSUPPORTED);
+  if (int rc = etxb_group_wait(grp)) return rc;
+  for (auto* c : grp->lanes) {
+    if (int rc = etxb_set_film_pixel_size(c, size)) {
+      std::lock_guard<std::mutex> lock(grp->m);
+      grp->error_text = etxb_last_error(c);
+      return rc;
+    }
+  }
+  return ETXB_OK;
+}
+
 int etxb_group_update_scene(etxb_group* grp, const void* scene_blob, uint64_t scene_bytes, const void* camera_blob, uint64_t camera_bytes, etxb_update_info* info) {
   const auto t0 = std::chrono::steady_clock::now();
   if (info) memset(info, 0, sizeof(*info));
@@ -2858,6 +2902,8 @@ int etxb_group_comm_init(etxb_group* grp, uint32_t world, uint32_t rank, const v
   if (int rc = etxb_group_wait(grp)) return rc;
   if (grp->reduce_comm != nullptr) return group_refuse(grp, "etxb_group_comm_init: the group already has a communicator");
   if ((world > 1u) && (grp->plan.split_lane != 0xffffffffu)) return group_refuse(grp, "etxb_group_comm_init: pixel tiles and a split lane exclude each other");
+  for (auto* c : grp->lanes)
+    if (c->target_pixel_size > 1u) return group_refuse(grp, "etxb_group_comm_init: the coarse preview (film pixel size above 1) renders on one GPU", ETXB_ERR_UNSUPPORTED);
   const uint8_t* bytes = static_cast<const uint8_t*>(ids);
   for (size_t l = 0; l < grp->lanes.size(); ++l) {
     if (int rc = etxb_comm_init(grp->lanes[l], world, rank, bytes + l * sizeof(ncclUniqueId), sizeof(ncclUniqueId))) {
@@ -2919,6 +2965,8 @@ int etxb_group_comm_init_replicas(etxb_group* grp, uint32_t world, uint32_t rank
   if (!grp || !id || (bytes < sizeof(ncclUniqueId)) || (world == 0u) || (rank >= world)) return ETXB_ERR_INVALID_ARGUMENT;
   if (int rc = etxb_group_wait(grp)) return rc;
   if (grp->reduce_comm != nullptr) return group_refuse(grp, "etxb_group_comm_init_replicas: the group already has a communicator");
+  for (auto* c : grp->lanes)
+    if (c->target_pixel_size > 1u) return group_refuse(grp, "etxb_group_comm_init_replicas: the coarse preview (film pixel size above 1) renders on one GPU", ETXB_ERR_UNSUPPORTED);
   cudaSetDevice(grp->device);
   if (int rc = comm_init_rank(grp->lanes[0], &grp->reduce_comm, world, rank, id)) return rc;
   std::lock_guard<std::mutex> lock(grp->m);

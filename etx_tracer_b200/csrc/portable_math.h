@@ -53,6 +53,25 @@ PM_FN double abs_d(double x) { return bits_to_double(double_to_bits(x) & 0x7ffff
 PM_FN bool sign_d(double x) { return (double_to_bits(x) >> 63) != 0; }
 PM_FN bool is_inf(double x) { return abs_d(x) == inf_d(); }
 
+// The coarse preview's pixel offset inside an s x s block for path `index` of `iteration` (include/etx_b200.h, etxb_set_film_pixel_size): the
+// reference draws it from rand(); here x is the first 32-bit value of a hash of (index, iteration) and y the second, each % s, so that an
+// iteration stays a function of its index.  Shared like the transcendentals: the device and the oracle call this one definition.  The
+// mixer is Wellons' "lowbias32".
+PM_FN uint32_t preview_hash(uint32_t x) {
+  x ^= x >> 16;
+  x *= 0x7feb352du;
+  x ^= x >> 15;
+  x *= 0x846ca68bu;
+  x ^= x >> 16;
+  return x;
+}
+PM_FN void preview_offset(uint32_t index, uint32_t iteration, uint32_t size, uint32_t& dx, uint32_t& dy) {
+  const uint32_t first = preview_hash(index ^ preview_hash(iteration ^ 0x9e3779b9u));
+  const uint32_t second = preview_hash(first ^ 0x85ebca6bu);
+  dx = first % size;
+  dy = second % size;
+}
+
 // 2^k for k in [-1022, 1023]
 PM_FN double pow2i(int k) { return bits_to_double(uint64_t(k + 1023) << 52); }
 

@@ -71,6 +71,15 @@ class IntegratorAdapter {
     if (was_running) run();
     return rc;
   }
+  // Film::set_pixel_size + restart, as the application does when the camera starts (8) and stops (1) moving (app.cxx:131-141): the size is
+  // taken by the next run(), which a running render gets at once
+  int set_film_pixel_size(uint32_t size) {
+    if (!enabled()) return _create_result;
+    const bool was_running = (_state.load() != State::Stopped);
+    int rc = etxb_set_film_pixel_size(_ctx, size);
+    if ((rc == ETXB_OK) && was_running) run();
+    return rc;
+  }
   int upload_tables(const float* xyz_441x3, const float* rgb_response_391x3, const uint8_t* sobol, const uint8_t* scrambling, const uint8_t* ranking) {
     if (!enabled()) return _create_result;
     int rc = etxb_upload_color_tables(_ctx, xyz_441x3, rgb_response_391x3);

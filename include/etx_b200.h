@@ -366,6 +366,21 @@ int etxb_set_next_iteration(etxb_ctx* ctx, uint32_t iteration);
 /* CPUVCMImpl::start (vcm_cpu.cxx:81-93): clears film, sets iteration = first_iteration. */
 int etxb_begin(etxb_ctx* ctx, uint32_t first_iteration);
 
+/* ---- coarse preview: Film pixel size (film.cxx:147-230, 345-461) ------------------------------------------------------------------
+ * Film::set_pixel_size: the size is clamped to [1, 1024] and takes effect at the next etxb_begin (or etxb_update_scene, which ends in
+ * it), like Film::clear.  At pixel size s both integrators trace Film::pixel_count() = ceil(W / s) x ceil(H / s) paths per iteration,
+ * path i in the s x s block (i % ceil(W / s), i / ceil(W / s)); the block's pixels each take the path's value with their own sample count.
+ * The film and every layer stay W x H; the path-indexed buffers (ETXB_BUF_*_SAMPLER, _LIGHT_PATH_*, _CAMERA_GATHERED) keep W x H
+ * entries, of which the first Film::pixel_count() belong to the iteration.  The application previews with 8 while the camera moves and
+ * goes back to 1 when it stops (app.cxx:131-141).  Refused (ETXB_ERR_UNSUPPORTED) above 1 on a context with a communicator or a pixel
+ * partition, and on a group with communicators: tiles and replica splits index film pixels.  Which pixel of its block a path
+ * samples is the one departure from the reference: Film::active_pixel offsets the block origin by rand() % s in x and then in y, and rand()
+ * is process-global state called from worker threads in timing-dependent order, so no run of the reference can be repeated.  Here the
+ * offset is a hash of (path index, iteration) — x from a first 32-bit value, y from a second, each % s (pm::preview_offset in
+ * etx_tracer_b200/csrc/portable_math.h, the one definition the device and the oracle call).  It does not draw from the path's sampler,
+ * so every iteration stays a function of the scene, the options and its index. */
+int etxb_set_film_pixel_size(etxb_ctx* ctx, uint32_t size);
+
 /* ---- film export (SURVEY 8(f) N4): RTApplication::on_save_image_selected (sources/raytracer/app.cxx:261-295) -------------------------
  * The reference saves the selected Film layer either as float OpenEXR (tinyexr SaveEXR) or tone-mapped to 8-bit PNG (1 - exp(-exposure c),
  * sRGB curve, stb_image_write).  etxb_read_film_ldr tone-maps on the device (4 bytes per pixel leave the GPU); the two writers and the host
@@ -429,7 +444,8 @@ const void* etxb_scene_file_table(const etxb_scene_file* sf, const char* name, u
  * etxb_set_integrator selects which algorithm etxb_begin / etxb_enqueue_iteration / etxb_poll / etxb_read_film drive: with
  * ETXB_INTEGRATOR_PT one iteration = one path per active pixel (CPUPathTracingImpl::execute_range) followed by update()'s
  * film.estimate_noise_levels(current_iteration, samples, noise_threshold); a pixel the estimate marks converged is skipped from
- * then on (Film::active_pixel).  Progressive preview (pixel_size > 1, film.cxx:440-449) is not part of it: its pixel choice is rand(). */
+ * then on (Film::active_pixel).  The coarse preview (etxb_set_film_pixel_size) applies to it as to the VCM: a path whose chosen pixel has
+ * converged is skipped with its whole block. */
 #define ETXB_INTEGRATOR_VCM 0u
 #define ETXB_INTEGRATOR_PT 1u
 /* PTOptions (path_tracing_shared.hxx:8-14); the reference's option ids are "nee", "direct", "mis", "bn" (path_tracing.cxx:36-39) */
@@ -639,6 +655,8 @@ uint32_t etxb_group_lanes(const etxb_group* group);
 etxb_ctx* etxb_group_lane(etxb_group* group, uint32_t lane);
 const char* etxb_group_last_error(const etxb_group* group);
 int etxb_group_begin(etxb_group* group, uint32_t first_iteration);   /* Integrator::run: clears every lane's film */
+/* etxb_set_film_pixel_size for every lane (waits for the group to go idle); ETXB_ERR_UNSUPPORTED above 1 on a group with communicators */
+int etxb_group_set_film_pixel_size(etxb_group* group, uint32_t size);
 /* etxb_update_scene for every lane: waits for the group to go idle, validates and hashes once (and builds a new geometry's BVH once),
  * updates each lane, then etxb_group_begin(group, 0).  `info` is lane 0's, with `kept` the bits every lane kept.  ETXB_ERR_UNSUPPORTED on
  * a group with communicators (etxb_group_comm_init, etxb_group_comm_init_replicas). */
