@@ -127,6 +127,7 @@ def load_library(flavor="fast"):
     lib.etxb_stream.argtypes = [vp]
     lib.etxb_debug_trace.argtypes = [vp, vp, vp, u32, vp, vp]
     lib.etxb_debug_select_tree.argtypes = [vp, C.c_int]
+    lib.etxb_debug_build_trees.argtypes = [vp, vp, u32, vp, u32, u32, vp]
     lib.etxb_debug_occluded.argtypes = [vp, vp, u32, vp]
     lib.etxb_debug_sampler.argtypes = [vp, vp, vp, u32, u32, vp, vp]
     lib.etxb_debug_math.argtypes = [vp, u32, vp, vp, u32, vp]
@@ -497,6 +498,29 @@ class GPUVCM:
         """etxb_debug_trace / etxb_debug_occluded walk the BVH2 (False) or the product build's 4-wide quantised tree (True); returns whether that
         tree exists."""
         return self.lib.etxb_debug_select_tree(self.h, 1 if wide else 0) == 1
+
+    def debug_build_trees(self, positions, indices, device):
+        """Both trees of a triangle soup (positions float[V, 3], indices uint32[T, 3]) without committing a scene: built by the host builder
+        (device=False, the specification) or on the device (device=True, what an upload runs).  Returns a dict: bvh_nodes (S.BVH_NODE),
+        tri_pos (float32[3 * slots, 4]), tri_index (uint32[slots]), wide_nodes (S.WIDE_NODE), max_depth, max_stack, seconds."""
+        positions = np.ascontiguousarray(positions, dtype=np.float32).reshape(-1, 3)
+        indices = np.ascontiguousarray(indices, dtype=np.uint32).reshape(-1, 3)
+        cap = max(1, indices.shape[0])
+        nodes = np.zeros(cap, dtype=S.BVH_NODE)
+        tri_pos = np.zeros((cap * 3, 4), dtype=np.float32)
+        tri_index = np.zeros(cap, dtype=np.uint32)
+        wide = np.zeros(cap, dtype=S.WIDE_NODE)
+
+        class Trees(C.Structure):
+            _fields_ = [("bvh_nodes", C.c_void_p), ("tri_pos", C.c_void_p), ("tri_index", C.c_void_p), ("wide_nodes", C.c_void_p),
+                        ("bvh_node_count", C.c_uint32), ("slot_count", C.c_uint32), ("wide_node_count", C.c_uint32), ("max_depth", C.c_uint32),
+                        ("max_stack", C.c_uint32), ("pad", C.c_uint32), ("seconds", C.c_double)]
+
+        t = Trees(_p(nodes), _p(tri_pos), _p(tri_index), _p(wide))
+        self._check(self.lib.etxb_debug_build_trees(self.h, _p(positions), positions.shape[0], _p(indices), indices.shape[0], 1 if device else 0,
+                                                    C.byref(t)))
+        return {"bvh_nodes": nodes[:t.bvh_node_count], "tri_pos": tri_pos[:t.slot_count * 3], "tri_index": tri_index[:t.slot_count],
+                "wide_nodes": wide[:t.wide_node_count], "max_depth": int(t.max_depth), "max_stack": int(t.max_stack), "seconds": float(t.seconds)}
 
     def debug_trace(self, rays, seeds):
         rays = np.ascontiguousarray(rays, dtype=np.float32)

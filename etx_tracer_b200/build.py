@@ -10,8 +10,8 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["module.cu", "bvh_build.cpp", "film_io.cpp", "scene_loader.cpp"]
-HEADERS = ["bvh.h", "bvh_build.h", "dcore.cuh", "dscene.cuh", "dimage.cuh", "dbsdf.cuh", "dclosure.cuh", "dtrace.cuh", "dtrav.cuh", "dwide.cuh", "dmedium.cuh", "dsss.cuh", "dvcm.cuh", "dpt.cuh", "kernels.cuh", "kernels_pt.cuh", "portable_math.h", "scene_loader_formats.inl", "scene_loader_build.inl", "scene_loader_atmosphere.inl", "scene_loader_tangents.inl", "scene_loader_nvdb.inl", "scene_loader_jpeg.inl",
+SOURCES = ["module.cu", "bvh_build.cpp", "bvh_build_device.cu", "film_io.cpp", "scene_loader.cpp"]
+HEADERS = ["bvh.h", "bvh_build.h", "bvh_build_device.h", "dcore.cuh", "dscene.cuh", "dimage.cuh", "dbsdf.cuh", "dclosure.cuh", "dtrace.cuh", "dtrav.cuh", "dwide.cuh", "dmedium.cuh", "dsss.cuh", "dvcm.cuh", "dpt.cuh", "kernels.cuh", "kernels_pt.cuh", "portable_math.h", "scene_loader_formats.inl", "scene_loader_build.inl", "scene_loader_atmosphere.inl", "scene_loader_tangents.inl", "scene_loader_nvdb.inl", "scene_loader_jpeg.inl",
            os.path.join("..", "..", "include", "etx_b200.h")]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared", "--expt-relaxed-constexpr", "-Wno-deprecated-gpu-targets"]
@@ -34,9 +34,13 @@ def lib_path(flavor="fast"):
 UNIT_DEPS = {
     "module.cu": [h for h in HEADERS if not h.endswith(".inl")],
     "bvh_build.cpp": ["bvh.h", "bvh_build.h"],
+    "bvh_build_device.cu": ["bvh.h", "bvh_build_device.h"],
     "film_io.cpp": [os.path.join("..", "..", "include", "etx_b200.h")],
     "scene_loader.cpp": ["scene_loader_formats.inl", "scene_loader_build.inl", "scene_loader_atmosphere.inl", "scene_loader_tangents.inl", "scene_loader_nvdb.inl", "scene_loader_jpeg.inl", os.path.join("..", "..", "include", "etx_b200.h")],
 }
+# Translation units compiled with their own floating-point flags in every flavour.  The device BVH builder must reproduce the host builder's
+# floats bit for bit (IEEE division, no contraction, denormals kept: under -ftz=true even a comparison flushes a denormal operand).
+UNIT_FLAGS = {"bvh_build_device.cu": ["-fmad=false", "-ftz=false", "-prec-div=true", "-prec-sqrt=true"]}
 OBJ_ROOT = os.path.join(HERE, "build")  # git-ignored scratch: objects, one folder per flavour
 
 
@@ -69,7 +73,7 @@ def build(flavors=("fast", "parity", "count"), force=False, verbose=False, extra
             objs.append(obj)
             deps = [os.path.join(CSRC, src)] + [os.path.join(CSRC, d) for d in UNIT_DEPS[src]] + [os.path.abspath(__file__)]
             if force or extra or _newer(deps, obj):
-                cmd = ["nvcc"] + ARCH + compile_flags + flags + list(extra) + ["-c", os.path.join(CSRC, src), "-o", obj]
+                cmd = ["nvcc"] + ARCH + compile_flags + UNIT_FLAGS.get(src, flags) + list(extra) + ["-c", os.path.join(CSRC, src), "-o", obj]
                 if verbose:
                     cmd.insert(1, "-Xptxas=-v")
                     print(" ".join(cmd), flush=True)

@@ -24,6 +24,7 @@
 #include <nccl.h>
 
 #include "bvh_build.h"
+#include "bvh_build_device.h"
 #include "kernels.cuh"
 #include "kernels_pt.cuh"
 
@@ -64,11 +65,13 @@ enum KernelId : uint32_t {
   K_PT_SHADE,
   K_PT_ACCUMULATE,
   K_FILM_NOISE,
+  K_BVH_BUILD,
+  K_BVH_WIDE,
   K_COUNT
 };
 const char* kKernelNames[K_COUNT] = {"light_begin", "trace_closest(light)", "light_bounce", "lv_scan", "lv_reorder", "grid_bbox", "grid_keys", "grid_sort", "grid_build",
   "camera_begin", "trace_closest(camera)", "camera_shade", "camera_connect", "shadow_trace", "queue_sort", "camera_merge_sort", "camera_merge", "camera_merge_generic", "camera_continue", "film_commit_light", "nccl_allreduce_light_image", "nccl_allgather_photons",
-  "pt_begin", "pt_shade", "pt_accumulate", "film_noise_levels"};
+  "pt_begin", "pt_shade", "pt_accumulate", "film_noise_levels", "bvh_build", "bvh_collapse_wide"};
 
 // Queue sizes from which a pass takes its large-queue branches (the context's `thresholds`; etxb_debug_set_thresholds overrides them):
 //   merge_sort_min_queries  the gather queue is sorted by its merge keys (below it, a latency-bound tail, the sort launches cost more than they save)
@@ -1110,7 +1113,7 @@ int run_pt_iteration(etxb_ctx* ctx) {
 
 // ---- scene upload / update ------------------------------------------------------------------------------------------------------------------
 // etxb_upload_scene and etxb_update_scene run the same stages: validate_scene makes every check and touches nothing on the device,
-// prepare_scene hashes the bulk arrays (prepare_bvh builds the host BVH when the geometry is new), commit_scene copies to the device.  An
+// prepare_scene hashes the bulk arrays (prepare_bvh uploads a new geometry and builds its BVH2 on the device), commit_scene commits to the device.  An
 // update keeps the device copies whose content hashes did not change; everything small is derived from the PODs again on every call.
 struct SceneClass {
   bool stochastic = false;  // has_stochastic_merge
@@ -1122,9 +1125,15 @@ struct ScenePrep {
   SceneHashes hashes;
   double fingerprint_seconds = 0.0, bvh_seconds = 0.0;
   uint64_t bytes_hashed = 0;
-  Bvh bvh;                  // built by prepare_bvh (have_bvh), or only its nodes downloaded for a new 4-wide tree
+  // a new geometry's device copies and BVH2 (prepare_bvh: built once, copied into each context that commits it)
+  DevBuf<DVertex> vertices;
+  DevBuf<DTriangle> triangles;
+  DevBuf<BvhNode> bvh_nodes;
+  DevBuf<float4> bvh_tris;
+  uint32_t max_depth = 0;
   bool have_bvh = false;
-  WideBvh wide;
+  DevBuf<WideNode> wide;  // the 4-wide tree collapsed from the first committing context's BVH2
+  uint32_t max_stack = 0;
   bool have_wide = false;
 };
 
@@ -1301,17 +1310,51 @@ int prepare_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, Sc
   return ETXB_OK;
 }
 
-// the host BVH of a new geometry, and the check of its depth against the traversal stack
+// takes ownership of a cudaMalloc'd array of n elements
+template <class T>
+void adopt(DevBuf<T>& buf, T* ptr, size_t n) {
+  buf.release();
+  buf.ptr = ptr;
+  buf.count = n;
+}
+
+// a device-to-device copy into `dst`, sized as `src`
+template <class T>
+int copy_device(etxb_ctx* ctx, DevBuf<T>& dst, const DevBuf<T>& src) {
+  CUDA_OK(ctx, dst.alloc(src.count));
+  if (src.count) CUDA_OK(ctx, cudaMemcpyAsync(dst.ptr, src.ptr, src.bytes(), cudaMemcpyDeviceToDevice, ctx->stream));
+  return ETXB_OK;
+}
+
+// A new geometry's vertices and triangles on the device, its BVH2 built there (bvh_build_device.cu: the tree of build_bvh), and the check of
+// its depth against the traversal stack.  Everything goes into the prep's own buffers: a refusal or a CUDA error leaves the committed scene as it was.
 int prepare_bvh(etxb_ctx* ctx, const etxb_scene& s, ScenePrep& p) {
   if (p.have_bvh) return ETXB_OK;
   auto t0 = std::chrono::steady_clock::now();
-  auto c0 = std::clock();
-  build_bvh(reinterpret_cast<const float*>(s.vertices.a), sizeof(etxb_vertex), reinterpret_cast<const uint32_t*>(s.triangles.a), sizeof(etxb_triangle),
-    uint32_t(s.triangles.count), p.bvh);
-  ctx->bvh_build_seconds = double(std::clock() - c0) / CLOCKS_PER_SEC;
+  const auto* verts = static_cast<const etxb_vertex*>(s.vertices.a);
+  std::vector<DVertex> dverts(s.vertices.count);
+  for (uint64_t i = 0; i < s.vertices.count; ++i) {
+    const etxb_vertex& v = verts[i];
+    dverts[i].pos_u = make_float4(v.pos[0], v.pos[1], v.pos[2], v.tex[0]);
+    dverts[i].nrm_v = make_float4(v.nrm[0], v.nrm[1], v.nrm[2], v.tex[1]);
+    dverts[i].tan = make_float4(v.tan[0], v.tan[1], v.tan[2], 0.0f);
+    dverts[i].btn = make_float4(v.btn[0], v.btn[1], v.btn[2], 0.0f);
+  }
+  if (int rc = upload(ctx, p.vertices, dverts.data(), dverts.size())) return rc;
+  if (int rc = upload(ctx, p.triangles, reinterpret_cast<const DTriangle*>(s.triangles.a), size_t(s.triangles.count))) return rc;
+  const auto b0 = std::chrono::steady_clock::now();
+  DeviceBvhOut out;
+  CUDA_OK(ctx, build_bvh_device(reinterpret_cast<const float*>(p.vertices.ptr), sizeof(DVertex), reinterpret_cast<const uint32_t*>(p.triangles.ptr), sizeof(DTriangle),
+    uint32_t(s.triangles.count), false, ctx->stream, out));
+  adopt(p.bvh_nodes, out.nodes, out.node_count);
+  adopt(p.bvh_tris, reinterpret_cast<float4*>(out.tri_pos), size_t(out.slot_count) * 3u);
+  p.max_depth = out.max_depth;
+  ctx->bvh_build_seconds = seconds_since(b0);
+  ctx->kernel_ms[K_BVH_BUILD] += float(ctx->bvh_build_seconds * 1.0e3);
+  ctx->kernel_count[K_BVH_BUILD] += 1;
   p.bvh_seconds += seconds_since(t0);
   p.have_bvh = true;
-  if (p.bvh.max_depth >= uint32_t(kBvhStackSize)) return fail(ctx, ETXB_ERR_UNSUPPORTED, "BVH depth %u exceeds the traversal stack (%d)", p.bvh.max_depth, kBvhStackSize);
+  if (p.max_depth >= uint32_t(kBvhStackSize)) return fail(ctx, ETXB_ERR_UNSUPPORTED, "BVH depth %u exceeds the traversal stack (%d)", p.max_depth, kBvhStackSize);
   return ETXB_OK;
 }
 
@@ -1440,17 +1483,8 @@ int commit_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, Sce
   // ---- geometry ------------------------------------------------------------------------------------------------------
   static_assert(sizeof(DTriangle) == sizeof(etxb_triangle), "triangle layout");
   if (!keep_geometry) {
-    const auto* verts = static_cast<const etxb_vertex*>(s.vertices.a);
-    std::vector<DVertex> dverts(s.vertices.count);
-    for (uint64_t i = 0; i < s.vertices.count; ++i) {
-      const etxb_vertex& v = verts[i];
-      dverts[i].pos_u = make_float4(v.pos[0], v.pos[1], v.pos[2], v.tex[0]);
-      dverts[i].nrm_v = make_float4(v.nrm[0], v.nrm[1], v.nrm[2], v.tex[1]);
-      dverts[i].tan = make_float4(v.tan[0], v.tan[1], v.tan[2], 0.0f);
-      dverts[i].btn = make_float4(v.btn[0], v.btn[1], v.btn[2], 0.0f);
-    }
-    if (int rc = upload(ctx, ctx->vertices, dverts.data(), dverts.size())) return rc;
-    if (int rc = upload(ctx, ctx->triangles, reinterpret_cast<const DTriangle*>(s.triangles.a), size_t(s.triangles.count))) return rc;
+    if (int rc = copy_device(ctx, ctx->vertices, p.vertices)) return rc;
+    if (int rc = copy_device(ctx, ctx->triangles, p.triangles)) return rc;
   }
   if (int rc = upload(ctx, ctx->tri_emitter, static_cast<const uint32_t*>(s.triangle_to_emitter.a), size_t(s.triangle_to_emitter.count))) return rc;
   if (int rc = upload(ctx, ctx->materials, mats, size_t(s.materials.count))) return rc;
@@ -1460,9 +1494,9 @@ int commit_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, Sce
   if (int rc = upload(ctx, ctx->emitter_dist, static_cast<const etxb_distribution_entry*>(s.emitters_distribution.values.a), size_t(s.emitter_instances.count) + 1u))
     return rc;
   if (!keep_geometry) {
-    if (int rc = upload(ctx, ctx->bvh_nodes, p.bvh.nodes.data(), p.bvh.nodes.size())) return rc;
-    if (int rc = upload(ctx, ctx->bvh_tris, reinterpret_cast<const float4*>(p.bvh.tri_pos.data()), p.bvh.tri_pos.size())) return rc;
-    d.bvh_node_count = uint32_t(p.bvh.nodes.size());
+    if (int rc = copy_device(ctx, ctx->bvh_nodes, p.bvh_nodes)) return rc;
+    if (int rc = copy_device(ctx, ctx->bvh_tris, p.bvh_tris)) return rc;
+    d.bvh_node_count = uint32_t(p.bvh_nodes.count);
   }
   d.vertices = ctx->vertices.ptr;
   d.triangles = ctx->triangles.ptr;
@@ -1491,20 +1525,22 @@ int commit_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, Sce
     // the sampler streams of such a scene's stochastic stages are the product build's own already: its traversal kernels may meet candidates in
     // another order, so they walk the 4-wide quantised form of the tree (dwide.cuh); Lambert / delta scenes keep the oracle's candidate order
     if (!p.have_wide) {
+      // collapsed on the device from the committed BVH2 (new or kept: bvh_build_device.cu, the tree of build_wide_bvh)
       auto t0 = std::chrono::steady_clock::now();
-      if (!p.have_bvh) {
-        // kept geometry that now needs the 4-wide tree: it is collapsed from the device's BVH2 nodes (the builder reads nothing else)
-        p.bvh.nodes.resize(ctx->bvh_nodes.count);
-        CUDA_OK(ctx, cudaMemcpy(p.bvh.nodes.data(), ctx->bvh_nodes.ptr, ctx->bvh_nodes.bytes(), cudaMemcpyDeviceToHost));
-      }
-      build_wide_bvh(p.bvh, p.wide);
+      WideNode* wide = nullptr;
+      uint32_t count = 0;
+      CUDA_OK(ctx, build_wide_bvh_device(ctx->bvh_nodes.ptr, d.bvh_node_count, ctx->stream, &wide, &count, &p.max_stack));
+      adopt(p.wide, wide, count);
       p.have_wide = true;
-      p.bvh_seconds += seconds_since(t0);
+      const double seconds = seconds_since(t0);
+      ctx->kernel_ms[K_BVH_WIDE] += float(seconds * 1.0e3);
+      ctx->kernel_count[K_BVH_WIDE] += 1;
+      p.bvh_seconds += seconds;
     }
-    if (p.wide.max_stack < uint32_t(kWideStackSize)) {
-      if (int rc = upload(ctx, ctx->wide_nodes, p.wide.nodes.data(), p.wide.nodes.size())) return rc;
+    if (p.max_stack < uint32_t(kWideStackSize)) {
+      if (int rc = copy_device(ctx, ctx->wide_nodes, p.wide)) return rc;
       d.wide_nodes = ctx->wide_nodes.ptr;
-      d.wide_node_count = uint32_t(p.wide.nodes.size());
+      d.wide_node_count = uint32_t(p.wide.count);
     } else {
       ctx->wide_rejected = true;
     }
@@ -2424,6 +2460,18 @@ int etxb_device_pointer(etxb_ctx* ctx, uint32_t buffer_id, void** out_ptr, uint6
     case ETXB_BUF_PIXEL_ERROR:
       if (ctx->pt_error.count != n) return fail(ctx, ETXB_ERR_NOT_READY, "the path tracer has not run on this film");
       *out_ptr = ctx->pt_error.ptr; *out_bytes = n * 4; break;
+    case ETXB_BUF_BVH_NODES:
+    case ETXB_BUF_BVH_TRIS:
+    case ETXB_BUF_WIDE_NODES:
+      if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
+      if (buffer_id == ETXB_BUF_BVH_NODES) {
+        *out_ptr = ctx->bvh_nodes.ptr; *out_bytes = size_t(ctx->dscene.bvh_node_count) * sizeof(BvhNode);
+      } else if (buffer_id == ETXB_BUF_BVH_TRIS) {
+        *out_ptr = ctx->bvh_tris.ptr; *out_bytes = ctx->bvh_tris.bytes();
+      } else {
+        *out_ptr = const_cast<WideNode*>(ctx->dscene.wide_nodes); *out_bytes = size_t(ctx->dscene.wide_node_count) * sizeof(WideNode);
+      }
+      break;
     default: return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "buffer %u has no direct device pointer", buffer_id);
   }
   return ETXB_OK;
@@ -2513,6 +2561,65 @@ int etxb_debug_occluded(etxb_ctx* ctx, const float* segments, uint32_t count, ui
   ctx->kernel_launches += 1;
   CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
   CUDA_OK(ctx, cudaMemcpy(occluded, d_occluded.ptr, d_occluded.bytes(), cudaMemcpyDeviceToHost));
+  return ETXB_OK;
+}
+
+// Test hook: both trees of a triangle soup from the host builder (the specification) or from the device builder, nothing committed
+int etxb_debug_build_trees(etxb_ctx* ctx, const float* positions, uint32_t vertex_count, const uint32_t* indices, uint32_t triangle_count, uint32_t device,
+  etxb_debug_trees* out) {
+  if (!ctx || !out || !out->bvh_nodes || !out->tri_pos || !out->tri_index || !out->wide_nodes || (device > 1u)) return ETXB_ERR_INVALID_ARGUMENT;
+  if ((triangle_count && !indices) || (vertex_count && !positions)) return ETXB_ERR_INVALID_ARGUMENT;
+  for (uint64_t i = 0; i < uint64_t(triangle_count) * 3u; ++i)
+    if (indices[i] >= vertex_count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "triangle %llu: vertex index out of range", (unsigned long long)(i / 3u));
+  const size_t cap = std::max<uint32_t>(triangle_count, 1u);
+  auto t0 = std::chrono::steady_clock::now();
+  if (device == 0u) {
+    Bvh bvh;
+    build_bvh(positions, 12u, indices, 12u, triangle_count, bvh);
+    WideBvh wide;
+    build_wide_bvh(bvh, wide);
+    out->seconds = seconds_since(t0);
+    memcpy(out->bvh_nodes, bvh.nodes.data(), bvh.nodes.size() * sizeof(BvhNode));
+    memcpy(out->tri_pos, bvh.tri_pos.data(), bvh.tri_pos.size() * sizeof(F4));
+    memcpy(out->tri_index, bvh.tri_index.data(), bvh.tri_index.size() * 4u);
+    memcpy(out->wide_nodes, wide.nodes.data(), wide.nodes.size() * sizeof(WideNode));
+    out->bvh_node_count = uint32_t(bvh.nodes.size());
+    out->slot_count = uint32_t(bvh.tri_index.size());
+    out->wide_node_count = uint32_t(wide.nodes.size());
+    out->max_depth = bvh.max_depth;
+    out->max_stack = wide.max_stack;
+    return ETXB_OK;
+  }
+  cudaSetDevice(ctx->device);
+  DevBuf<float> d_pos;
+  DevBuf<uint32_t> d_idx;
+  if (int rc = upload(ctx, d_pos, positions, size_t(vertex_count) * 3u)) return rc;
+  if (int rc = upload(ctx, d_idx, indices, size_t(triangle_count) * 3u)) return rc;
+  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+  t0 = std::chrono::steady_clock::now();
+  DeviceBvhOut bvh;
+  CUDA_OK(ctx, build_bvh_device(d_pos.ptr, 12u, d_idx.ptr, 12u, triangle_count, true, ctx->stream, bvh));
+  DevBuf<BvhNode> nodes;
+  DevBuf<F4> tri_pos;
+  DevBuf<uint32_t> tri_index;
+  adopt(nodes, bvh.nodes, cap);
+  adopt(tri_pos, bvh.tri_pos, cap * 3u);
+  adopt(tri_index, bvh.tri_index, cap);
+  DevBuf<WideNode> wide;
+  WideNode* w = nullptr;
+  uint32_t wide_count = 0, max_stack = 0;
+  CUDA_OK(ctx, build_wide_bvh_device(bvh.nodes, bvh.node_count, ctx->stream, &w, &wide_count, &max_stack));
+  adopt(wide, w, wide_count);
+  out->seconds = seconds_since(t0);
+  CUDA_OK(ctx, cudaMemcpy(out->bvh_nodes, bvh.nodes, size_t(bvh.node_count) * sizeof(BvhNode), cudaMemcpyDeviceToHost));
+  CUDA_OK(ctx, cudaMemcpy(out->tri_pos, bvh.tri_pos, size_t(bvh.slot_count) * 3u * sizeof(F4), cudaMemcpyDeviceToHost));
+  CUDA_OK(ctx, cudaMemcpy(out->tri_index, bvh.tri_index, size_t(bvh.slot_count) * 4u, cudaMemcpyDeviceToHost));
+  CUDA_OK(ctx, cudaMemcpy(out->wide_nodes, w, size_t(wide_count) * sizeof(WideNode), cudaMemcpyDeviceToHost));
+  out->bvh_node_count = bvh.node_count;
+  out->slot_count = bvh.slot_count;
+  out->wide_node_count = wide_count;
+  out->max_depth = bvh.max_depth;
+  out->max_stack = max_stack;
   return ETXB_OK;
 }
 

@@ -175,7 +175,11 @@ VCM_FULL = VCM_CONNECT_ONLY | VCM_ENABLE_MERGING | VCM_MERGE_VERTICES
 FILM_RESULT, FILM_CAMERA, FILM_LIGHT, FILM_LIGHT_ITERATION, FILM_NORMALS, FILM_ALBEDO, FILM_CAMERA_ADAPTIVE = range(7)
 (BUF_LIGHT_PATH_COUNT, BUF_LIGHT_PATH_OFFSET, BUF_LIGHT_PATH_WAVELENGTH, BUF_LIGHT_SAMPLER, BUF_CAMERA_SAMPLER, BUF_LV_POS,
  BUF_LV_THROUGHPUT, BUF_LV_MIS, BUF_FILM_LIGHT_ITERATION, BUF_FILM_CAMERA, BUF_FILM_LIGHT, BUF_PHOTON_RECORDS,
- BUF_CAMERA_GATHERED, BUF_PIXEL_INFO, BUF_PIXEL_ERROR) = range(15)
+ BUF_CAMERA_GATHERED, BUF_PIXEL_INFO, BUF_PIXEL_ERROR, BUF_BVH_NODES, BUF_BVH_TRIS, BUF_WIDE_NODES) = range(18)
+# the trees' 64-byte nodes (csrc/bvh.h BvhNode, WideNode)
+BVH_NODE = np.dtype([("lo0", "<f4", 3), ("hi0", "<f4", 3), ("lo1", "<f4", 3), ("hi1", "<f4", 3), ("child0", "<i4"), ("child1", "<i4"), ("pad", "<u4", 2)])
+WIDE_NODE = np.dtype([("origin", "<f4", 3), ("exp", "u1", 3), ("count", "u1"), ("qlo", "u1", (4, 3)), ("qhi", "u1", (4, 3)), ("child", "<i4", 4),
+                      ("pad", "<u4", 2)])
 INTEGRATOR_VCM, INTEGRATOR_PT = 0, 1
 PIXEL_COUNT_MASK, PIXEL_CONVERGED, PIXEL_TMP = (1 << 30) - 1, 1 << 30, 1 << 31
 PT_OPTIONS = np.dtype([("nee", np.uint32), ("direct", np.uint32), ("mis", np.uint32), ("blue_noise", np.uint32)])

@@ -288,6 +288,9 @@ enum {
   ETXB_BUF_CAMERA_GATHERED = 12,   /* float[3*N] last iteration's camera contribution per path */
   ETXB_BUF_PIXEL_INFO = 13,        /* uint32[N]  Film's InternalData in film storage order (film.cxx:27-32): sample_count bits 0-29, converged bit 30, tmp bit 31 */
   ETXB_BUF_PIXEL_ERROR = 14,       /* float[N]   InternalData::error_level */
+  ETXB_BUF_BVH_NODES = 15,         /* the committed BVH2: 64-byte nodes (csrc/bvh.h BvhNode), root first */
+  ETXB_BUF_BVH_TRIS = 16,          /* float4[3*S] leaf-ordered triangle corners; .w of the first corner holds the triangle index */
+  ETXB_BUF_WIDE_NODES = 17,        /* the committed 4-wide tree: 64-byte nodes (csrc/bvh.h WideNode); empty where the scene walks the BVH2 */
   ETXB_BUF_COUNT
 };
 
@@ -324,8 +327,8 @@ int etxb_upload_scene(etxb_ctx* ctx, const void* scene, uint64_t scene_bytes, co
  * Every check of the upload runs before any device buffer changes: a refused update returns the error and the previous scene stays
  * committed and renderable.  A CUDA failure part-way leaves the scene not ready, like a failed upload.  Iterations in flight are drained
  * first.  Without a committed scene it is an upload.  ETXB_ERR_UNSUPPORTED on a context with a communicator (etxb_comm_init).
- * `info` (may be NULL) reports what was kept, the bytes hashed and the host time spent hashing, building trees (BVH2 and 4-wide) and in
- * the whole call. */
+ * `info` (may be NULL) reports what was kept, the bytes hashed, the host time spent hashing, the time spent building trees (BVH2 and
+ * 4-wide, both on the device: wall time including the new geometry's upload) and in the whole call. */
 typedef struct etxb_update_info {
   uint32_t kept; /* ETXB_KEPT_* bits */
   uint32_t images_kept, images_uploaded;
@@ -505,6 +508,20 @@ int etxb_debug_occluded(etxb_ctx* ctx, const float* segments, uint32_t count, ui
 /* Which tree etxb_debug_trace and etxb_debug_occluded walk: 0 = the BVH2 shared with the oracle, 1 = the product build's 4-wide quantised tree
  * (returns 1 if it exists). */
 int etxb_debug_select_tree(etxb_ctx* ctx, int wide);
+/* Both trees of a triangle soup, built without committing a scene: with the host builder (device = 0: csrc/bvh_build.cpp, the specification)
+ * or on the device (device = 1: what etxb_upload_scene runs).  positions = float[3*vertex_count], indices = uint32[3*triangle_count] (each
+ * index below vertex_count).  The caller sizes every array for max(1, triangle_count) entries (nodes of 64 bytes, tri_pos of 3 float4, tri_index
+ * of one uint32, wide nodes of 64 bytes); the counts, max_depth and max_stack come back, and `seconds` is the wall time of the two builds. */
+typedef struct etxb_debug_trees {
+  void* bvh_nodes;
+  float* tri_pos;
+  uint32_t* tri_index;
+  void* wide_nodes;
+  uint32_t bvh_node_count, slot_count, wide_node_count, max_depth, max_stack, pad;
+  double seconds;
+} etxb_debug_trees;
+int etxb_debug_build_trees(etxb_ctx* ctx, const float* positions, uint32_t vertex_count, const uint32_t* indices, uint32_t triangle_count, uint32_t device,
+                           etxb_debug_trees* out);
 /* Sampler / spectral KATs evaluated on the device (sampler.hxx:54,66; spectrum.hxx:219,234). */
 int etxb_debug_sampler(etxb_ctx* ctx, const uint32_t* a, const uint32_t* b, uint32_t count, uint32_t draws, uint32_t* out_seed, float* out_values);
 int etxb_debug_math(etxb_ctx* ctx, uint32_t fn, const float* x, const float* y, uint32_t count, float* out);
