@@ -115,6 +115,8 @@ def load_library(flavor="fast"):
     lib.etxb_read_film.argtypes = [vp, u32, vp, u64]
     lib.etxb_film_size.argtypes = [vp, C.POINTER(u32), C.POINTER(u32)]
     lib.etxb_read_film_ldr.argtypes = [vp, u32, C.c_float, vp, u64]
+    lib.etxb_denoise.argtypes = [vp, u32]
+    lib.etxb_debug_denoise.argtypes = [vp, vp, vp, vp, vp, vp, vp, u32, u32, vp, vp]
     lib.etxb_save_film.argtypes = [vp, u32, C.c_char_p, u32, C.c_float]
     lib.etxb_write_exr.argtypes = [C.c_char_p, vp, u32, u32]
     lib.etxb_write_png.argtypes = [C.c_char_p, vp, u32, u32]
@@ -464,13 +466,18 @@ class GPUVCM:
         """RTApplication::on_save_image_selected (app.cxx:261-295): the float layer as OpenEXR, or tone-mapped as PNG."""
         self._check(self.lib.etxb_save_film(self.h, layer, os.fsencode(file_name), 1 if tonemapped else 0, C.c_float(exposure)))
 
+    def denoise(self, layer=S.FILM_RESULT):
+        """Film::denoise(layer): filters the Result or Camera layer into S.FILM_DENOISED on the device (DESIGN §13: non-local means with a
+        two-half-buffer variance estimate, guided by the normal and albedo layers under the path tracer).  Needs two iterations on the film."""
+        self._check(self.lib.etxb_denoise(self.h, layer))
+
     def counters(self):
         c = np.zeros(1, dtype=S.COUNTERS)
         self._check(self.lib.etxb_get_counters(self.h, _p(c)))
         return _fields(c)
 
     def kernel_times(self):
-        cap = 32
+        cap = self._check(self.lib.etxb_get_kernel_times(self.h, None, None, None, 0))  # the module's number of timed kernels
         names = (C.c_char_p * cap)()
         ms = (C.c_float * cap)()
         launches = (C.c_uint32 * cap)()
@@ -538,6 +545,24 @@ class GPUVCM:
         out = np.zeros(n, dtype=np.uint32)
         self._check(self.lib.etxb_debug_occluded(self.h, _p(segments), n, _p(out)))
         return out != 0
+
+    def debug_denoise(self, color, camera, half, counts, normals=None, albedo=None):
+        """etxb_denoise's kernels on host arrays: color / camera / half (and the optional guides) float32 (H, W, 3 or 4), counts uint32 (H, W).
+        Returns (denoised float32 (H, W, 4), smoothed variance of the mean float32 (H, W, 4))."""
+        def rgba(a):
+            a = np.asarray(a, dtype=np.float32)
+            out = np.zeros(a.shape[:2] + (4,), dtype=np.float32)
+            out[..., :a.shape[2]] = a
+            return np.ascontiguousarray(out)
+        c, f, hh = rgba(color), rgba(camera), rgba(half)
+        h, w = c.shape[:2]
+        n = np.ascontiguousarray(counts, dtype=np.uint32).reshape(h, w)
+        g = [rgba(x) if x is not None else None for x in (normals, albedo)]
+        out = np.zeros((h, w, 4), dtype=np.float32)
+        var = np.zeros((h, w, 4), dtype=np.float32)
+        self._check(self.lib.etxb_debug_denoise(self.h, _p(c), _p(f), _p(hh), _p(n), _p(g[0]) if g[0] is not None else None,
+                                                _p(g[1]) if g[1] is not None else None, w, h, _p(out), _p(var)))
+        return out, var
 
     def debug_sampler(self, a, b, draws):
         a = np.ascontiguousarray(a, dtype=np.uint32)

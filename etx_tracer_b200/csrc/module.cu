@@ -27,6 +27,7 @@
 #include "bvh_build_device.h"
 #include "kernels.cuh"
 #include "kernels_pt.cuh"
+#include "kernels_denoise.cuh"
 
 using namespace etxb;
 
@@ -67,11 +68,16 @@ enum KernelId : uint32_t {
   K_FILM_NOISE,
   K_BVH_BUILD,
   K_BVH_WIDE,
+  K_FILM_ADAPTIVE,
+  K_DENOISE_VARIANCE,
+  K_DENOISE_SMOOTH,
+  K_DENOISE_NLM,
   K_COUNT
 };
 const char* kKernelNames[K_COUNT] = {"light_begin", "trace_closest(light)", "light_bounce", "lv_scan", "lv_reorder", "grid_bbox", "grid_keys", "grid_sort", "grid_build",
   "camera_begin", "trace_closest(camera)", "camera_shade", "camera_connect", "shadow_trace", "queue_sort", "camera_merge_sort", "camera_merge", "camera_merge_generic", "camera_continue", "film_commit_light", "nccl_allreduce_light_image", "nccl_allgather_photons",
-  "pt_begin", "pt_shade", "pt_accumulate", "film_noise_levels", "bvh_build", "bvh_collapse_wide"};
+  "pt_begin", "pt_shade", "pt_accumulate", "film_noise_levels", "bvh_build", "bvh_collapse_wide",
+  "film_adaptive_vcm", "denoise_variance", "denoise_smooth", "denoise_nlm"};
 
 // Queue sizes from which a pass takes its large-queue branches (the context's `thresholds`; etxb_debug_set_thresholds overrides them):
 //   merge_sort_min_queries  the gather queue is sorted by its merge keys (below it, a latency-bound tail, the sort launches cost more than they save)
@@ -232,7 +238,11 @@ struct etxb_ctx {
   // unidirectional path tracer (SURVEY 8(f) N3): the same context renders with CPUPathTracing's algorithm once etxb_set_integrator selects it
   uint32_t integrator = ETXB_INTEGRATOR_VCM;
   etxb_pt_options pt_options = {1u, 1u, 1u, 1u};
-  DevBuf<float4> film_normals, film_albedo, film_adaptive;  // Film's Normals / Albedo / CameraAdaptive layers (allocated with the first PT run)
+  DevBuf<float4> film_normals, film_albedo, film_adaptive;  // Film's Normals / Albedo / CameraAdaptive layers (allocated with the first PT run;
+                                                           // CameraAdaptive also with the first VCM camera pass)
+  DevBuf<float4> film_denoised;                             // Film's Denoised layer: the last etxb_denoise, zeros before it (StorageDenoised)
+  DevBuf<float4> denoise_u, denoise_var_raw, denoise_var;   // etxb_denoise scratch: colour with its flags, variance, smoothed variance
+  DevBuf<uint32_t> denoise_flag;                            // set by k_denoise_variance where a pixel has fewer than two samples
   DevBuf<uint32_t> film_ldr;                                 // the tone-mapped RGBA8 frame of etxb_read_film_ldr
   DevBuf<uint32_t> pt_info, pt_info_next, pt_stats;          // InternalData (sample count, converged, tmp); [converged this pass, error sum bits]
   DevBuf<float> pt_error;
@@ -857,6 +867,8 @@ int launch_merge(etxb_ctx* ctx, const LaunchParams& p, const uint32_t* q, const 
   return ETXB_OK;
 }
 
+int film_ensure_adaptive(etxb_ctx* ctx);
+
 template <bool SP, bool PLAIN>
 int run_camera_pass(etxb_ctx* ctx) {
   LaunchParams p = make_params(ctx);
@@ -930,6 +942,12 @@ int run_camera_pass(etxb_ctx* ctx) {
   if (ctx->pixel_size != 1u) {
     LaunchTimer t(ctx, K_CAMERA_CONTINUE);
     k_film_fill_blocks<false><<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(p, PtFilm{}, ctx->iteration);
+  }
+  if ((p.camera_sample_index % 2u) == 0u) {
+    // CameraAdaptive, the even-sample mean the denoiser's variance estimate reads (an odd sample leaves it as it is)
+    if (int rc = film_ensure_adaptive(ctx)) return rc;
+    LaunchTimer t(ctx, K_FILM_ADAPTIVE);
+    k_film_adaptive_vcm<<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(p, ctx->film_adaptive.ptr);
   }
   CUDA_OK(ctx, cudaGetLastError());
   return ETXB_OK;
@@ -1020,15 +1038,25 @@ int finish_iteration(etxb_ctx* ctx) {
 }
 
 // ---- unidirectional path tracer (SURVEY 8(f) N3) -----------------------------------------------------------------------------------------
+// CameraAdaptive (film.cxx:173-230): written by both integrators, allocated (as zeros) with the first pass that writes it at this film size
+int film_ensure_adaptive(etxb_ctx* ctx) {
+  const size_t n = ctx->path_count;
+  if (ctx->film_adaptive.count == n) return ETXB_OK;
+  CUDA_OK(ctx, ctx->film_adaptive.alloc(n));
+  CUDA_OK(ctx, cudaMemsetAsync(ctx->film_adaptive.ptr, 0, n * 16, ctx->stream));
+  return ETXB_OK;
+}
+
 // The film layers and the per-pixel history only CPUPathTracing touches (film.cxx:14-40, 104-121), allocated with the first run.
 int pt_ensure_film(etxb_ctx* ctx) {
   const size_t n = ctx->path_count;
   if (ctx->film_normals.count == n) return ETXB_OK;
-  DevBuf<float4>* f4[] = {&ctx->film_normals, &ctx->film_albedo, &ctx->film_adaptive};
+  DevBuf<float4>* f4[] = {&ctx->film_normals, &ctx->film_albedo};
   for (auto* b : f4) {
     CUDA_OK(ctx, b->alloc(n));
     CUDA_OK(ctx, cudaMemsetAsync(b->ptr, 0, n * 16, ctx->stream));
   }
+  if (int rc = film_ensure_adaptive(ctx)) return rc;
   CUDA_OK(ctx, ctx->pt_info.alloc(n));
   CUDA_OK(ctx, ctx->pt_info_next.alloc(n));
   CUDA_OK(ctx, ctx->pt_error.alloc(n));
@@ -1578,6 +1606,7 @@ int commit_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, Sce
     allocations += 1;
     return b.alloc(count);
   };
+  if ((ctx->width != cam.film_size[0]) || (ctx->height != cam.film_size[1])) ctx->film_denoised.release();  // Denoised starts over at a new film size
   ctx->width = cam.film_size[0];
   ctx->height = cam.film_size[1];
   ctx->path_count = ctx->width * ctx->height;
@@ -1747,16 +1776,26 @@ int film_layer_source(etxb_ctx* ctx, uint32_t layer, const float4** out_src) {
     case ETXB_FILM_LIGHT_ITERATION:
       src = ctx->film_light_iteration.ptr;
       break;
+    case ETXB_FILM_CAMERA_ADAPTIVE:
+      if (int rc = film_ensure_adaptive(ctx)) return rc;
+      src = ctx->film_adaptive.ptr;
+      break;
+    case ETXB_FILM_DENOISED:
+      if (ctx->film_denoised.count != ctx->path_count) {
+        CUDA_OK(ctx, ctx->film_denoised.alloc(ctx->path_count));
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->film_denoised.ptr, 0, ctx->film_denoised.bytes(), ctx->stream));
+      }
+      src = ctx->film_denoised.ptr;
+      break;
     case ETXB_FILM_NORMALS:
-    case ETXB_FILM_ALBEDO:
-    case ETXB_FILM_CAMERA_ADAPTIVE: {
+    case ETXB_FILM_ALBEDO: {
       if (int rc = pt_ensure_film(ctx)) return rc;
       if (layer == ETXB_FILM_NORMALS) {
         k_film_layer_normals<<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(ctx->film_normals.ptr, ctx->film_out.ptr, ctx->path_count);
         ctx->kernel_launches += 1;
         src = ctx->film_out.ptr;
       } else {
-        src = (layer == ETXB_FILM_ALBEDO) ? ctx->film_albedo.ptr : ctx->film_adaptive.ptr;
+        src = ctx->film_albedo.ptr;
       }
       break;
     }
@@ -1764,6 +1803,42 @@ int film_layer_source(etxb_ctx* ctx, uint32_t layer, const float4** out_src) {
       return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "unknown film layer %u", layer);
   }
   *out_src = src;
+  return ETXB_OK;
+}
+
+// Film::denoise (DESIGN §13): the three kernels of kernels_denoise.cuh on `in`, into `out` (and the smoothed variance into `out_variance`, when
+// given).  ETXB_ERR_NOT_READY, with `out` untouched, where a pixel has fewer than two samples.  Synchronous.
+int run_denoise(etxb_ctx* ctx, const DenoiseInputs& in, float4* out, float4* out_variance) {
+  const uint32_t n = in.width * in.height;
+  DevBuf<float4>* scratch[] = {&ctx->denoise_u, &ctx->denoise_var_raw, &ctx->denoise_var};
+  for (auto* b : scratch)
+    if (b->count != n) CUDA_OK(ctx, b->alloc(n));
+  if (!ctx->denoise_flag.ptr) CUDA_OK(ctx, ctx->denoise_flag.alloc(1));
+  CUDA_OK(ctx, cudaMemsetAsync(ctx->denoise_flag.ptr, 0, 4, ctx->stream));
+  {
+    LaunchTimer t(ctx, K_DENOISE_VARIANCE);
+    k_denoise_variance<<<blocks_for(n, 256), 256, 0, ctx->stream>>>(in, ctx->denoise_u.ptr, ctx->denoise_var_raw.ptr, ctx->denoise_flag.ptr);
+  }
+  uint32_t not_ready = 0;
+  CUDA_OK(ctx, cudaMemcpyAsync(&not_ready, ctx->denoise_flag.ptr, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+  if (not_ready) {
+    resolve_timers(ctx);
+    return fail(ctx, ETXB_ERR_NOT_READY, "denoise: a pixel has fewer than two samples (the variance estimate needs both half buffers)");
+  }
+  {
+    LaunchTimer t(ctx, K_DENOISE_SMOOTH);
+    k_denoise_smooth<<<blocks_for(n, 256), 256, 0, ctx->stream>>>(ctx->denoise_var_raw.ptr, ctx->denoise_var.ptr, in.width, in.height);
+  }
+  {
+    LaunchTimer t(ctx, K_DENOISE_NLM);
+    const dim3 tiles((in.width + kDenoiseTile - 1) / kDenoiseTile, (in.height + kDenoiseTile - 1) / kDenoiseTile);
+    k_denoise_nlm<<<tiles, kDenoiseTile * kDenoiseTile, 0, ctx->stream>>>(in, ctx->denoise_u.ptr, ctx->denoise_var.ptr, out);
+  }
+  if (out_variance) CUDA_OK(ctx, cudaMemcpyAsync(out_variance, ctx->denoise_var.ptr, size_t(n) * 16, cudaMemcpyDeviceToDevice, ctx->stream));
+  CUDA_OK(ctx, cudaGetLastError());
+  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+  resolve_timers(ctx);
   return ETXB_OK;
 }
 
@@ -2127,9 +2202,10 @@ int etxb_begin(etxb_ctx* ctx, uint32_t first_iteration) {
     // Film::clear(ClearCameraData) (film.cxx:345-368): the per-pixel history starts over
     CUDA_OK(ctx, cudaMemsetAsync(ctx->pt_info.ptr, 0, n * 4, ctx->stream));
     CUDA_OK(ctx, cudaMemsetAsync(ctx->pt_error.ptr, 0, n * 4, ctx->stream));
-    DevBuf<float4>* layers[] = {&ctx->film_normals, &ctx->film_albedo, &ctx->film_adaptive};
+    DevBuf<float4>* layers[] = {&ctx->film_normals, &ctx->film_albedo};
     for (auto* b : layers) CUDA_OK(ctx, cudaMemsetAsync(b->ptr, 0, n * 16, ctx->stream));
   }
+  if (ctx->film_adaptive.count == n) CUDA_OK(ctx, cudaMemsetAsync(ctx->film_adaptive.ptr, 0, n * 16, ctx->stream));
   // Film::clear applies the stored pixel size (film.cxx:365)
   ctx->pixel_size = ctx->target_pixel_size;
   ctx->launch_count = film_dims_x(ctx) * film_dims_y(ctx);
@@ -2367,6 +2443,31 @@ int etxb_read_film(etxb_ctx* ctx, uint32_t layer, float* dst_rgba, uint64_t dst_
   CUDA_OK(ctx, cudaMemcpyAsync(dst_rgba, src, n * 16, cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
   return ETXB_OK;
+}
+
+// Film::denoise (film.cxx:420-423) with the filter of DESIGN §13 in place of OpenImageDenoise: Result or Camera into the Denoised layer
+int etxb_denoise(etxb_ctx* ctx, uint32_t layer) {
+  if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;
+  if ((layer != ETXB_FILM_RESULT) && (layer != ETXB_FILM_CAMERA)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "etxb_denoise: layer %u is neither Result nor Camera", layer);
+  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
+  if ((ctx->comm != nullptr) || (ctx->world > 1u)) return fail(ctx, ETXB_ERR_UNSUPPORTED, "etxb_denoise: the film of a context with pixel tiles holds only its own tiles");
+  if (int rc = ctx_drain(ctx)) return rc;
+  cudaSetDevice(ctx->device);
+  const size_t n = ctx->path_count;
+  const bool pt = ctx->integrator == ETXB_INTEGRATOR_PT;
+  if ((ctx->film_adaptive.count != n) || (pt && (ctx->pt_info.count != n)) || (!pt && (ctx->completed < 2u)))
+    return fail(ctx, ETXB_ERR_NOT_READY, "etxb_denoise: fewer than two iterations on this film");
+  const float4* color = nullptr;
+  if (int rc = film_layer_source(ctx, layer, &color)) return rc;
+  if (ctx->film_denoised.count != n) {
+    CUDA_OK(ctx, ctx->film_denoised.alloc(n));
+    CUDA_OK(ctx, cudaMemsetAsync(ctx->film_denoised.ptr, 0, n * 16, ctx->stream));  // zeros if the variance estimate refuses
+  }
+  // the path tracer's per-pixel sample counts and its guides; the VCM: every pixel has `completed` samples and, as in the reference (whose VCM
+  // writes zero normals and albedo), no guides
+  DenoiseInputs in = {color, ctx->film_camera.ptr, ctx->film_adaptive.ptr, pt ? ctx->pt_info.ptr : nullptr, ctx->completed,
+    pt ? ctx->film_normals.ptr : nullptr, pt ? ctx->film_albedo.ptr : nullptr, ctx->width, ctx->height};
+  return run_denoise(ctx, in, ctx->film_denoised.ptr, nullptr);
 }
 
 // The tone-mapped 8-bit frame the application shows and exports (app.cxx:268-282): computed on the device, 4 bytes per pixel cross the bus.
@@ -2660,6 +2761,31 @@ int etxb_debug_math(etxb_ctx* ctx, uint32_t fn, const float* x, const float* y, 
   ctx->kernel_launches += 1;
   CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
   CUDA_OK(ctx, cudaMemcpy(out, dout.ptr, dout.bytes(), cudaMemcpyDeviceToHost));
+  return ETXB_OK;
+}
+
+// Test hook: etxb_denoise's kernels on host arrays (RGBA float per pixel, storage order; `counts` per pixel; guides may be null)
+int etxb_debug_denoise(etxb_ctx* ctx, const float* color, const float* camera, const float* half, const uint32_t* counts, const float* normals, const float* albedo,
+                       uint32_t width, uint32_t height, float* out, float* out_variance) {
+  if (!ctx || !color || !camera || !half || !counts || !out || !width || !height) return ETXB_ERR_INVALID_ARGUMENT;
+  cudaSetDevice(ctx->device);
+  const size_t n = size_t(width) * height;
+  DevBuf<float4> dc, df, dh, dn, da, dout, dvar;
+  DevBuf<uint32_t> dcount;
+  if (int rc = upload(ctx, dc, reinterpret_cast<const float4*>(color), n)) return rc;
+  if (int rc = upload(ctx, df, reinterpret_cast<const float4*>(camera), n)) return rc;
+  if (int rc = upload(ctx, dh, reinterpret_cast<const float4*>(half), n)) return rc;
+  if (int rc = upload(ctx, dcount, counts, n)) return rc;
+  if (normals)
+    if (int rc = upload(ctx, dn, reinterpret_cast<const float4*>(normals), n)) return rc;
+  if (albedo)
+    if (int rc = upload(ctx, da, reinterpret_cast<const float4*>(albedo), n)) return rc;
+  CUDA_OK(ctx, dout.alloc(n));
+  CUDA_OK(ctx, dvar.alloc(n));
+  DenoiseInputs in = {dc.ptr, df.ptr, dh.ptr, dcount.ptr, 0u, normals ? dn.ptr : nullptr, albedo ? da.ptr : nullptr, width, height};
+  if (int rc = run_denoise(ctx, in, dout.ptr, dvar.ptr)) return rc;
+  CUDA_OK(ctx, cudaMemcpy(out, dout.ptr, n * 16, cudaMemcpyDeviceToHost));
+  if (out_variance) CUDA_OK(ctx, cudaMemcpy(out_variance, dvar.ptr, n * 16, cudaMemcpyDeviceToHost));
   return ETXB_OK;
 }
 

@@ -106,6 +106,9 @@ class IntegratorAdapter {
 
   // Film::layer (film.cxx:381-418; the path tracer adds NORMALS / ALBEDO / CAMERA_ADAPTIVE): row-major float4, y flipped in storage like the reference
   int read_film(uint32_t layer, float* rgba, uint64_t bytes) { return enabled() ? etxb_read_film(_ctx, layer, rgba, bytes) : _create_result; }
+  // Film::denoise (film.cxx:420-423, the application's Denoise button): `layer` (RESULT or CAMERA) into ETXB_FILM_DENOISED, on the device; waits for
+  // the iteration in flight.  The filter is the module's own (DESIGN §13), not OpenImageDenoise.
+  int denoise(uint32_t layer) { return enabled() ? etxb_denoise(_ctx, layer) : _create_result; }
   etxb_ctx* context() { return _ctx; }
 
  protected:

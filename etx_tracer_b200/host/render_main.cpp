@@ -6,8 +6,10 @@
 // etx_tracer_b200/render.py is the same program through the ctypes mirror.
 //
 //   g++ -std=c++17 -O2 -pthread -I<repo> etx_tracer_b200/host/render_main.cpp <repo>/etx_tracer_b200/libetx_b200.so -Wl,-rpath,<repo>/etx_tracer_b200 -o etx_render
-//   etx_render scene.json -o out.exr [--integrator vcm|pt] [--spp N] [--option key=value]... [--png-exposure E] [--layer N]
+//   etx_render scene.json -o out.exr [--integrator vcm|pt] [--spp N] [--option key=value]... [--png-exposure E] [--layer N] [--denoise]
 //   etx_render --options bin/options.json -o out.exr        the application's own options file names the scene and the integrator
+//   --denoise filters the Result layer on the device (Film::denoise, the application's Denoise button) and saves the Denoised layer unless
+//   --layer names another
 //
 // Exit codes: 0 rendered and saved; 2 usage; 3 the scene could not be loaded; 4 no CUDA device (the module has no CPU path); 5 device error; 6 save failed.
 #include <chrono>
@@ -26,7 +28,7 @@ namespace {
 
 struct Arguments {
   std::string scene, output = "out.exr", integrator = "vcm", options_file;
-  bool integrator_given = false;
+  bool integrator_given = false, layer_given = false, denoise = false;
   std::vector<std::pair<std::string, double>> options;
   uint32_t spp = 0, layer = ETXB_FILM_RESULT;
   float exposure = 1.0f;
@@ -55,6 +57,9 @@ Arguments parse(int argc, char** argv) {
       const char* v = next();
       if (!v) return a;
       a.layer = uint32_t(strtoul(v, nullptr, 10));
+      a.layer_given = true;
+    } else if (s == "--denoise") {
+      a.denoise = true;
     } else if (s == "--png-exposure") {
       const char* v = next();
       if (!v) return a;
@@ -95,6 +100,7 @@ Arguments parse(int argc, char** argv) {
       }
     }
   }
+  if (a.denoise && !a.layer_given) a.layer = ETXB_FILM_DENOISED;
   a.ok = !a.scene.empty();
   return a;
 }
@@ -135,6 +141,10 @@ int pump(Integrator& integrator, const Arguments& args, etxb_scene_file* file, u
   }
   const etxb_camera* cam = etxb_scene_file_camera(file);
   std::printf("%s: %u of %u iterations, %u x %u, %.3f s\n", integrator.name(), st.completed_iterations, samples, cam->film_size[0], cam->film_size[1], seconds);
+  if (args.denoise && (integrator.denoise(ETXB_FILM_RESULT) != ETXB_OK)) {
+    std::fprintf(stderr, "could not denoise: %s\n", integrator.status_str());
+    return 5;
+  }
   uint32_t mode = ends_with(args.output, ".png") ? ETXB_SAVE_PNG_TONEMAPPED : ETXB_SAVE_EXR;
   if (etxb_save_film(integrator.context(), args.layer, args.output.c_str(), mode, args.exposure) != ETXB_OK) {
     std::fprintf(stderr, "could not save %s: %s\n", args.output.c_str(), integrator.status_str());
@@ -148,7 +158,7 @@ int pump(Integrator& integrator, const Arguments& args, etxb_scene_file* file, u
 int main(int argc, char** argv) {
   Arguments args = parse(argc, argv);
   if (!args.ok) {
-    std::fprintf(stderr, "usage: %s scene.json [-o out.exr|out.png] [--integrator vcm|pt] [--spp N] [--option key=value] [--options options.json] [--png-exposure E] [--layer N]\n", argv[0]);
+    std::fprintf(stderr, "usage: %s scene.json [-o out.exr|out.png] [--integrator vcm|pt] [--spp N] [--option key=value] [--options options.json] [--png-exposure E] [--layer N] [--denoise]\n", argv[0]);
     return 2;
   }
   char error[1024] = {};

@@ -12,7 +12,8 @@ import time
 from . import loader, structs as S
 from .api import GPUPathTracing, GPUVCM, SceneFile
 
-LAYERS = {"result": S.FILM_RESULT, "camera": S.FILM_CAMERA, "light": S.FILM_LIGHT, "normals": S.FILM_NORMALS, "albedo": S.FILM_ALBEDO}
+LAYERS = {"result": S.FILM_RESULT, "camera": S.FILM_CAMERA, "light": S.FILM_LIGHT, "normals": S.FILM_NORMALS, "albedo": S.FILM_ALBEDO,
+          "denoised": S.FILM_DENOISED}
 
 
 def main(argv=None):
@@ -21,10 +22,12 @@ def main(argv=None):
     ap.add_argument("-o", "--output", default="render.exr", help=".exr (float layer) or .png (tone-mapped)")
     ap.add_argument("--integrator", choices=("vcm", "pt"), default="vcm")
     ap.add_argument("--spp", type=int, default=0, help="iterations; 0 = the scene's `samples`")
-    ap.add_argument("--layer", choices=sorted(LAYERS), default="result")
+    ap.add_argument("--layer", choices=sorted(LAYERS), default=None, help="film layer to export (default: result, or denoised with --denoise)")
     ap.add_argument("--exposure", type=float, default=1.0, help="tone map exposure of a .png output")
     ap.add_argument("--option", action="append", default=[], metavar="KEY=VALUE", help="integrator option in the reference's ids, e.g. vcm-merging=0 or nee=0")
     ap.add_argument("--loader", choices=("cpp", "python"), default="cpp", help="the module's C++ scene loader (etxb_scene_file_load) or its Python twin (loader.py)")
+    ap.add_argument("--denoise", action="store_true", help="denoise the Result layer before the export (the application's Denoise button); "
+                    "--layer defaults to denoised")
     ap.add_argument("--noise-threshold", type=float, default=None, help="pt: Scene::noise_threshold of the adaptive sampling (default: the scene's)")
     args = ap.parse_args(argv)
 
@@ -48,7 +51,10 @@ def main(argv=None):
     st = g.status()
     n = sd.width * sd.height * st["completed_iterations"]
     print(f"{st['completed_iterations']} iterations in {st['total_time']:.3f} s of device time: {n / max(st['total_time'], 1e-9) / 1e6:.2f} Msamples/s", file=sys.stderr)
-    g.save_image(args.output, LAYERS[args.layer], tonemapped=args.output.lower().endswith(".png"), exposure=args.exposure)
+    if args.denoise:
+        g.denoise(S.FILM_RESULT)
+    layer = args.layer or ("denoised" if args.denoise else "result")
+    g.save_image(args.output, LAYERS[layer], tonemapped=args.output.lower().endswith(".png"), exposure=args.exposure)
     print(args.output)
     g.close()
     return 0

@@ -172,7 +172,7 @@ VCM_CONNECT_ONLY = VCM_DIRECT_HIT | VCM_CONNECT_TO_LIGHT | VCM_CONNECT_TO_CAMERA
 VCM_FULL = VCM_CONNECT_ONLY | VCM_ENABLE_MERGING | VCM_MERGE_VERTICES
 
 # film layers / buffer ids (include/etx_b200.h)
-FILM_RESULT, FILM_CAMERA, FILM_LIGHT, FILM_LIGHT_ITERATION, FILM_NORMALS, FILM_ALBEDO, FILM_CAMERA_ADAPTIVE = range(7)
+FILM_RESULT, FILM_CAMERA, FILM_LIGHT, FILM_LIGHT_ITERATION, FILM_NORMALS, FILM_ALBEDO, FILM_CAMERA_ADAPTIVE, FILM_DENOISED = range(8)
 (BUF_LIGHT_PATH_COUNT, BUF_LIGHT_PATH_OFFSET, BUF_LIGHT_PATH_WAVELENGTH, BUF_LIGHT_SAMPLER, BUF_CAMERA_SAMPLER, BUF_LV_POS,
  BUF_LV_THROUGHPUT, BUF_LV_MIS, BUF_FILM_LIGHT_ITERATION, BUF_FILM_CAMERA, BUF_FILM_LIGHT, BUF_PHOTON_RECORDS,
  BUF_CAMERA_GATHERED, BUF_PIXEL_INFO, BUF_PIXEL_ERROR, BUF_BVH_NODES, BUF_BVH_TRIS, BUF_WIDE_NODES) = range(18)

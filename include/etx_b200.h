@@ -268,7 +268,10 @@ enum {
   /* layers the path tracer fills (Film::Normals shown as n * 0.5 + 0.5, Film::Albedo, Film::CameraAdaptive; film.cxx:406-414) */
   ETXB_FILM_NORMALS = 4,
   ETXB_FILM_ALBEDO = 5,
-  ETXB_FILM_CAMERA_ADAPTIVE = 6
+  /* the mean of the even-indexed samples, kept by both integrators: the second half buffer of etxb_denoise's variance estimate */
+  ETXB_FILM_CAMERA_ADAPTIVE = 6,
+  /* Film::Denoised: the last etxb_denoise; zeros before it, kept until the next etxb_denoise or a film resize */
+  ETXB_FILM_DENOISED = 7
 };
 
 /* Named device buffers for etxb_read_buffer / etxb_device_pointer (parity tests + multi-GPU exchange). */
@@ -488,6 +491,12 @@ int etxb_stop(etxb_ctx* ctx, int wait_for_iteration);
 /* Film::layer (film.cxx:381-418): row-major float4, y already flipped in storage like the reference. */
 int etxb_read_film(etxb_ctx* ctx, uint32_t layer, float* dst_rgba, uint64_t dst_bytes);
 int etxb_film_size(const etxb_ctx* ctx, uint32_t* width, uint32_t* height);
+/* Film::denoise(layer) (film.cxx:420-423): filters ETXB_FILM_RESULT or ETXB_FILM_CAMERA into ETXB_FILM_DENOISED on the device.  The filter is
+ * non-local means with a two-half-buffer variance estimate and, for the path tracer, normal and albedo feature weights (DESIGN §13) — not
+ * OpenImageDenoise, whose trained weights this module does not have.  Drains the context first, like etxb_read_film.  ETXB_ERR_INVALID_ARGUMENT
+ * for other layers; ETXB_ERR_NOT_READY without a scene or where a pixel has fewer than two samples; ETXB_ERR_UNSUPPORTED on a context with a
+ * communicator or a pixel partition (its film holds only its own tiles).  The same output for the same film on the same build. */
+int etxb_denoise(etxb_ctx* ctx, uint32_t layer);
 
 int etxb_get_counters(etxb_ctx* ctx, etxb_counters* out);
 /* Per-kernel device time of the last iteration (CUDA events): names[i] -> ms[i]; returns count. */
@@ -522,6 +531,11 @@ typedef struct etxb_debug_trees {
 } etxb_debug_trees;
 int etxb_debug_build_trees(etxb_ctx* ctx, const float* positions, uint32_t vertex_count, const uint32_t* indices, uint32_t triangle_count, uint32_t device,
                            etxb_debug_trees* out);
+/* etxb_denoise's kernels on host arrays: color / camera / half / normals / albedo / out / out_variance are float[4 * width * height] (RGBA,
+ * one layout for every array); counts = uint32[width * height] samples per pixel; normals and albedo may be null (no feature weight) and
+ * out_variance may be null.  out_variance receives the smoothed per-pixel variance of the mean.  ETXB_ERR_NOT_READY where a count is below 2. */
+int etxb_debug_denoise(etxb_ctx* ctx, const float* color, const float* camera, const float* half, const uint32_t* counts, const float* normals,
+                       const float* albedo, uint32_t width, uint32_t height, float* out, float* out_variance);
 /* Sampler / spectral KATs evaluated on the device (sampler.hxx:54,66; spectrum.hxx:219,234). */
 int etxb_debug_sampler(etxb_ctx* ctx, const uint32_t* a, const uint32_t* b, uint32_t count, uint32_t draws, uint32_t* out_seed, float* out_values);
 int etxb_debug_math(etxb_ctx* ctx, uint32_t fn, const float* x, const float* y, uint32_t count, float* out);
