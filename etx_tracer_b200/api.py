@@ -82,8 +82,6 @@ def load_library(flavor="fast"):
     lib.etxb_group_wait.argtypes = [vp]
     lib.etxb_group_poll.argtypes = [vp, vp]
     lib.etxb_group_read_film.argtypes = [vp, u32, vp, u64]
-    lib.etxb_group_set_stride.argtypes = [vp, u32]
-    lib.etxb_group_combine.argtypes = [vp, u32, C.POINTER(vp), C.POINTER(u64), C.POINTER(u32)]
     lib.etxb_comm_unique_id.argtypes = [vp, u64]
     lib.etxb_comm_init.argtypes = [vp, u32, u32, vp, u64]
     lib.etxb_comm_world.argtypes = [vp, C.POINTER(u32), C.POINTER(u32)]
@@ -101,14 +99,10 @@ def load_library(flavor="fast"):
     lib.etxb_pt_get_status.argtypes = [vp, vp]
     lib.etxb_set_scene_settings.argtypes = [vp, C.c_float, C.c_float]
     lib.etxb_set_partition.argtypes = [vp, u32, u32]
-    lib.etxb_set_iteration_stride.argtypes = [vp, u32]
     lib.etxb_begin.argtypes = [vp, u32]
     lib.etxb_set_film_pixel_size.argtypes = [vp, u32]
     lib.etxb_group_set_film_pixel_size.argtypes = [vp, u32]
     lib.etxb_enqueue_iteration.argtypes = [vp]
-    lib.etxb_enqueue_light_pass.argtypes = [vp]
-    lib.etxb_enqueue_grid_build.argtypes = [vp, vp, u64]
-    lib.etxb_enqueue_camera_pass.argtypes = [vp]
     lib.etxb_poll.argtypes = [vp, vp]
     lib.etxb_wait.argtypes = [vp]
     lib.etxb_stop.argtypes = [vp, C.c_int]
@@ -124,7 +118,6 @@ def load_library(flavor="fast"):
     lib.etxb_get_counters.argtypes = [vp, vp]
     lib.etxb_get_kernel_times.argtypes = [vp, C.POINTER(C.c_char_p), C.POINTER(C.c_float), C.POINTER(u32), u32]
     lib.etxb_read_buffer.argtypes = [vp, u32, vp, u64, C.POINTER(u64)]
-    lib.etxb_device_pointer.argtypes = [vp, u32, C.POINTER(vp), C.POINTER(u64)]
     lib.etxb_stream.restype = vp
     lib.etxb_stream.argtypes = [vp]
     lib.etxb_debug_trace.argtypes = [vp, vp, vp, u32, vp, vp]
@@ -385,10 +378,6 @@ class GPUVCM:
         s x s block of the film takes its path's value; the film stays W x H."""
         self._check(self.lib.etxb_set_film_pixel_size(self.h, size))
 
-    def set_iteration_stride(self, stride):
-        """This context renders iterations first, first + stride, ... (iteration-interleaved multi-GPU runs)."""
-        self._check(self.lib.etxb_set_iteration_stride(self.h, stride))
-
     def _push_options(self):
         self._check(self.lib.etxb_set_options(self.h, _p(self.options)))
 
@@ -426,16 +415,6 @@ class GPUVCM:
 
     def iterate(self):
         self._check(self.lib.etxb_enqueue_iteration(self.h))
-
-    def light_pass(self):
-        self._check(self.lib.etxb_enqueue_light_pass(self.h))
-
-    def grid_build(self, records_ptr=None, count=0):
-        """complete_light_vertices: commits the light image, builds the photon grid (from gathered records in multi-GPU runs)."""
-        self._check(self.lib.etxb_enqueue_grid_build(self.h, records_ptr, count))
-
-    def camera_pass(self):
-        self._check(self.lib.etxb_enqueue_camera_pass(self.h))
 
     def stop(self, wait_for_iteration=True):
         self._running = False
@@ -491,11 +470,6 @@ class GPUVCM:
         if n.value:
             self._check(self.lib.etxb_read_buffer(self.h, buf_id, _p(out), out.nbytes, C.byref(n)))
         return out
-
-    def device_pointer(self, buf_id):
-        ptr, n = C.c_void_p(), C.c_uint64(0)
-        self._check(self.lib.etxb_device_pointer(self.h, buf_id, C.byref(ptr), C.byref(n)))
-        return ptr.value, n.value
 
     def stream(self):
         return self.lib.etxb_stream(self.h)
@@ -767,18 +741,8 @@ class GPUVCMGroup:
         self._check(self.lib.etxb_group_comm_reduce_film(self.h, layer, _p(out) if rank == 0 else None, out.nbytes if rank == 0 else 0))
         return out if rank == 0 else None
 
-    def set_stride(self, stride):
-        """Iteration-interleaved multi-GPU runs: this group renders indices first, first + stride, ..."""
-        self._check(self.lib.etxb_group_set_stride(self.h, stride))
-
     def enqueue(self, iterations=1):
         self._check(self.lib.etxb_group_enqueue(self.h, iterations))
-
-    def combined(self, layer=S.FILM_RESULT):
-        """(device pointer, bytes, iterations) of the combined layer, left on the device."""
-        ptr, n, done = C.c_void_p(), C.c_uint64(0), C.c_uint32(0)
-        self._check(self.lib.etxb_group_combine(self.h, layer, C.byref(ptr), C.byref(n), C.byref(done)))
-        return ptr.value, n.value, done.value
 
     def wait(self):
         self._check(self.lib.etxb_group_wait(self.h))

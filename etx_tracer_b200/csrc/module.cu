@@ -254,7 +254,7 @@ struct etxb_ctx {
 
   etxb_vcm_options options = {};
   uint32_t iteration = 0;            // absolute iteration index (VCMIteration::iteration)
-  uint32_t iteration_stride = 1;     // etxb_set_iteration_stride: this context renders iterations first, first + stride, ...
+  bool external_iteration = false;   // etxb_set_next_iteration: the caller sets every iteration's index, it does not advance by itself
   uint32_t completed = 0;            // iterations finished since etxb_begin
   uint32_t rank = 0, world = 1;
   bool light_full = false;           // camera-split iterations (etxb_group replicas): the partition applies to the camera pass only, the light pass traces every path
@@ -263,7 +263,6 @@ struct etxb_ctx {
   double last_iteration_time = 0.0, total_time = 0.0;
   uint64_t kernel_launches = 0;
   GridData grid = {};
-  bool light_pass_done = false, grid_done = false;
   // queue sizes from which a pass takes its large-queue branches (etxb_debug_set_thresholds; 0 = always, 0xffffffff = never), and what ran
   etxb_debug_thresholds thresholds = kDefaultThresholds;
   etxb_debug_branch_counts branch_counts = {};
@@ -383,7 +382,7 @@ struct etxb_group {
   std::vector<std::thread> workers;
   std::mutex m;
   std::condition_variable cv_work, cv_idle;
-  uint32_t first_iteration = 0, stride = 1, taken = 0;  // the k-th iteration handed out renders index first + k * stride
+  uint32_t first_iteration = 0, taken = 0;  // the k-th iteration handed out renders index first + k
   uint32_t in_flight = 0;
   WorkPlan plan;
   bool quit = false;
@@ -748,18 +747,16 @@ int run_light_pass(etxb_ctx* ctx) {
   }
   ctx->last_light_vertices = total;
   CUDA_OK(ctx, cudaGetLastError());
-  ctx->light_pass_done = true;
   return ETXB_OK;
 }
 
 template <bool SP>
 int run_grid_build(etxb_ctx* ctx, const LightVertexRec* records, uint32_t count) {
   ctx->grid = {};
-  ctx->grid_done = true;
   LaunchParams p = make_params(ctx);
   {
-    // complete_light_vertices -> Film::commit_light_iteration(iteration) (vcm_cpu.cxx:209-211); in a multi-GPU run the
-    // host has all-reduced ETXB_BUF_FILM_LIGHT_ITERATION across ranks before this call
+    // complete_light_vertices -> Film::commit_light_iteration(iteration) (vcm_cpu.cxx:209-211); with pixel tiles over several GPUs
+    // comm_exchange has all-reduced the per-iteration light image across ranks before this call
     LaunchTimer t(ctx, K_FILM_COMMIT);
     // the running mean counts the iterations THIS context has accumulated since etxb_begin (= the absolute index in the reference's flow,
     // which always starts at 0; after etxb_begin(ctx, k != 0) or with interleaved iterations the absolute index would scale the first
@@ -959,11 +956,10 @@ int run_camera_pass(etxb_ctx* ctx) {
 //   (b) merging queries the photon map of ALL light paths (vcm_cpu.cxx:219-221): all-gather of the path-major vertex records (96 B each, block
 //       sizes differ per rank: counts first, then one broadcast per owner inside a group call = an uneven all-gather), into the allocation-order
 //       pool, which is free once the path-major pool exists; every rank then builds the same grid.
-// Camera tiles are disjoint: they meet only when a frame is wanted (etxb_comm_reduce_film).
-int comm_exchange(etxb_ctx* ctx, const void** records, uint64_t* count) {
+// Camera tiles are disjoint: they meet only when a frame is wanted (etxb_comm_reduce_film).  With merging on, `records` / `count` are set to
+// the gathered pool; otherwise they are left as they are.
+int comm_exchange(etxb_ctx* ctx, const LightVertexRec** records, uint32_t* count) {
   NcclApi* n = nccl_api();
-  *records = nullptr;
-  *count = 0;
   // the collectives run on the context's high-priority stream, fenced against its work stream by events on both sides
   cudaStream_t cs = ctx->comm_stream;
   auto fence_out = [&]() -> cudaError_t {
@@ -1008,7 +1004,7 @@ int comm_exchange(etxb_ctx* ctx, const void** records, uint64_t* count) {
     NCCL_OK(ctx, n->GroupEnd());
     CUDA_OK(ctx, fence_out());
     *records = ctx->lv_tmp.ptr;
-    *count = total;
+    *count = uint32_t(total);
   }
   return ETXB_OK;
 }
@@ -1031,9 +1027,7 @@ int finish_iteration(etxb_ctx* ctx) {
   ctx->total_time += ctx->last_iteration_time;
   resolve_timers(ctx);
   ctx->completed += 1;
-  ctx->iteration += ctx->iteration_stride;
-  ctx->light_pass_done = false;
-  ctx->grid_done = false;
+  if (!ctx->external_iteration) ctx->iteration += 1;
   return ETXB_OK;
 }
 
@@ -1709,6 +1703,27 @@ int commit_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, Sce
   return etxb_begin(ctx, 0);
 }
 
+// The three passes of a VCM iteration, each instantiated for the context's scene class.  The light pass starts the iteration's clock,
+// the camera pass stops it (finish_iteration).
+int light_pass(etxb_ctx* ctx) {
+  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
+  cudaSetDevice(ctx->device);
+  CUDA_OK(ctx, cudaEventRecord(ctx->ev_iter_start, ctx->stream));
+  if (ctx->spectral) return ctx->plain_scene ? run_light_pass<true, true>(ctx) : run_light_pass<true, false>(ctx);
+  return ctx->plain_scene ? run_light_pass<false, true>(ctx) : run_light_pass<false, false>(ctx);
+}
+
+int grid_build(etxb_ctx* ctx, const LightVertexRec* records, uint32_t count) {
+  return ctx->spectral ? run_grid_build<true>(ctx, records, count) : run_grid_build<false>(ctx, records, count);
+}
+
+int camera_pass(etxb_ctx* ctx) {
+  int rc = ctx->spectral ? (ctx->plain_scene ? run_camera_pass<true, true>(ctx) : run_camera_pass<true, false>(ctx))
+                         : (ctx->plain_scene ? run_camera_pass<false, true>(ctx) : run_camera_pass<false, false>(ctx));
+  if (rc) return rc;
+  return finish_iteration(ctx);
+}
+
 // one whole iteration on the calling thread; returns when it has finished (the bounce loops read queue sizes back)
 int run_iteration_blocking(etxb_ctx* ctx) {
   if (ctx->integrator == ETXB_INTEGRATOR_PT) {
@@ -1716,14 +1731,14 @@ int run_iteration_blocking(etxb_ctx* ctx) {
     if (ctx->spectral) return ctx->plain_scene ? run_pt_iteration<true, true>(ctx) : run_pt_iteration<true, false>(ctx);
     return ctx->plain_scene ? run_pt_iteration<false, true>(ctx) : run_pt_iteration<false, false>(ctx);
   }
-  if (int rc = etxb_enqueue_light_pass(ctx)) return rc;
-  const void* records = nullptr;
-  uint64_t count = 0;
+  if (int rc = light_pass(ctx)) return rc;
+  const LightVertexRec* records = ctx->lv_final.ptr;
+  uint32_t count = ctx->last_light_vertices;
   if (ctx->comm != nullptr) {  // pixel tiles over several GPUs: light image + photon records are exchanged here (comm_exchange)
     if (int rc = comm_exchange(ctx, &records, &count)) return rc;
   }
-  if (int rc = etxb_enqueue_grid_build(ctx, records, count)) return rc;
-  return etxb_enqueue_camera_pass(ctx);
+  if (int rc = grid_build(ctx, records, count)) return rc;
+  return camera_pass(ctx);
 }
 
 void ctx_worker(etxb_ctx* ctx) {
@@ -1921,7 +1936,7 @@ void group_worker(etxb_group* grp, uint32_t lane) {
     const WorkItem item = queue.front();
     queue.pop_front();
     grp->taken = std::max(grp->taken, item.ordinal + 1u);
-    uint32_t iteration = grp->first_iteration + item.ordinal * grp->stride;
+    uint32_t iteration = grp->first_iteration + item.ordinal;
     grp->in_flight += 1;
     lock.unlock();
     if (item.parts > 1u) {
@@ -2165,16 +2180,10 @@ int etxb_set_partition(etxb_ctx* ctx, uint32_t rank, uint32_t world) {
   return ETXB_OK;
 }
 
-int etxb_set_iteration_stride(etxb_ctx* ctx, uint32_t stride) {
-  if (!ctx || (stride == 0u)) return ETXB_ERR_INVALID_ARGUMENT;
-  ctx->iteration_stride = stride;
-  return ETXB_OK;
-}
-
 int etxb_set_next_iteration(etxb_ctx* ctx, uint32_t iteration) {
   if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;
   ctx->iteration = iteration;
-  ctx->iteration_stride = 0;  // externally driven: no auto-advance, the film mean counts this context's own iterations
+  ctx->external_iteration = true;  // no auto-advance; the film mean counts this context's own iterations
   return ETXB_OK;
 }
 
@@ -2220,44 +2229,9 @@ int etxb_begin(etxb_ctx* ctx, uint32_t first_iteration) {
   ctx->overflow_flag = 0;
   ctx->kernel_launches = 0;
   ctx->branch_counts = {};
-  ctx->light_pass_done = ctx->grid_done = false;
   memset(ctx->kernel_ms, 0, sizeof(ctx->kernel_ms));
   memset(ctx->kernel_count, 0, sizeof(ctx->kernel_count));
   return ETXB_OK;
-}
-
-int etxb_enqueue_light_pass(etxb_ctx* ctx) {
-  if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;
-  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
-  cudaSetDevice(ctx->device);
-  CUDA_OK(ctx, cudaEventRecord(ctx->ev_iter_start, ctx->stream));
-  if (ctx->spectral) return ctx->plain_scene ? run_light_pass<true, true>(ctx) : run_light_pass<true, false>(ctx);
-  return ctx->plain_scene ? run_light_pass<false, true>(ctx) : run_light_pass<false, false>(ctx);
-}
-
-int etxb_enqueue_grid_build(etxb_ctx* ctx, const void* device_photon_records, uint64_t photon_count) {
-  if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;
-  if (!ctx->light_pass_done) return fail(ctx, ETXB_ERR_NOT_READY, "light pass has not run");
-  cudaSetDevice(ctx->device);
-  const LightVertexRec* records = ctx->lv_final.ptr;
-  uint32_t count = ctx->last_light_vertices;
-  if (device_photon_records != nullptr) {
-    // multi-GPU: the caller all-gathered every rank's path-major records (ETXB_BUF_PHOTON_RECORDS, 96 B each) into one device buffer
-    if (photon_count > ctx->lv_capacity) return fail(ctx, ETXB_ERR_OVERFLOW, "gathered photon count %llu exceeds capacity %u", (unsigned long long)photon_count, ctx->lv_capacity);
-    records = static_cast<const LightVertexRec*>(device_photon_records);
-    count = uint32_t(photon_count);
-  }
-  return ctx->spectral ? run_grid_build<true>(ctx, records, count) : run_grid_build<false>(ctx, records, count);
-}
-
-int etxb_enqueue_camera_pass(etxb_ctx* ctx) {
-  if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;
-  if (!ctx->light_pass_done || !ctx->grid_done) return fail(ctx, ETXB_ERR_NOT_READY, "light pass / grid build have not run");
-  cudaSetDevice(ctx->device);
-  int rc = ctx->spectral ? (ctx->plain_scene ? run_camera_pass<true, true>(ctx) : run_camera_pass<true, false>(ctx))
-                         : (ctx->plain_scene ? run_camera_pass<false, true>(ctx) : run_camera_pass<false, false>(ctx));
-  if (rc) return rc;
-  return finish_iteration(ctx);
 }
 
 int etxb_enqueue_iteration(etxb_ctx* ctx) {
@@ -2541,8 +2515,9 @@ int etxb_get_kernel_times(etxb_ctx* ctx, const char** names, float* ms, uint32_t
   return int(K_COUNT);
 }
 
-int etxb_device_pointer(etxb_ctx* ctx, uint32_t buffer_id, void** out_ptr, uint64_t* out_bytes) {
-  if (!ctx || !out_ptr || !out_bytes) return ETXB_ERR_INVALID_ARGUMENT;
+namespace {
+// the device buffer behind an ETXB_BUF_* id that etxb_read_buffer copies as it is
+int buffer_pointer(etxb_ctx* ctx, uint32_t buffer_id, void** out_ptr, uint64_t* out_bytes) {
   size_t n = ctx->path_count;
   switch (buffer_id) {
     case ETXB_BUF_LIGHT_PATH_COUNT: *out_ptr = ctx->lv_count.ptr; *out_bytes = n * 4; break;
@@ -2577,6 +2552,7 @@ int etxb_device_pointer(etxb_ctx* ctx, uint32_t buffer_id, void** out_ptr, uint6
   }
   return ETXB_OK;
 }
+}  // namespace
 
 int etxb_read_buffer(etxb_ctx* ctx, uint32_t buffer_id, void* dst, uint64_t dst_bytes, uint64_t* out_bytes) {
   if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;
@@ -2605,7 +2581,7 @@ int etxb_read_buffer(etxb_ctx* ctx, uint32_t buffer_id, void* dst, uint64_t dst_
   }
   void* ptr = nullptr;
   uint64_t bytes = 0;
-  if (int rc = etxb_device_pointer(ctx, buffer_id, &ptr, &bytes)) return rc;
+  if (int rc = buffer_pointer(ctx, buffer_id, &ptr, &bytes)) return rc;
   if (buffer_id == ETXB_BUF_CAMERA_GATHERED) {
     uint64_t need = uint64_t(ctx->path_count) * 12;
     if (out_bytes) *out_bytes = need;
@@ -3080,13 +3056,6 @@ int etxb_group_update_scene(etxb_group* grp, const void* scene_blob, uint64_t sc
   return etxb_group_begin(grp, 0);
 }
 
-int etxb_group_set_stride(etxb_group* grp, uint32_t stride) {
-  if (!grp || (stride == 0u)) return ETXB_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> lock(grp->m);
-  grp->stride = stride;
-  return ETXB_OK;
-}
-
 int etxb_group_enqueue(etxb_group* grp, uint32_t iterations) {
   if (!grp) return ETXB_ERR_INVALID_ARGUMENT;
   {
@@ -3111,19 +3080,11 @@ int etxb_group_poll(etxb_group* grp, etxb_status* status) {
     status->light_vertices = std::max(status->light_vertices, c->last_light_vertices);
     status->overflow |= c->overflow_flag;
   }
-  status->current_iteration = grp->first_iteration + grp->taken * grp->stride;
+  status->current_iteration = grp->first_iteration + grp->taken;
   status->iteration_in_flight = group_idle(grp) ? 0u : 1u;
   status->last_iteration_time = grp->last_iteration_seconds;
   status->total_time = grp->busy_seconds;
   if (status->iteration_in_flight) status->total_time += std::chrono::duration<double>(std::chrono::steady_clock::now() - grp->busy_since).count();
-  return ETXB_OK;
-}
-
-int etxb_group_combine(etxb_group* grp, uint32_t layer, void** device_ptr, uint64_t* bytes, uint32_t* completed) {
-  if (!grp || (layer > ETXB_FILM_LIGHT)) return ETXB_ERR_INVALID_ARGUMENT;
-  if (int rc = group_combine_into(grp, layer, grp->combined, completed)) return rc;
-  if (device_ptr) *device_ptr = grp->combined.ptr;
-  if (bytes) *bytes = uint64_t(grp->lanes[0]->path_count) * 16u;
   return ETXB_OK;
 }
 
@@ -3260,12 +3221,11 @@ int etxb_group_comm_reduce_film(etxb_group* grp, uint32_t layer, float* dst_rgba
 }
 
 int etxb_group_read_film(etxb_group* grp, uint32_t layer, float* dst_rgba, uint64_t dst_bytes) {
-  if (!grp || !dst_rgba) return ETXB_ERR_INVALID_ARGUMENT;
-  void* src = nullptr;
-  uint64_t bytes = 0;
-  if (int rc = etxb_group_combine(grp, layer, &src, &bytes, nullptr)) return rc;
+  if (!grp || !dst_rgba || (layer > ETXB_FILM_LIGHT)) return ETXB_ERR_INVALID_ARGUMENT;
+  if (int rc = group_combine_into(grp, layer, grp->combined, nullptr)) return rc;
   etxb_ctx* first = grp->lanes[0];
+  const uint64_t bytes = uint64_t(first->path_count) * 16u;
   if (dst_bytes < bytes) return fail(first, ETXB_ERR_INVALID_ARGUMENT, "film buffer too small");
-  CUDA_OK(first, cudaMemcpy(dst_rgba, src, bytes, cudaMemcpyDeviceToHost));
+  CUDA_OK(first, cudaMemcpy(dst_rgba, grp->combined.ptr, bytes, cudaMemcpyDeviceToHost));
   return ETXB_OK;
 }

@@ -1,154 +1,18 @@
-"""Multi-GPU drivers (one process per GPU), SURVEY.md §8(e).
+"""The host's part in a multi-GPU render (one process per GPU).
 
-Two ways to spread a render over the ranks:
-
-* InterleavedVCM (default of bench.py): the unit of work is one ITERATION of the whole frame.  Rank r renders iterations r, r + N,
-  r + 2N, ... (the iteration index drives the merge radius and the sampler seeds, so the set of iterations rendered is exactly the
-  single-GPU sequence); there is no data-path collective, only one reduce of the float4 film when a frame is wanted.  VCM
-  iterations are independent by construction (vcm_cpu.cxx:95-113), and this keeps every GPU on full-size wavefronts.
-* ShardedVCM: pixel-tile sharding of ONE iteration, below.  Needed when a single iteration must finish sooner (interactive
-  preview); it pays for replicating the photon map on every rank and for the latency-bound tails of the bounce loops, which do not
-  shrink with the tile count.
-
-Pixel-tile sharding of one VCM iteration across ranks:
-
-Per iteration:  light pass on the rank's tiles  ->  all-reduce(sum) of the per-iteration light image (splats land anywhere)
-                ->  all-gather of the ranks' photon records (the merge queries the GLOBAL photon map; skipped when merging is off)
-                ->  grid build + camera pass on the rank's tiles.
-At the end:     reduce(sum) of the camera image to rank 0 (tiles are disjoint, non-owned pixels are zero).
-
-The exchange is plain `torch.distributed` (NCCL on GPUs; gloo on CPU for the host-logic tests), on buffers the CUDA module
-exposes through etxb_device_pointer.  There is no fused compute+collective here: the path has no dense step feeding a
-collective — each exchange happens once per iteration on data that is complete only when its pass has finished.
+The module runs every multi-GPU exchange itself, over NCCL: the pixel-tile exchange inside etxb_enqueue_iteration (etxb_comm_init,
+etxb_group_comm_init) and the frame reduce of whole-frame replicas (etxb_group_comm_init_replicas).  All the host does is hand the same NCCL
+unique ids to every rank, over whatever process group the launcher set up.
 """
-import numpy as np
-
 from . import structs as S
 
-RECORD_BYTES = 96  # LightVertexRec (etx_tracer_b200/csrc/dvcm.cuh)
-
-
-def tile_owner(width, height, world, tile=32):
-    """owner[y, x] = rank owning the pixel: 32x32 tiles dealt round-robin (must match pixel_owned() in kernels.cuh)."""
-    ys, xs = np.mgrid[0:height, 0:width]
-    tiles_x = (width + tile - 1) // tile
-    return (((ys // tile) * tiles_x + (xs // tile)) % world).astype(np.int32)
-
-
-def gather_layout(counts):
-    """Offsets of each rank's block in the gathered photon buffer + total."""
-    counts = [int(c) for c in counts]
-    offsets = [0]
-    for c in counts[:-1]:
-        offsets.append(offsets[-1] + c)
-    return offsets, sum(counts)
-
-
-class DevicePointerTensor:
-    """Zero-copy torch view of a raw device pointer via __cuda_array_interface__."""
-
-    def __init__(self, ptr, nbytes, dtype="<f4"):
-        item = np.dtype(dtype).itemsize
-        self.__cuda_array_interface__ = {"shape": (nbytes // item,), "typestr": dtype, "data": (ptr, False), "version": 2}
-
-
-def as_tensor(ptr, nbytes, dtype="<f4", device="cuda"):
-    import torch
-    return torch.as_tensor(DevicePointerTensor(ptr, nbytes, dtype), device=device)
-
-
-class ShardedVCM:
-    """Drives GPUVCM instances of all ranks through one iteration with the exchanges in between."""
-
-    def __init__(self, gpu, dist, rank, world, device="cuda", view=as_tensor):
-        """`gpu` is an api.GPUVCM; `device`/`view` exist so the exchange logic can be driven on CPU tensors over gloo
-        (tests/test_multigpu_host.py) with a stand-in that exposes the same light_pass / grid_build / camera_pass / device_pointer."""
-        import torch
-        self.g, self.dist, self.rank, self.world, self.torch = gpu, dist, rank, world, torch
-        self.device, self.view = device, view
-        gpu.set_partition(rank, world)
-        self._gather_buf = None
-        self.phase_seconds = None  # set to {} to collect per-phase wall time (adds a device sync at every phase boundary)
-        self._t = 0.0
-
-    def _mark(self, name):
-        if self.phase_seconds is None:
-            return
-        import time
-        if self.device == "cuda":
-            self.g.wait()
-            self.torch.cuda.synchronize()
-        now = time.perf_counter()
-        if name is not None:
-            self.phase_seconds[name] = self.phase_seconds.get(name, 0.0) + (now - self._t)
-        self._t = now
-
-    def _sync(self):
-        if self.device == "cuda":
-            self.torch.cuda.current_stream().synchronize()
-
-    def merging(self):
-        o = int(self.g.options["options"][0])
-        return bool(o & S.VCM_ENABLE_MERGING) and bool(o & S.VCM_MERGE_VERTICES)
-
-    def iterate(self):
-        torch, dist, g = self.torch, self.dist, self.g
-        self._mark(None)
-        g.light_pass()
-        self._mark("light_pass")
-        ptr, nbytes = g.device_pointer(S.BUF_FILM_LIGHT_ITERATION)
-        dist.all_reduce(self.view(ptr, nbytes), op=dist.ReduceOp.SUM)
-        self._mark("light_image_all_reduce")
-        records_ptr, total = None, 0
-        if self.merging():
-            ptr, nbytes = g.device_pointer(S.BUF_PHOTON_RECORDS)
-            mine = nbytes // RECORD_BYTES
-            counts = torch.zeros(self.world, dtype=torch.int64, device=self.device)
-            dist.all_gather_into_tensor(counts, torch.tensor([mine], dtype=torch.int64, device=self.device))
-            counts = counts.tolist()
-            offsets, total = gather_layout(counts)
-            need = max(total, 1) * RECORD_BYTES // 4
-            if self._gather_buf is None or self._gather_buf.numel() < need:
-                self._gather_buf = torch.empty(int(need * 1.25) + 1024, dtype=torch.float32, device=self.device)
-            outs = [self._gather_buf[offsets[r] * RECORD_BYTES // 4:(offsets[r] + counts[r]) * RECORD_BYTES // 4] for r in range(self.world)]
-            if mine:
-                outs[self.rank].copy_(self.view(ptr, nbytes))
-            # blocks differ in size per rank: one broadcast per owner into its slice (what an uneven all_gather lowers to)
-            pending = [dist.broadcast(outs[r], src=r, async_op=True) for r in range(self.world) if counts[r]]
-            for work in pending:
-                work.wait()
-            records_ptr = self._gather_buf.data_ptr()
-        self._sync()
-        self._mark("photon_exchange")
-        g.grid_build(records_ptr, total)
-        self._mark("grid_build")
-        g.camera_pass()
-        self._mark("camera_pass")
-
-    def reduce_film(self):
-        """Sum the (disjoint) camera tiles on rank 0; returns the Result layer there, None elsewhere."""
-        torch, dist, g = self.torch, self.dist, self.g
-        ptr, nbytes = g.device_pointer(S.BUF_FILM_CAMERA)
-        # reduce a COPY: the live film keeps only this rank's own tiles, so a second call (progressive preview) does not double-count
-        live = self.view(ptr, nbytes)
-        total = live.clone()
-        dist.reduce(total, dst=0, op=dist.ReduceOp.SUM)
-        self._sync()
-        if self.rank != 0:
-            return None
-        mine = live.clone()
-        live.copy_(total)
-        self._sync()
-        result = g.film(S.FILM_RESULT).copy()
-        live.copy_(mine)
-        self._sync()
-        return result
+# bytes of one ETXB_BUF_PHOTON_RECORDS record; kept at this import path for code written against the earlier host-driven exchange
+RECORD_BYTES = S.LIGHT_VERTEX_REC.itemsize
 
 
 def distribute_comm_ids(dist, rank, count, make_ids, device="cuda"):
-    """The one thing the host does for the module's own multi-GPU path (etxb_comm_init / etxb_group_comm_init): rank 0 asks the module for
-    `count` NCCL unique ids (make_ids(count) -> uint8[count * 128]) and every rank receives the same bytes (one broadcast over whatever process
-    group the launcher set up)."""
+    """Rank 0 asks the module for `count` NCCL unique ids (make_ids(count) -> uint8[count * 128]) and every rank receives the same bytes (one
+    broadcast over `dist`'s default process group)."""
     import numpy as np
     import torch
     n = count * 128
@@ -159,63 +23,3 @@ def distribute_comm_ids(dist, rank, count, make_ids, device="cuda"):
         buf.copy_(torch.from_numpy(ids))
     dist.broadcast(buf, src=0)
     return buf.cpu().numpy()
-
-
-class InterleavedVCM:
-    """Iteration-interleaved rendering: rank r owns iterations r, r + world, r + 2 world, ...
-
-    `group` is an api.GPUVCMGroup (several iterations in flight on this rank's GPU).  `enqueue(n)` queues n more of this rank's
-    iterations, `reduce_film()` combines the per-rank means (each over the iterations that rank finished) into the mean over all
-    iterations on rank 0: sum_r n_r * film_r / sum_r n_r, one reduce of the float4 Result layer."""
-
-    def __init__(self, group, dist, rank, world, device="cuda", view=as_tensor):
-        import torch
-        self.g, self.dist, self.rank, self.world, self.torch = group, dist, rank, world, torch
-        self.device, self.view = device, view
-        group.set_stride(world)
-
-    def _sync(self):
-        if str(self.device) != "cpu":
-            self.torch.cuda.current_stream().synchronize()
-
-    def begin(self):
-        """Integrator::run: clears the film; this rank's first iteration is `rank`."""
-        self.g.run(self.rank)
-
-    def enqueue(self, iterations=1):
-        self.g.enqueue(iterations)
-
-    def wait(self):
-        self.g.wait()
-
-    def reduce_film(self, layer=S.FILM_RESULT):
-        """Mean over all iterations finished so far, on rank 0 (a float4 [pixels, 4] tensor); None elsewhere.
-        Camera / Light layers are linear in the per-rank means; Result = max(0, camera + light) is reduced as the sum of those two."""
-        torch, dist = self.torch, self.dist
-        # both layers come back in the group's ONE combine buffer, filled on a lane's (non-blocking) stream: each copy must have finished on
-        # torch's stream before the next combine may overwrite the buffer
-        ptr, nbytes, done_cam = self.g.combined(S.FILM_CAMERA)
-        cam = self.view(ptr, nbytes).clone()
-        self._sync()
-        ptr, nbytes, done = self.g.combined(S.FILM_LIGHT)
-        light = self.view(ptr, nbytes).clone()
-        self._sync()
-        done = min(done, done_cam)
-        counts = torch.tensor([float(done)], dtype=torch.float64, device=self.device)
-        dist.all_reduce(counts, op=dist.ReduceOp.SUM)
-        total = float(counts.item())
-        weight = (done / total) if total > 0 else 0.0
-        if layer == S.FILM_CAMERA:
-            t = cam * weight
-        elif layer == S.FILM_LIGHT:
-            t = light * weight
-        else:
-            t = (cam + light) * weight
-        dist.reduce(t, dst=0, op=dist.ReduceOp.SUM)
-        if self.rank != 0:
-            return None
-        t = t.view(-1, 4)
-        if layer == S.FILM_RESULT:
-            t = torch.clamp_min(t, 0.0)  # Film::layer(Result) (film.cxx:381-418): max(0, camera + light)
-        t[:, 3] = 1.0
-        return t

@@ -9,8 +9,8 @@
  *
  * Conventions: plain C, no C++/torch types; all functions return 0 on success or a negative etxb_error;
  * the caller owns every host buffer it passes, the module owns all device memory; one context drives one
- * CUDA device (one process per GPU; multi-GPU sharding is expressed with etxb_set_partition + the
- * exchange buffers below, the collective itself is issued by the host with NCCL).
+ * CUDA device (one process per GPU; for multi-GPU runs the module issues the NCCL collectives itself, the
+ * host only distributes the communicator ids: see etxb_comm_init and etxb_group_comm_init below).
  *
  * The scene is passed in the reference's OWN in-memory layout (struct etx::Scene, 528 B, and
  * struct etx::Camera, 176 B — sources/etx/render/shared/scene.hxx:22-65, camera.hxx:8-39), so the
@@ -274,7 +274,7 @@ enum {
   ETXB_FILM_DENOISED = 7
 };
 
-/* Named device buffers for etxb_read_buffer / etxb_device_pointer (parity tests + multi-GPU exchange). */
+/* Named device buffers for etxb_read_buffer (parity tests). */
 enum {
   ETXB_BUF_LIGHT_PATH_COUNT = 0,   /* uint32[N]  vertices stored per light path (VCMLightPath::count) */
   ETXB_BUF_LIGHT_PATH_OFFSET = 1,  /* uint32[N]  first vertex of the path in the pool (VCMLightPath::index) */
@@ -284,10 +284,10 @@ enum {
   ETXB_BUF_LV_POS = 5,             /* float[3*P] light vertex positions, path-major order */
   ETXB_BUF_LV_THROUGHPUT = 6,      /* float[3*P] */
   ETXB_BUF_LV_MIS = 7,             /* float[3*P] d_vcm, d_vc, d_vm */
-  ETXB_BUF_FILM_LIGHT_ITERATION = 8, /* float4[N] per-iteration light splats (all-reduced across ranks) */
+  ETXB_BUF_FILM_LIGHT_ITERATION = 8, /* float4[N] per-iteration light splats (summed over the ranks of a pixel-tile run) */
   ETXB_BUF_FILM_CAMERA = 9,        /* float4[N] */
   ETXB_BUF_FILM_LIGHT = 10,        /* float4[N] */
-  ETXB_BUF_PHOTON_RECORDS = 11,    /* packed photon records of this rank (all-gathered across ranks) */
+  ETXB_BUF_PHOTON_RECORDS = 11,    /* packed photon records of this context's last light pass, path-major, 96 B each */
   ETXB_BUF_CAMERA_GATHERED = 12,   /* float[3*N] last iteration's camera contribution per path */
   ETXB_BUF_PIXEL_INFO = 13,        /* uint32[N]  Film's InternalData in film storage order (film.cxx:27-32): sample_count bits 0-29, converged bit 30, tmp bit 31 */
   ETXB_BUF_PIXEL_ERROR = 14,       /* float[N]   InternalData::error_level */
@@ -356,14 +356,9 @@ void etxb_options_default(etxb_vcm_options* opt);
 int etxb_options_set_key(etxb_vcm_options* opt, const char* key, double value);
 int etxb_set_options(etxb_ctx* ctx, const etxb_vcm_options* opt);
 
-/* Pixel-tile sharding across ranks (one process per GPU): rank r owns 32x32 tiles with (tile % world) == r.
+/* The pixel-tile rule without a communicator: this context renders only the 32x32 tiles with (tile % world) == rank, on one GPU.
  * world == 1 (default) renders the full frame. */
 int etxb_set_partition(etxb_ctx* ctx, uint32_t rank, uint32_t world);
-
-/* Iteration-interleaved multi-GPU runs: this context renders iterations first_iteration, first_iteration + stride, ...
- * (VCMIteration::iteration drives the merge radius, vcm_cpu.cxx:95-113, and the per-path sampler seeds, vcm_shared.hxx:286-300),
- * and its film is the mean over the iterations it rendered.  Default stride 1 = the reference's sequence. */
-int etxb_set_iteration_stride(etxb_ctx* ctx, uint32_t stride);
 
 /* Externally driven iteration index: the next enqueued iteration renders VCMIteration::iteration = `iteration`; the index no
  * longer advances by itself (used by etxb_group below). */
@@ -476,10 +471,6 @@ int etxb_set_scene_settings(etxb_ctx* ctx, float noise_threshold, float radiance
  * gather_camera_vertices + complete_camera_vertices (vcm_cpu.cxx:95-241).  Asynchronous: returns after
  * the work is queued on the context's stream. */
 int etxb_enqueue_iteration(etxb_ctx* ctx);
-/* The same iteration in three phases for multi-GPU runs (exchange photons / light image in between). */
-int etxb_enqueue_light_pass(etxb_ctx* ctx);
-int etxb_enqueue_grid_build(etxb_ctx* ctx, const void* device_photon_records, uint64_t photon_count);
-int etxb_enqueue_camera_pass(etxb_ctx* ctx);
 
 /* CPUVCM::update (vcm_cpu.cxx:264-276): non-blocking; fills status. */
 int etxb_poll(etxb_ctx* ctx, etxb_status* status);
@@ -502,9 +493,8 @@ int etxb_get_counters(etxb_ctx* ctx, etxb_counters* out);
 /* Per-kernel device time of the last iteration (CUDA events): names[i] -> ms[i]; returns count. */
 int etxb_get_kernel_times(etxb_ctx* ctx, const char** names, float* ms, uint32_t* launches, uint32_t capacity);
 
-/* Introspection for parity tests and NCCL exchange. */
+/* Introspection for parity tests. */
 int etxb_read_buffer(etxb_ctx* ctx, uint32_t buffer_id, void* dst, uint64_t dst_bytes, uint64_t* out_bytes);
-int etxb_device_pointer(etxb_ctx* ctx, uint32_t buffer_id, void** out_ptr, uint64_t* out_bytes);
 void* etxb_stream(etxb_ctx* ctx); /* cudaStream_t the module launches on */
 
 /* Unit entry points used by the parity tests (same kernels the iteration uses). */
@@ -692,14 +682,10 @@ int etxb_group_set_film_pixel_size(etxb_group* group, uint32_t size);
  * updates each lane, then etxb_group_begin(group, 0).  `info` is lane 0's, with `kept` the bits every lane kept.  ETXB_ERR_UNSUPPORTED on
  * a group with communicators (etxb_group_comm_init, etxb_group_comm_init_replicas). */
 int etxb_group_update_scene(etxb_group* group, const void* scene, uint64_t scene_bytes, const void* camera, uint64_t camera_bytes, etxb_update_info* info);
-int etxb_group_set_stride(etxb_group* group, uint32_t stride);       /* the k-th iteration handed out renders index first + k * stride
-                                                                        (iteration-interleaved multi-GPU runs: first = rank, stride = ranks) */
 int etxb_group_enqueue(etxb_group* group, uint32_t iterations);      /* asynchronous: queues `iterations` more iterations */
 int etxb_group_wait(etxb_group* group);                              /* blocks until the queue has drained; returns the first error */
 int etxb_group_poll(etxb_group* group, etxb_status* status);         /* completed = sum over lanes; total_time = wall time with work in flight */
 int etxb_group_read_film(etxb_group* group, uint32_t layer, float* dst_rgba, uint64_t dst_bytes);
-/* The same combined layer left on the device (float4[N]) + the number of iterations behind it: what a multi-GPU host reduces. */
-int etxb_group_combine(etxb_group* group, uint32_t layer, void** device_ptr, uint64_t* bytes, uint32_t* completed_iterations);
 
 /* ---- pixel-tile sharding over several GPUs (one process per GPU, NCCL over NVLink) ----------------------------------------
  * The reference renders one frame with one thread pool (vcm_cpu.cxx:115-241).  Here rank r owns the 32x32 pixel tiles with tile % world == r

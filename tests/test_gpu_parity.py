@@ -188,7 +188,8 @@ def test_full_size_properties_config2(api):
 
 def test_pixel_tile_partition_is_exact_without_merging(api):
     """Two ranks' tiles = the full frame: camera subpaths only touch their paired light path (vcm_shared.hxx:771)."""
-    sd = scenes.cornell_box(96, 80, **C1)
+    W, H = 96, 80
+    sd = scenes.cornell_box(W, H, **C1)
     imgs = []
     for rank, world in ((0, 1), (0, 2), (1, 2)):
         g = api.GPUVCM(sd, flavor="parity")
@@ -200,6 +201,12 @@ def test_pixel_tile_partition_is_exact_without_merging(api):
     full, r0, r1 = imgs
     assert bit_equal(r0[0] + r1[0], full[0])  # disjoint pixels: one of the two is exactly zero everywhere
     assert rel_l2(r0[1] + r1[1], full[1]) < 1e-6  # light splats land anywhere: summed like the NCCL all-reduce does
+    # path (x, y) lies in tile (y // 32) * ceil(W / 32) + x // 32 and rank r renders the tiles with tile % 2 == r; the Camera layer is
+    # stored y-flipped (film.cxx:189), so film row H - 1 - y holds path row y
+    ys, xs = np.mgrid[0:H, 0:W]
+    owner = (((H - 1 - ys) // 32) * ((W + 31) // 32) + xs // 32) % 2
+    for rank, (camera, _) in enumerate((r0, r1)):
+        assert (camera.view(np.uint32)[owner != rank] == 0).all(), f"rank {rank} wrote camera pixels outside its tiles"
 
 
 @pytest.mark.parametrize("spectral", [False, True])

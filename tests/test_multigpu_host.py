@@ -1,201 +1,18 @@
-"""World-size-2 run of the multi-GPU exchange logic (etx_tracer_b200/multigpu.py) on CPU tensors over gloo.
-
-The CUDA module is replaced by a stand-in with the same pass / buffer surface, so what is tested is the host side of SURVEY.md §8(e):
-tile ownership, the all-reduce of the per-iteration light image, the rank-major layout of the gathered photon records (block sizes
-differ per rank) and the final reduce of the disjoint camera tiles."""
-import ctypes
+"""World-size-2 run of the host's part in the module's multi-GPU path (etx_tracer_b200/multigpu.py) on CPU tensors over gloo."""
 import os
 import socket
 
 import numpy as np
-import pytest
-import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-from etx_tracer_b200 import multigpu, structs as S
-
-W, H = 96, 64
-REC_FLOATS = multigpu.RECORD_BYTES // 4
-
-
-class StandInGPU:
-    """Mimics api.GPUVCM for ShardedVCM: buffers are CPU tensors, 'device pointers' are buffer ids."""
-
-    def __init__(self, rank, world, merging=True):
-        self.rank, self.world = rank, world
-        self.options = np.zeros(1, dtype=S.VCM_OPTIONS)
-        self.options["options"] = S.VCM_FULL if merging else S.VCM_CONNECT_ONLY
-        self.owner = multigpu.tile_owner(W, H, world)
-        self.partition = None
-        self.t = {}
-        self.received = None
-        self.calls = []
-
-    def set_partition(self, rank, world):
-        self.partition = (rank, world)
-
-    def light_pass(self):
-        self.calls.append("light")
-        light = torch.zeros(H * W * 4, dtype=torch.float32)
-        light.view(H, W, 4)[..., 0] = float(self.rank + 1)  # splats land anywhere: every rank contributes to every pixel
-        self.t[S.BUF_FILM_LIGHT_ITERATION] = light
-        count = 3 + 2 * self.rank
-        rec = torch.arange(count * REC_FLOATS, dtype=torch.float32) + 1000.0 * self.rank
-        self.t[S.BUF_PHOTON_RECORDS] = rec
-
-    def device_pointer(self, buf):
-        return buf, self.t[buf].numel() * 4
-
-    def view(self, ptr, nbytes, dtype="<f4"):
-        return self.t[ptr][:nbytes // 4]
-
-    def grid_build(self, records_ptr, total):
-        self.calls.append("grid")
-        if records_ptr is None:
-            self.received = None
-            return
-        arr = (ctypes.c_float * (total * REC_FLOATS)).from_address(records_ptr)
-        self.received = np.frombuffer(arr, dtype=np.float32).copy()
-
-    def camera_pass(self):
-        self.calls.append("camera")
-        cam = torch.zeros(H, W, 4, dtype=torch.float32)
-        mine = torch.from_numpy(self.owner == self.rank)
-        ys, xs = np.mgrid[0:H, 0:W]
-        cam[..., 0] = torch.from_numpy((ys * W + xs).astype(np.float32)) * mine
-        cam[..., 3] = mine.float()
-        self.t[S.BUF_FILM_CAMERA] = cam.reshape(-1)
-
-    def film(self, layer):
-        return self.t[S.BUF_FILM_CAMERA].view(H, W, 4).numpy()
-
-
-def _worker(rank, world, port, merging, out_dir):
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    try:
-        g = StandInGPU(rank, world, merging)
-        sh = multigpu.ShardedVCM(g, dist, rank, world, device="cpu", view=g.view)
-        sh.iterate()
-        film = sh.reduce_film()
-        np.savez(os.path.join(out_dir, f"rank{rank}.npz"), light=g.t[S.BUF_FILM_LIGHT_ITERATION].numpy(),
-                 received=np.zeros(0, np.float32) if g.received is None else g.received,
-                 got_records=np.array([g.received is not None]), film=np.zeros(0) if film is None else film,
-                 calls=np.array(g.calls), partition=np.array(g.partition))
-    finally:
-        dist.destroy_process_group()
+from etx_tracer_b200 import multigpu
 
 
 def _free_port():
     with socket.socket() as s:
         s.bind(("127.0.0.1", 0))
         return s.getsockname()[1]
-
-
-@pytest.mark.parametrize("merging", [True, False])
-def test_sharded_iteration_over_gloo(tmp_path, merging):
-    world = 2
-    mp.spawn(_worker, args=(world, _free_port(), merging, str(tmp_path)), nprocs=world, join=True)
-    r = [np.load(tmp_path / f"rank{k}.npz") for k in range(world)]
-    for k in range(world):
-        assert list(r[k]["calls"]) == ["light", "grid", "camera"]
-        assert tuple(r[k]["partition"]) == (k, world)
-        # light image: sum over ranks everywhere
-        light = r[k]["light"].reshape(H, W, 4)
-        assert (light[..., 0] == 3.0).all() and (light[..., 1:] == 0.0).all()
-        if merging:
-            # photon records: rank-major, rank 0's 3 records then rank 1's 5, each block intact
-            expect = np.concatenate([np.arange(3 * REC_FLOATS, dtype=np.float32), np.arange(5 * REC_FLOATS, dtype=np.float32) + 1000.0])
-            assert bool(r[k]["got_records"][0]) and np.array_equal(r[k]["received"], expect)
-        else:
-            assert not bool(r[k]["got_records"][0])  # no exchange when merging is off
-    # camera film: the disjoint tiles of both ranks add up to the full image on rank 0 only
-    film = r[0]["film"]
-    ys, xs = np.mgrid[0:H, 0:W]
-    assert np.array_equal(film[..., 0], (ys * W + xs).astype(np.float32)) and (film[..., 3] == 1.0).all()
-    assert r[1]["film"].size == 0
-
-
-def test_tile_owner_is_a_partition():
-    for world in (1, 2, 3, 4, 8):
-        owner = multigpu.tile_owner(W, H, world)
-        assert owner.min() == 0 and owner.max() == min(world, (W // 32) * (H // 32)) - 1
-        # whole 32x32 tiles, dealt round-robin in row-major tile order
-        assert (owner[:32, :32] == 0).all() and (owner[:32, 32:64] == 1 % world).all()
-        counts = np.bincount(owner.ravel(), minlength=world)
-        assert counts.sum() == W * H and counts.max() - counts.min() <= 32 * 32
-
-
-def test_gather_layout():
-    assert multigpu.gather_layout([3, 0, 5]) == ([0, 3, 3], 8)
-    assert multigpu.gather_layout([0]) == ([0], 0)
-
-
-class StandInGroup:
-    """api.GPUVCMGroup stand-in for InterleavedVCM: iteration k contributes the constant k to the camera layer and 10 k to the light
-    layer; the layers are means over the iterations this group rendered."""
-
-    def __init__(self):
-        self.stride, self.first, self.rendered = 1, 0, []
-
-    def set_stride(self, stride):
-        self.stride = stride
-
-    def run(self, first_iteration=0):
-        self.first, self.rendered = first_iteration, []
-
-    def enqueue(self, iterations=1):
-        for _ in range(iterations):
-            self.rendered.append(self.first + len(self.rendered) * self.stride)
-
-    def wait(self):
-        pass
-
-    def combined(self, layer):
-        mean = float(np.mean(self.rendered)) if self.rendered else 0.0
-        value = {S.FILM_CAMERA: mean, S.FILM_LIGHT: 10.0 * mean}[layer]
-        self.t = torch.full((H * W * 4,), value, dtype=torch.float32)
-        return "combined", self.t.numel() * 4, len(self.rendered)
-
-    def view(self, ptr, nbytes, dtype="<f4"):
-        return self.t[:nbytes // 4]
-
-
-def _interleaved_worker(rank, world, port, per_rank, out_dir):
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    try:
-        g = StandInGroup()
-        iv = multigpu.InterleavedVCM(g, dist, rank, world, device="cpu", view=g.view)
-        iv.begin()
-        iv.enqueue(2)                   # warm-up block
-        iv.enqueue(per_rank[rank] - 2)  # timed block: the rank's sequence keeps running
-        iv.wait()
-        film = iv.reduce_film()
-        np.savez(os.path.join(out_dir, f"rank{rank}.npz"), rendered=np.array(g.rendered), film=np.zeros(0) if film is None else film.numpy())
-    finally:
-        dist.destroy_process_group()
-
-
-@pytest.mark.parametrize("per_rank", [(4, 4), (5, 3)])
-def test_interleaved_iterations_over_gloo(tmp_path, per_rank):
-    """Rank r renders indices r, r + N, ...; the reduced film is the mean over every iteration rendered anywhere, weighted by how many
-    each rank finished (rank 0 only)."""
-    world = 2
-    mp.spawn(_interleaved_worker, args=(world, _free_port(), per_rank, str(tmp_path)), nprocs=world, join=True)
-    r = [np.load(tmp_path / f"rank{k}.npz") for k in range(world)]
-    for k in range(world):
-        assert r[k]["rendered"].tolist() == [k + j * world for j in range(per_rank[k])]
-    everything = np.concatenate([r[0]["rendered"], r[1]["rendered"]])
-    assert len(set(everything.tolist())) == len(everything)
-    mean = float(everything.mean())
-    film = r[0]["film"]
-    assert film.shape == (H * W, 4) and r[1]["film"].size == 0
-    np.testing.assert_allclose(film[:, 0], mean + 10.0 * mean, rtol=1e-6)
-    assert (film[:, 3] == 1.0).all()
 
 
 def _ids_worker(rank, world, port, out_dir):
