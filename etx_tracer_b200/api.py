@@ -129,6 +129,7 @@ def load_library(flavor="fast"):
     lib.etxb_debug_closure_eval.argtypes = [vp, vp, u32, u32, vp]
     lib.etxb_debug_bsdf_sample.argtypes = [vp, vp, u32, u32, vp]
     lib.etxb_debug_emitter.argtypes = [vp, vp, u32, u32, vp]
+    lib.etxb_debug_medium.argtypes = [vp, vp, u32, u32, vp]
     lib.etxb_debug_set_thresholds.argtypes = [vp, vp]
     lib.etxb_debug_get_branch_counts.argtypes = [vp, vp]
     lib.etxb_debug_merge.argtypes = [vp, vp, u32, vp, vp, u32, vp, vp]
@@ -576,6 +577,14 @@ class GPUVCM:
         queries = np.ascontiguousarray(queries, dtype=S.EMITTER_QUERY)
         out = np.zeros((queries.shape[0], int(repetitions)), dtype=S.EMITTER_RESULT)
         self._check(self.lib.etxb_debug_emitter(self.h, _p(queries), queries.shape[0], int(repetitions), _p(out)))
+        return out
+
+    def debug_medium(self, queries, repetitions=1):
+        """The media routines for S.MEDIUM_QUERY records on the uploaded scene, repetition r of each query on the sampler (seed, r); returns
+        S.MEDIUM_RESULT records shaped (n, repetitions), laid out as etxb_debug_medium documents (include/etx_b200.h)."""
+        queries = np.ascontiguousarray(queries, dtype=S.MEDIUM_QUERY)
+        out = np.zeros((queries.shape[0], int(repetitions)), dtype=S.MEDIUM_RESULT)
+        self._check(self.lib.etxb_debug_medium(self.h, _p(queries), queries.shape[0], int(repetitions), _p(out)))
         return out
 
     def debug_thresholds(self, **fields):

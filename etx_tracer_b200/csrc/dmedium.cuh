@@ -55,8 +55,12 @@ DEV bool medium_intersects_bounds(const DMedium& medium, V3 in_pos, V3 in_direct
   V3 end_pos = in_pos + in_direction * in_max_t;
   V3 medium_end_pos = bounds_to_local(medium, end_pos);
   medium_pos = bounds_to_local(medium, in_pos);
-  medium_dir = normalize(medium_end_pos - medium_pos);
-  float segment = length(medium_end_pos - medium_pos);
+  // __fsub_rn: the product build would otherwise contract the difference of the two local points with one of their products into an FMA,
+  // and a component along which the ray does not move would keep that product's rounding error (~1e-8) instead of being exactly 0 --
+  // the slab of a ray parallel to a face then ends at t = 0 instead of being skipped as 0 / 0.  Without -fmad this is the plain difference.
+  const V3 delta = {__fsub_rn(medium_end_pos.x, medium_pos.x), __fsub_rn(medium_end_pos.y, medium_pos.y), __fsub_rn(medium_end_pos.z, medium_pos.z)};
+  medium_dir = normalize(delta);
+  float segment = length(delta);
   return medium_bounds(medium_pos, medium_dir, segment, t_min, t_max);
 }
 

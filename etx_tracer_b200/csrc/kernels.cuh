@@ -1877,6 +1877,52 @@ __global__ void k_debug_emitter(const __grid_constant__ DeviceScene sc, const et
   out[t] = o;
 }
 
+// one thread per (etxb_medium_query, repetition): the media routines of dmedium.cuh and the shadow-ray walk of dtrace.cuh as the passes
+// call them; ops and record layout in include/etx_b200.h
+static_assert(sizeof(etxb_medium_query) == 96u && sizeof(etxb_medium_result) == 64u, "etxb_medium_query / etxb_medium_result layout");
+template <bool SP>
+__global__ void k_debug_medium(const __grid_constant__ DeviceScene sc, const etxb_medium_query* queries, uint32_t count, uint32_t reps, etxb_medium_result* out) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= count * reps) return;
+  const uint32_t i = t / reps, r = t % reps;
+  const etxb_medium_query& q = queries[i];
+  const float wavelength = SP ? q.wavelength : -1.0f;
+  const V3 origin = {q.origin[0], q.origin[1], q.origin[2]}, direction = {q.direction[0], q.direction[1], q.direction[2]};
+  const auto put = [](float* dst, V3 a) {
+    dst[0] = a.x;
+    dst[1] = a.y;
+    dst[2] = a.z;
+  };
+  etxb_medium_result o = {};
+  Smp smp;
+  smp.init(q.seed, r);
+  o.seed_start = smp.seed;
+  if (q.op == ETXB_MEDIUM_BOUNDS) {
+    V3 pos = origin, dir = direction;
+    o.flag = medium_intersects_bounds(sc.mediums[q.medium], origin, direction, q.max_t, pos, dir, o.t_min, o.t_max) ? 1u : 0u;
+    put(o.pos, pos);
+    put(o.dir, dir);
+  } else if (q.op == ETXB_MEDIUM_DENSITY) {
+    o.value[0] = medium_sample_density(sc.mediums[q.medium], origin);
+  } else if (q.op == ETXB_MEDIUM_TRANSMITTANCE) {
+    put(o.value, medium_transmittance<SP>(sc, sc.mediums[q.medium], wavelength, smp, origin, direction, q.max_t).as_v3());
+  } else if (q.op == ETXB_MEDIUM_SAMPLE) {
+    const Spec<SP> throughput = Spec<SP>::make3({q.throughput[0], q.throughput[1], q.throughput[2]});
+    const MediumSample<SP> s = sample_medium<SP>(sc, sc.mediums[q.medium], wavelength, throughput, smp, origin, direction, q.max_t);
+    put(o.value, s.weight.as_v3());
+    put(o.pos, s.pos);
+    o.t = s.sampled_medium_t;
+  } else if (q.op == ETXB_MEDIUM_PHASE) {
+    o.value[0] = phase_function(direction, {q.w_o[0], q.w_o[1], q.w_o[2]}, q.g);
+    put(o.dir, sample_phase_function(direction, q.g, {q.rnd[0], q.rnd[1]}));
+  } else {
+    STATS_DECL;  // as every other caller: the count build's trace_transmittance is compiled for a non-null stats pointer
+    put(o.value, trace_transmittance<SP, false>(sc, wavelength, origin, {q.end[0], q.end[1], q.end[2]}, q.medium, smp, stats).as_v3());
+  }
+  o.seed_end = smp.seed;
+  out[t] = o;
+}
+
 // etxb_debug_merge: query i becomes path i of a one-bounce queue, staged in the columns the gather kernels read (hit record, ray
 // direction, throughput, MIS terms, sampler, depth, medium, wavelength), with the merge key k_camera_shade would give it.  Writes the
 // staged camera vertex's position and normal to pos_nrm[2 i], [2 i + 1], and i to queue slot i.

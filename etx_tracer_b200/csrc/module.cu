@@ -2848,6 +2848,110 @@ int etxb_debug_emitter(etxb_ctx* ctx, const etxb_emitter_query* queries, uint32_
   return ETXB_OK;
 }
 
+// Test hook: the media routines of dmedium.cuh and the shadow-ray walk of dtrace.cuh, query by query and repetition by repetition (layout
+// and ops in include/etx_b200.h).  Every query is checked before the launch against what makes those loops end: a finite local segment,
+// tracking steps that still advance t in float32, and a free-flight redraw loop that ends in a few thousand draws on average.
+namespace {
+constexpr double kMediumCoordMax = 1e15;       // |world coordinate| of an origin or an end point
+constexpr double kMediumLocalSegmentMax = 1e18;  // local segment length: its float32 square stays finite
+constexpr double kMediumTrackingMax = 65536.0;   // max_sigma x (|local origin| + 2): a mean tracking step of ~1000 float32 ulps of t or more
+constexpr double kMediumRedrawMax = 8.0;         // extinction x kRayEpsilon: the homogeneous redraw loop runs exp(8) ~ 3000 times on average
+
+// A heterogeneous medium's tracking from a to b (world points; b = nullptr: a only) ends: finite local points, a local segment whose
+// float32 length is finite, and steps of 1 / max_sigma well above an ulp of the local t.
+bool tracking_bounded(const DMedium& m, const double* a, const double* b) {
+  if ((m.cls != 1u) || !(m.max_sigma > 0.0f)) return true;
+  const double lo[3] = {m.bounds_min.x, m.bounds_min.y, m.bounds_min.z}, hi[3] = {m.bounds_max.x, m.bounds_max.y, m.bounds_max.z};
+  double magnitude = 0.0, length2 = 0.0;
+  for (int k = 0; k < 3; ++k) {
+    const double ext = hi[k] - lo[k];
+    if (!(ext > 0.0)) return false;
+    const double pa = (a[k] - lo[k]) / ext, pb = b ? (b[k] - lo[k]) / ext : pa;
+    if (!std::isfinite(pa) || !std::isfinite(pb)) return false;
+    magnitude = std::max(magnitude, std::fabs(pa));
+    length2 += (pb - pa) * (pb - pa);
+  }
+  return (std::sqrt(length2) <= kMediumLocalSegmentMax) && (double(m.max_sigma) * (magnitude + 2.0) <= kMediumTrackingMax);
+}
+
+double spectrum_max(const std::vector<DSpectrum>& spectra, uint32_t index) {
+  if (index >= spectra.size()) return 0.0;
+  const DSpectrum& s = spectra[index];
+  double v = std::max({double(s.rgb[0]), double(s.rgb[1]), double(s.rgb[2])});
+  for (float p : s.power) v = std::max(v, double(p));
+  return v;
+}
+}  // namespace
+
+int etxb_debug_medium(etxb_ctx* ctx, const etxb_medium_query* queries, uint32_t count, uint32_t repetitions, etxb_medium_result* out) {
+  if (!ctx || !queries || !out || (repetitions == 0)) return ETXB_ERR_INVALID_ARGUMENT;
+  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
+  if (count == 0) return ETXB_OK;
+  if (uint64_t(count) * repetitions > 0x7fffffffull) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "%u queries x %u repetitions exceed 2^31 samples", count, repetitions);
+  cudaSetDevice(ctx->device);
+  std::vector<DMedium> meds(ctx->mediums.count);
+  std::vector<DSpectrum> spectra(ctx->spectra.count);
+  if (!meds.empty()) CUDA_OK(ctx, cudaMemcpy(meds.data(), ctx->mediums.ptr, meds.size() * sizeof(DMedium), cudaMemcpyDeviceToHost));
+  if (!spectra.empty()) CUDA_OK(ctx, cudaMemcpy(spectra.data(), ctx->spectra.ptr, spectra.size() * sizeof(DSpectrum), cudaMemcpyDeviceToHost));
+  const auto bounded3 = [](const float* v) {
+    return (std::fabs(double(v[0])) <= kMediumCoordMax) && (std::fabs(double(v[1])) <= kMediumCoordMax) && (std::fabs(double(v[2])) <= kMediumCoordMax);
+  };
+  for (uint32_t i = 0; i < count; ++i) {
+    const etxb_medium_query& q = queries[i];
+    if (q.op > ETXB_MEDIUM_SEGMENT) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: op must be 0 to 5", i);
+    if (ctx->spectral && !std::isfinite(q.wavelength)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: non-finite wavelength", i);
+    const bool unset = (q.op == ETXB_MEDIUM_SEGMENT) && (q.medium == ETXB_INVALID_INDEX);
+    if ((q.op != ETXB_MEDIUM_PHASE) && !unset && (q.medium >= meds.size())) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: medium index out of range", i);
+    if ((q.op == ETXB_MEDIUM_DENSITY) && (ctx->medium_density[q.medium].count == 0)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: density of a homogeneous medium", i);
+    if ((q.op != ETXB_MEDIUM_PHASE) && !bounded3(q.origin)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: origin not finite or past 1e15", i);
+    const double o[3] = {q.origin[0], q.origin[1], q.origin[2]};
+    if (q.op == ETXB_MEDIUM_SEGMENT) {
+      if (!bounded3(q.end)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: segment end not finite or past 1e15", i);
+      // every medium the walk can track through starts from a point of the segment: bound both ends in each heterogeneous medium
+      const double e[3] = {q.end[0], q.end[1], q.end[2]};
+      for (const DMedium& m : meds) {
+        if (!tracking_bounded(m, o, e) || !tracking_bounded(m, e, o)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: segment too far from a heterogeneous medium to track", i);
+      }
+      continue;
+    }
+    if (q.op == ETXB_MEDIUM_DENSITY) continue;
+    const float* d = q.direction;
+    if (!std::isfinite(d[0]) || !std::isfinite(d[1]) || !std::isfinite(d[2]) || ((d[0] == 0.0f) && (d[1] == 0.0f) && (d[2] == 0.0f)))
+      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: zero or non-finite direction", i);
+    if (q.op == ETXB_MEDIUM_PHASE) continue;
+    if (!std::isfinite(q.max_t) && (q.max_t != kMaxFloat)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: non-finite max_t", i);
+    if ((q.op == ETXB_MEDIUM_SAMPLE) && !(q.max_t >= kRayEpsilon)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: sample needs max_t >= kRayEpsilon", i);
+    if (!std::isfinite(q.throughput[0]) || !std::isfinite(q.throughput[1]) || !std::isfinite(q.throughput[2]))
+      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: non-finite throughput", i);
+    const DMedium& m = meds[q.medium];
+    if (q.max_t < kMaxFloat) {  // medium_intersects_bounds refuses max_t = kMaxFloat before any arithmetic
+      double e[3];
+      for (int k = 0; k < 3; ++k) e[k] = o[k] + double(d[k]) * double(q.max_t);
+      if (!(std::fabs(e[0]) <= 1e30) || !(std::fabs(e[1]) <= 1e30) || !(std::fabs(e[2]) <= 1e30))
+        return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: the segment's end overflows", i);
+      if (!tracking_bounded(m, o, e)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: segment too long or too far from the medium to track", i);
+    }
+    if ((q.op == ETXB_MEDIUM_SAMPLE) && (m.cls == 0u) &&
+        ((spectrum_max(spectra, m.absorption_index) + spectrum_max(spectra, m.scattering_index)) * kRayEpsilon > kMediumRedrawMax))
+      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: extinction too high for the free-flight redraw loop", i);
+  }
+  const uint32_t total = count * repetitions;
+  DevBuf<etxb_medium_query> d_queries;
+  DevBuf<etxb_medium_result> d_out;
+  if (int rc = upload(ctx, d_queries, queries, count)) return rc;
+  CUDA_OK(ctx, d_out.alloc(total));
+  if (ctx->spectral) {
+    k_debug_medium<true><<<blocks_for(total, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
+  } else {
+    k_debug_medium<false><<<blocks_for(total, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
+  }
+  ctx->kernel_launches += 1;
+  CUDA_OK(ctx, cudaGetLastError());
+  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+  CUDA_OK(ctx, cudaMemcpy(out, d_out.ptr, d_out.bytes(), cudaMemcpyDeviceToHost));
+  return ETXB_OK;
+}
+
 // Test hook: the queue sizes from which the passes take their large-queue branches (NULL = the defaults), and what ran since etxb_begin
 int etxb_debug_set_thresholds(etxb_ctx* ctx, const etxb_debug_thresholds* thresholds) {
   if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;

@@ -128,6 +128,12 @@ EMITTER_RESULT = np.dtype([("value", f4, 3), ("origin", f4, 3), ("normal", f4, 3
                            ("medium_index", u4), ("flags", u4), ("seed_start", u4), ("seed_end", u4), ("reserved", u4)])
 EMITTER_SELECT, EMITTER_SAMPLE_IN, EMITTER_EMISSION, EMITTER_RADIANCE = 0, 1, 2, 3
 EMITTER_FLAG_DELTA, EMITTER_FLAG_DISTANT = 1, 2
+# etxb_medium_query (96 B) and the per-sample record etxb_debug_medium / oracle_medium return (include/etx_b200.h)
+MEDIUM_QUERY = np.dtype([("op", u4), ("medium", u4), ("seed", u4), ("reserved0", u4), ("wavelength", f4), ("origin", f4, 3), ("direction", f4, 3),
+                         ("max_t", f4), ("end", f4, 3), ("throughput", f4, 3), ("g", f4), ("rnd", f4, 2), ("w_o", f4, 3)])
+MEDIUM_RESULT = np.dtype([("value", f4, 3), ("pos", f4, 3), ("dir", f4, 3), ("t_min", f4), ("t_max", f4), ("t", f4), ("flag", u4),
+                          ("seed_start", u4), ("seed_end", u4), ("reserved", u4)])
+MEDIUM_BOUNDS, MEDIUM_DENSITY, MEDIUM_TRANSMITTANCE, MEDIUM_SAMPLE, MEDIUM_PHASE, MEDIUM_SEGMENT = 0, 1, 2, 3, 4, 5
 BSDF_DIFFUSE, BSDF_REFLECTION, BSDF_TRANSMISSION, BSDF_MEDIUM_CHANGED, BSDF_DELTA = 1, 2, 4, 8, 16
 # etxb_debug_thresholds / etxb_debug_branch_counts (include/etx_b200.h): a threshold of 0 always takes the large-queue branch, NEVER never does
 DEBUG_THRESHOLDS = np.dtype([("merge_sort_min_queries", u4), ("merge_min_warps_per_sm", u4), ("tail_queue", u4), ("sort_queue_min", u4), ("merge_qpw", u4)])
@@ -152,6 +158,7 @@ EXPECTED_SIZES = {
     "MEDIUM": (MEDIUM, 80), "CAMERA": (CAMERA, 176), "SCENE": (SCENE, 528), "CLOSURE_QUERY": (CLOSURE_QUERY, 96),
     "SAMPLE_QUERY": (SAMPLE_QUERY, 96), "SAMPLE_RESULT": (SAMPLE_RESULT, 48),
     "EMITTER_QUERY": (EMITTER_QUERY, 80), "EMITTER_RESULT": (EMITTER_RESULT, 104),
+    "MEDIUM_QUERY": (MEDIUM_QUERY, 96), "MEDIUM_RESULT": (MEDIUM_RESULT, 64),
     "LIGHT_VERTEX_REC": (LIGHT_VERTEX_REC, 96), "MERGE_QUERY": (MERGE_QUERY, 64), "MERGE_RESULT": (MERGE_RESULT, 48), "MERGE_GRID": (MERGE_GRID, 64),
 }
 for _name, (_dt, _size) in EXPECTED_SIZES.items():

@@ -607,6 +607,48 @@ typedef struct etxb_emitter_result {
   uint32_t emitter_index, triangle_index, medium_index, flags, seed_start, seed_end, reserved;
 } etxb_emitter_result;
 int etxb_debug_emitter(etxb_ctx* ctx, const etxb_emitter_query* queries, uint32_t count, uint32_t repetitions, etxb_emitter_result* out);
+/* Medium query (dmedium.cuh and trace_transmittance of dtrace.cuh, as the bounces and shadow rays call them) on the uploaded scene.  One
+ * query is 96 bytes: the op, a medium index, a sampler seed, the wavelength (ignored in RGB scenes), an origin, a direction, a distance
+ * max_t, an end point, a throughput (rgb; a spectral throughput is throughput[0]), a phase g, a 2-D random number and a second direction
+ * w_o.  The ops:
+ *   0 bounds         medium_intersects_bounds(medium, origin, direction, max_t): flag, pos / dir (the medium's local frame), t_min, t_max
+ *   1 density        medium_sample_density(medium, origin as a local coordinate): value[0]; the medium must be heterogeneous
+ *   2 transmittance  medium_transmittance(medium, origin, direction, max_t): value
+ *   3 sample         sample_medium(medium, throughput, origin, direction, max_t): value = weight, pos, t = sampled_medium_t;
+ *                    max_t must be at least kRayEpsilon (the homogeneous free-flight loop runs while t < kRayEpsilon)
+ *   4 phase          phase_function(direction, w_o, g): value[0]; sample_phase_function(direction, g, rnd): dir.  Ignores the medium.
+ *   5 segment        trace_transmittance<SP, false>(origin, end, medium) on the scene's BVH: value; medium 0xffffffff = no medium
+ * Every op runs on the sampler Smp::init(seed, r) of repetition r; ops 0, 1 and 4 draw nothing.  The hook refuses, before any launch, an
+ * op past 5, a medium index past the scene's count (except 0xffffffff for op 5; op 4 ignores it), a zero or non-finite direction
+ * (ops 0 to 4), a non-finite origin, end point, max_t, throughput or wavelength, coordinates past 1e15, heterogeneous tracking whose
+ * local segment would overflow or whose max_sigma x (|local origin| + 2) passes 2^16 (op 5: in every heterogeneous medium), a
+ * homogeneous sample whose extinction x kRayEpsilon passes 8, and count x repetitions past 2^31. */
+typedef struct etxb_medium_query {
+  uint32_t op, medium, seed, reserved0;
+  float wavelength;
+  float origin[3], direction[3];
+  float max_t;
+  float end[3];
+  float throughput[3];
+  float g;
+  float rnd[2];
+  float w_o[3];
+} etxb_medium_query;
+#define ETXB_MEDIUM_BOUNDS 0u
+#define ETXB_MEDIUM_DENSITY 1u
+#define ETXB_MEDIUM_TRANSMITTANCE 2u
+#define ETXB_MEDIUM_SAMPLE 3u
+#define ETXB_MEDIUM_PHASE 4u
+#define ETXB_MEDIUM_SEGMENT 5u
+/* One 64-byte record per (query, repetition), repetition-minor: value (rgb; a spectral value fills all three), pos, dir, t_min, t_max, t
+ * (sampled_medium_t), flag (op 0: 1 when the segment meets the bounds), and the sampler state Smp::init(seed, r) left and the state after
+ * the op, for every op.  Fields an op does not name are 0. */
+typedef struct etxb_medium_result {
+  float value[3], pos[3], dir[3];
+  float t_min, t_max, t;
+  uint32_t flag, seed_start, seed_end, reserved;
+} etxb_medium_result;
+int etxb_debug_medium(etxb_ctx* ctx, const etxb_medium_query* queries, uint32_t count, uint32_t repetitions, etxb_medium_result* out);
 /* Queue sizes from which the light and camera passes take their large-queue branches.  A pass of a long queue runs the same paths as
  * one of a short queue, in another order; these let a small film take either branch.  Each field is a queue size: 0 = always the
  * large-queue branch, 0xffffffff = never.

@@ -50,6 +50,8 @@ def load(flavor="parity"):
         lib.oracle_bsdf_sample.argtypes = [vp, vp, u32, u32, u32, vp]
     if hasattr(lib, "oracle_emitter"):
         lib.oracle_emitter.argtypes = [vp, vp, u32, u32, u32, vp]
+    if hasattr(lib, "oracle_medium"):
+        lib.oracle_medium.argtypes = [vp, vp, u32, u32, u32, vp]
     if hasattr(lib, "oracle_merge"):
         lib.oracle_merge.argtypes = [vp, vp, u32, vp, vp, u32, u32, u32, vp, vp]
     lib.oracle_sampler.argtypes = [vp, vp, u32, u32, vp, vp]
@@ -86,6 +88,11 @@ def has_bsdf_sample(flavor="parity"):
 def has_emitter(flavor="parity"):
     """Whether the built oracle exports oracle_emitter."""
     return hasattr(load(flavor), "oracle_emitter")
+
+
+def has_medium(flavor="parity"):
+    """Whether the built oracle exports oracle_medium."""
+    return hasattr(load(flavor), "oracle_medium")
 
 
 def has_merge(flavor="parity"):
@@ -279,6 +286,14 @@ class Oracle:
         queries = np.ascontiguousarray(queries, dtype=self.S.EMITTER_QUERY)
         out = np.zeros((queries.shape[0], int(repetitions)), dtype=self.S.EMITTER_RESULT)
         self.lib.oracle_emitter(self.h, _p(queries), queries.shape[0], int(repetitions), int(threads or os.cpu_count() or 1), _p(out))
+        return out
+
+    def medium(self, queries, repetitions=1, threads=None):
+        """The reference's media routines for S.MEDIUM_QUERY records, repetition r of each query on Sampler(seed, r); S.MEDIUM_RESULT records
+        shaped (n, repetitions), in the layout of GPUVCM.debug_medium."""
+        queries = np.ascontiguousarray(queries, dtype=self.S.MEDIUM_QUERY)
+        out = np.zeros((queries.shape[0], int(repetitions)), dtype=self.S.MEDIUM_RESULT)
+        self.lib.oracle_medium(self.h, _p(queries), queries.shape[0], int(repetitions), int(threads or os.cpu_count() or 1), _p(out))
         return out
 
     def merge(self, records, light_wavelengths, queries, repetitions=1, threads=None):

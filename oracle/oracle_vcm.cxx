@@ -1223,6 +1223,58 @@ void oracle_emitter(void* h, const etxb_emitter_query* queries, uint32_t count, 
   });
 }
 
+// The reference's own media routines (scene_medium.hxx, compiled in place: medium_intersects_bounds and medium_sample_density_internal lie
+// in its anonymous namespace, visible in this translation unit) for etxb_medium_query records (include/etx_b200.h), and for op 5
+// Raytracing::trace_transmittance above with Medium::Instance{.index = medium}.  One etxb_medium_result per (query, repetition r) on
+// Sampler(seed, r), as etxb_debug_medium writes them.  The caller keeps to the hook's checks (a valid index, max_t >= kRayEpsilon for op 3).
+static_assert(sizeof(etxb_medium_query) == 96);
+static_assert(sizeof(etxb_medium_result) == 64);
+void oracle_medium(void* h, const etxb_medium_query* queries, uint32_t count, uint32_t repetitions, uint32_t threads, etxb_medium_result* out) {
+  auto* o = static_cast<Oracle*>(h);
+  const Scene& scene = o->scene;
+  parallel_ranges(count * repetitions, threads, [&](uint32_t begin, uint32_t end, uint32_t, uint32_t) {
+    for (uint32_t t = begin; t < end; ++t) {
+      const etxb_medium_query& q = queries[t / repetitions];
+      const SpectralQuery spect = scene.spectral() ? SpectralQuery{q.wavelength, SpectralQuery::Spectral} : SpectralQuery::sample();
+      const float3 origin = {q.origin[0], q.origin[1], q.origin[2]}, direction = {q.direction[0], q.direction[1], q.direction[2]};
+      const auto put = [](float* d, const float3& a) {
+        d[0] = a.x;
+        d[1] = a.y;
+        d[2] = a.z;
+      };
+      const auto put_spectral = [&](float* d, const SpectralResponse& s) { put(d, s.spectral() ? float3{s.value, s.value, s.value} : s.integrated); };
+      etxb_medium_result dst = {};
+      Sampler smp(q.seed, t % repetitions);
+      dst.seed_start = smp.seed;
+      if (q.op == ETXB_MEDIUM_BOUNDS) {
+        float3 pos = origin, dir = direction;
+        dst.flag = medium_intersects_bounds(scene.mediums[q.medium], origin, direction, q.max_t, pos, dir, dst.t_min, dst.t_max) ? 1u : 0u;
+        put(dst.pos, pos);
+        put(dst.dir, dir);
+      } else if (q.op == ETXB_MEDIUM_DENSITY) {
+        dst.value[0] = medium_sample_density_internal(scene.mediums[q.medium], origin);
+      } else if (q.op == ETXB_MEDIUM_TRANSMITTANCE) {
+        put_spectral(dst.value, medium_transmittance(scene, scene.mediums[q.medium], spect, smp, origin, direction, q.max_t));
+      } else if (q.op == ETXB_MEDIUM_SAMPLE) {
+        const SpectralResponse throughput =
+          scene.spectral() ? SpectralResponse{spect, q.throughput[0]} : SpectralResponse{spect, float3{q.throughput[0], q.throughput[1], q.throughput[2]}};
+        const Medium::Sample s = sample_medium(scene, scene.mediums[q.medium], spect, throughput, smp, origin, direction, q.max_t);
+        put_spectral(dst.value, s.weight);
+        put(dst.pos, s.pos);
+        dst.t = s.sampled_medium_t;
+      } else if (q.op == ETXB_MEDIUM_PHASE) {
+        dst.value[0] = phase_function(direction, {q.w_o[0], q.w_o[1], q.w_o[2]}, q.g);
+        put(dst.dir, sample_phase_function(direction, q.g, {q.rnd[0], q.rnd[1]}));
+      } else {
+        const SpectralResponse tr = o->rt.trace_transmittance(spect, scene, origin, {q.end[0], q.end[1], q.end[2]}, Medium::Instance{.index = q.medium}, smp);
+        put_spectral(dst.value, tr);
+      }
+      dst.seed_end = smp.seed;
+      out[t] = dst;
+    }
+  });
+}
+
 // The reference's own photon gather (VCMSpatialGridData::gather, vcm_shared.hxx:886-924) for etxb_debug_merge's inputs: the light-vertex
 // records (device layout, 96 B) become o.light_vertices and build_grid runs on them at the current iteration; each query becomes the
 // Intersection make_intersection builds for its hit (as oracle_trace does) and a VCMPathState, and is gathered `repetitions` times on
