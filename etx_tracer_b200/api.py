@@ -111,6 +111,7 @@ def load_library(flavor="fast"):
     lib.etxb_read_film_ldr.argtypes = [vp, u32, C.c_float, vp, u64]
     lib.etxb_denoise.argtypes = [vp, u32]
     lib.etxb_debug_denoise.argtypes = [vp, vp, vp, vp, vp, vp, vp, u32, u32, vp, vp]
+    lib.etxb_debug_noise_estimate.argtypes = [vp, u32, u32, u32, C.c_float, vp, vp, vp, vp, vp, vp]
     lib.etxb_save_film.argtypes = [vp, u32, C.c_char_p, u32, C.c_float]
     lib.etxb_write_exr.argtypes = [C.c_char_p, vp, u32, u32]
     lib.etxb_write_png.argtypes = [C.c_char_p, vp, u32, u32]
@@ -365,7 +366,8 @@ class GPUVCM:
         self._check(self.lib.etxb_comm_init(self.h, world, rank, _p(comm_id), comm_id.nbytes))
 
     def comm_reduce_film(self, layer=S.FILM_RESULT, out=None):
-        """Collective: the whole frame on rank 0 (returned there; None elsewhere)."""
+        """Collective: the whole frame on rank 0 (returned there; None elsewhere).  Result, Camera, Light, and the path tracer's Normals, Albedo
+        and CameraAdaptive layers."""
         w, r = C.c_uint32(1), C.c_uint32(0)
         self._check(self.lib.etxb_comm_world(self.h, C.byref(w), C.byref(r)))
         if (out is None) and (r.value == 0):
@@ -539,6 +541,21 @@ class GPUVCM:
                                                 _p(g[1]) if g[1] is not None else None, w, h, _p(out), _p(var)))
         return out, var
 
+    def debug_noise_estimate(self, camera, adaptive, info, threshold, world=1):
+        """The path tracer's noise estimate as `world` pixel-tile ranks run it (etxb_debug_noise_estimate) on storage-order arrays: camera and
+        adaptive (H, W, 4) float32, info (H, W) uint32 S.BUF_PIXEL_INFO words.  Returns (info, error level, converged count, error sum)."""
+        camera = np.ascontiguousarray(camera, dtype=np.float32)
+        adaptive = np.ascontiguousarray(adaptive, dtype=np.float32)
+        info = np.ascontiguousarray(info, dtype=np.uint32)
+        h, w = info.shape
+        assert camera.shape == (h, w, 4) and adaptive.shape == (h, w, 4)
+        info_out = np.zeros((h, w), dtype=np.uint32)
+        error = np.zeros((h, w), dtype=np.float32)
+        stats = np.zeros(2, dtype=np.uint32)
+        self._check(self.lib.etxb_debug_noise_estimate(self.h, w, h, world, C.c_float(threshold), _p(camera), _p(adaptive), _p(info), _p(info_out), _p(error),
+                                                       _p(stats)))
+        return info_out, error, int(stats[0]), float(stats[1:2].view(np.float32)[0])
+
     def debug_sampler(self, a, b, draws):
         a = np.ascontiguousarray(a, dtype=np.uint32)
         b = np.ascontiguousarray(b, dtype=np.uint32)
@@ -647,10 +664,12 @@ class GPUPathTracing(GPUVCM):
         self._check(self.lib.etxb_pt_set_options(self.h, _p(self.pt_options)))
 
     def _converged(self, st):
-        """CPUPathTracingImpl::update (path_tracing.cxx:85-110): an iteration that processed no pixel (all converged) ends the run."""
+        """CPUPathTracingImpl::update (path_tracing.cxx:85-110): an iteration that processed no pixel (all converged) ends the run.  With a
+        communicator pixels_processed counts every rank's pixels, so all ranks stop at the same iteration."""
         return (st["completed_iterations"] > 0) and (self.pt_status()["pixels_processed"] == 0)
 
     def pt_status(self):
+        """etxb_pt_get_status; over all ranks on a context with a communicator."""
         st = np.zeros(1, dtype=S.PT_STATUS)
         self._check(self.lib.etxb_pt_get_status(self.h, _p(st)))
         return _fields(st)
@@ -693,7 +712,8 @@ class GPUVCMGroup:
     def set_integrator(self, integrator, pt_options=None):
         """Every lane renders with the VCM (default) or the path-tracing algorithm.  With iterations in flight each lane keeps its own film and per-pixel
         history, so the path tracer's adaptive sampling is switched off here (noise threshold 0: every pixel gets one sample per iteration, like the
-        reference with `noise_threshold 0`); the combined film is the mean over the iterations of all lanes."""
+        reference with `noise_threshold 0`); the combined film is the mean over the iterations of all lanes.  A group in pixel-tile mode
+        (comm_init with world >= 2) refuses the path tracer."""
         for g in self.lanes:
             g._check(self.lib.etxb_set_integrator(g.h, integrator))
             if integrator == S.INTEGRATOR_PT:

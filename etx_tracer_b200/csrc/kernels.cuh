@@ -150,13 +150,17 @@ DEV uint32_t film_path_pixel(const FilmBuffers& f, uint32_t i, uint32_t iteratio
   return x + y * f.width;
 }
 
+// the pixel-tile rule: film pixel (x, y) belongs to rank (tile % world) of the 32x32 tiles, numbered row by row
+__host__ __device__ inline uint32_t tile_rank(uint32_t width, uint32_t x, uint32_t y, uint32_t world) {
+  uint32_t tiles_x = (width + 31u) / 32u;
+  uint32_t tile = (y / 32u) * tiles_x + (x / 32u);
+  return tile % world;
+}
+
 DEV bool pixel_owned(const LaunchParams& p, uint32_t index, bool light_pass = false) {
   const uint32_t world = light_pass ? p.light_world : p.world;
   if (world <= 1u) return true;
-  uint32_t x = index % p.film.width, y = index / p.film.width;
-  uint32_t tiles_x = (p.film.width + 31u) / 32u;
-  uint32_t tile = (y / 32u) * tiles_x + (x / 32u);
-  return (tile % world) == p.rank;
+  return tile_rank(p.film.width, index % p.film.width, index / p.film.width, world) == p.rank;
 }
 
 template <bool SP>

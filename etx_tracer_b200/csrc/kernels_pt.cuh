@@ -5,7 +5,8 @@
 // (render/host/film.cxx:173-230), Film::active_pixel (:434-461), Film::estimate_noise_levels (:233-330).
 //
 // Stage list of one iteration:
-//   k_pt_begin -> { k_trace_closest* -> [sort by material] -> k_pt_shade [-> k_shadow_resolve] }* -> k_pt_accumulate -> [k_film_noise_level -> _rows -> _columns]
+//   k_pt_begin -> { k_trace_closest* -> [sort by material] -> k_pt_shade [-> k_shadow_resolve] }* -> k_pt_accumulate
+//     -> [k_film_noise_level -> (all-reduce of the active mask over the ranks) -> k_film_noise_dilate]
 // The payload lives in the VCM camera path's SoA columns (one PathBuffers allocation serves both integrators): thr.w = sampled_bsdf_pdf,
 // mis.x = eta, misc = (seed, path_length, medium, mis_weight), gathered = accumulated, bs_weight_pdf = view_albedo, bs_wo_eta = view_normal.
 #pragma once
@@ -20,7 +21,6 @@ struct PtFilm {
   float4* adaptive;      // StorageCameraAdaptive: the mean over every other sample
   uint32_t* info;        // InternalData: sample_count (bits 0-29), converged (bit 30), tmp (bit 31)
   float* error_level;
-  uint32_t* info_next;   // ping-pong partner of `info` for the two dilation passes
 };
 constexpr uint32_t kPtConverged = 1u << 30u;
 constexpr uint32_t kPtTmp = 1u << 31u;
@@ -252,14 +252,33 @@ __global__ void __launch_bounds__(256) k_film_fill_blocks(const __grid_constant_
   }
 }
 
-// Film::estimate_noise_levels (film.cxx:233-330), first pass: error level of every pixel that has not converged, the convergence decision, and
-// the two sums noise_level() is made of.  stats[0] = pixels that converged in this pass (the reference's `active_pixels`), stats[1] = bits of the
-// float sum of error levels (atomic adds: the summation order is not the reference's, which is itself thread-order dependent).
-__global__ void __launch_bounds__(256) k_film_noise_level(const __grid_constant__ FilmBuffers film, const __grid_constant__ PtFilm pf, float threshold, uint32_t* stats) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+// Film::estimate_noise_levels (film.cxx:233-330) as three steps that work on any set of 32x32 pixel tiles:
+//   k_film_noise_level   the first pass on this rank's pixels, and the packed ACTIVE MASK: bit = 1 where a pixel has not converged after it;
+//   exchange             on a context with a communicator, the ranks all-reduce (sum) the mask — every word has one owner, so the sum is the
+//                        one-GPU mask — and the small stats behind it;
+//   k_film_noise_dilate  the two dilation passes, read from the mask alone, written to this rank's pixels.
+// Mask layout: storage row r holds ceil(W / 32) words, word k the pixels x = 32k .. 32k + 31 (bit x % 32).  A tile is 32 pixels wide and
+// starts at a multiple of 32, and a storage row is one film row (y-flipped), so a word never spans two ranks.  The words of other ranks stay
+// zero on a rank, and zero reads as converged.
+// After the mask: kNoiseStats words, all-reduced with it (the float sum in a call of its own).
+constexpr uint32_t kNoiseStatConverged = 0u;  // pixels that converged in this pass (the reference's `active_pixels`)
+constexpr uint32_t kNoiseStatProcessed = 1u;  // CPUPathTracingImpl::pixels_processed of the iteration (written by the host)
+constexpr uint32_t kNoiseStatError = 2u;      // bits of the float sum of the error levels of this pass
+constexpr uint32_t kNoiseStats = 3u;
+__host__ __device__ inline uint32_t noise_mask_words_per_row(uint32_t width) { return (width + 31u) / 32u; }
+
+// first pass: error level of every owned pixel that has not converged, the convergence decision, the mask word (one warp per word, one ballot),
+// and the two sums noise_level() is made of (atomic adds: the summation order is not the reference's, which is itself thread-order dependent).
+__global__ void __launch_bounds__(256) k_film_noise_level(const __grid_constant__ FilmBuffers film, const __grid_constant__ PtFilm pf, float threshold, uint32_t rank,
+                                                          uint32_t world, uint32_t* mask, uint32_t* stats) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x, lane = t & 31u, word = t >> 5u;
+  const uint32_t wpr = noise_mask_words_per_row(film.width);
+  const uint32_t r = word / wpr, x = (word % wpr) * 32u + lane;
   float error_level = 0.0f;
   uint32_t converged = 0u;
-  if (i < film.width * film.height) {
+  bool active = false;
+  if ((r < film.height) && (x < film.width) && (tile_rank(film.width, x, film.height - 1u - r, world) == rank)) {
+    const uint32_t i = x + r * film.width;
     uint32_t info = pf.info[i];
     if ((info & kPtConverged) == 0u) {
       float4 c = film.camera[i], a = pf.adaptive[i];
@@ -267,53 +286,54 @@ __global__ void __launch_bounds__(256) k_film_noise_level(const __grid_constant_
       float error_norm = fabsf(c.x) + fabsf(c.y) + fabsf(c.z);
       error_level = error_diff / (((error_norm < 1.0f) ? sqrtf(error_norm) : error_norm) + kEpsilon);
       converged = (error_level < threshold) ? 1u : 0u;
+      active = (converged == 0u);
       pf.error_level[i] = error_level;
       pf.info[i] = (info & kPtCountMask) | (converged ? (kPtConverged | kPtTmp) : 0u);
     }
   }
+  const uint32_t bits = __ballot_sync(0xffffffffu, active);
   uint32_t n = __reduce_add_sync(0xffffffffu, converged);
   float sum = error_level;
   for (uint32_t o = 16u; o > 0u; o >>= 1u) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  if ((threadIdx.x & 31u) == 0u) {
-    if (n) atomicAdd(stats + 0, n);
-    if (sum != 0.0f) atomicAdd(reinterpret_cast<float*>(stats + 1), sum);
+  if ((lane == 0u) && (r < film.height)) {
+    mask[word] = bits;
+    if (n) atomicAdd(stats + kNoiseStatConverged, n);
+    if (sum != 0.0f) atomicAdd(reinterpret_cast<float*>(stats + kNoiseStatError), sum);
   }
 }
 
-// second pass (:283-298): every pixel that has not converged clears `tmp` of the pixels x - 5 .. x + 4 of its row — as a gather: pixel p loses
-// `tmp` when a pixel x in [p - 4, p + 5] of its row has not converged
-constexpr int32_t kNoiseBlock = 5;
-__global__ void __launch_bounds__(256) k_film_noise_rows(const __grid_constant__ FilmBuffers film, const uint32_t* info_in, uint32_t* info_out) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= film.width * film.height) return;
-  const int32_t w = int32_t(film.width), x = int32_t(i % film.width), row = int32_t(i / film.width) * w;
-  uint32_t info = info_in[i];
-  if (info & kPtTmp) {
-    for (int32_t q = max(0, x - (kNoiseBlock - 1)); q <= min(w - 1, x + kNoiseBlock); ++q) {
-      if ((info_in[row + q] & kPtConverged) == 0u) {
-        info &= ~kPtTmp;
-        break;
-      }
-    }
-  }
-  info_out[i] = info;
+// Which pixels of word k of a mask row have an active pixel x - 4 .. x + 5 in that row (pixels off the film read as converged)
+DEV uint32_t noise_row_window(const uint32_t* row, uint32_t k, uint32_t wpr) {
+  const uint32_t prev = (k > 0u) ? row[k - 1u] : 0u, cur = row[k], next = (k + 1u < wpr) ? row[k + 1u] : 0u;
+  uint32_t d = cur;
+#pragma unroll
+  for (uint32_t s = 1u; s <= 5u; ++s) d |= __funnelshift_r(cur, next, s);  // bit x: pixel x + s
+#pragma unroll
+  for (uint32_t s = 1u; s <= 4u; ++s) d |= __funnelshift_l(prev, cur, s);  // bit x: pixel x - s
+  return d;
 }
 
-// third pass (:304-320): every pixel without `tmp` clears `converged` of the pixels y - 5 .. y + 4 of its column
-__global__ void __launch_bounds__(256) k_film_noise_columns(const __grid_constant__ FilmBuffers film, const uint32_t* info_in, uint32_t* info_out) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= film.width * film.height) return;
-  const int32_t w = int32_t(film.width), h = int32_t(film.height), x = int32_t(i % film.width), y = int32_t(i / film.width);
-  uint32_t info = info_in[i];
-  if (info & kPtConverged) {
-    for (int32_t q = max(0, y - (kNoiseBlock - 1)); q <= min(h - 1, y + kNoiseBlock); ++q) {
-      if ((info_in[x + q * w] & kPtTmp) == 0u) {
-        info &= ~kPtConverged;
-        break;
-      }
-    }
-  }
-  info_out[i] = info;
+// second and third pass (:283-320) as one gather over the mask.  The reference clears `tmp` of x - 5 .. x + 4 around every active pixel, then
+// `converged` of y - 5 .. y + 4 around every pixel without `tmp`.  A pixel has `tmp` after the first pass exactly when it is not active (a pixel
+// converged in an earlier estimate kept both bits), so pixel p loses `tmp` when its row window [x - 4, x + 5] holds an active pixel, and
+// `converged` when the row window of any row in [y - 4, y + 5] does (test_pt_tiles_model.py checks this against the scatter form).
+__global__ void __launch_bounds__(256) k_film_noise_dilate(uint32_t width, uint32_t height, uint32_t rank, uint32_t world, const uint32_t* mask, uint32_t* info) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x, lane = t & 31u, word = t >> 5u;
+  const uint32_t wpr = noise_mask_words_per_row(width);
+  const uint32_t r = word / wpr, k = word % wpr, x = k * 32u + lane;
+  if ((r >= height) || (x >= width) || (tile_rank(width, x, height - 1u - r, world) != rank)) return;
+  const uint32_t i = x + r * width;
+  uint32_t v = info[i];
+  if ((v & (kPtConverged | kPtTmp)) == 0u) return;  // an active pixel has neither bit to lose
+  const uint32_t row = noise_row_window(mask + r * wpr, k, wpr);
+  uint32_t box = row;
+  const uint32_t r0 = (r >= 4u) ? (r - 4u) : 0u, r1 = umin(height - 1u, r + 5u);
+  for (uint32_t q = r0; q <= r1; ++q)
+    if (q != r) box |= noise_row_window(mask + q * wpr, k, wpr);
+  const uint32_t bit = 1u << lane;
+  if (row & bit) v &= ~kPtTmp;
+  if (box & bit) v &= ~kPtConverged;
+  info[i] = v;
 }
 
 // Film::layer for the layers the VCM integrator leaves empty (film.cxx:406-414): normals are shown as n * 0.5 + 0.5

@@ -72,12 +72,14 @@ enum KernelId : uint32_t {
   K_DENOISE_VARIANCE,
   K_DENOISE_SMOOTH,
   K_DENOISE_NLM,
+  K_COMM_PT_MASK,
+  K_COMM_PT_COUNT,
   K_COUNT
 };
 const char* kKernelNames[K_COUNT] = {"light_begin", "trace_closest(light)", "light_bounce", "lv_scan", "lv_reorder", "grid_bbox", "grid_keys", "grid_sort", "grid_build",
   "camera_begin", "trace_closest(camera)", "camera_shade", "camera_connect", "shadow_trace", "queue_sort", "camera_merge_sort", "camera_merge", "camera_merge_generic", "camera_continue", "film_commit_light", "nccl_allreduce_light_image", "nccl_allgather_photons",
   "pt_begin", "pt_shade", "pt_accumulate", "film_noise_levels", "bvh_build", "bvh_collapse_wide",
-  "film_adaptive_vcm", "denoise_variance", "denoise_smooth", "denoise_nlm"};
+  "film_adaptive_vcm", "denoise_variance", "denoise_smooth", "denoise_nlm", "nccl_allreduce_pt_mask", "nccl_allreduce_pt_count"};
 
 // Queue sizes from which a pass takes its large-queue branches (the context's `thresholds`; etxb_debug_set_thresholds overrides them):
 //   merge_sort_min_queries  the gather queue is sorted by its merge keys (below it, a latency-bound tail, the sort launches cost more than they save)
@@ -244,12 +246,14 @@ struct etxb_ctx {
   DevBuf<float4> denoise_u, denoise_var_raw, denoise_var;   // etxb_denoise scratch: colour with its flags, variance, smoothed variance
   DevBuf<uint32_t> denoise_flag;                            // set by k_denoise_variance where a pixel has fewer than two samples
   DevBuf<uint32_t> film_ldr;                                 // the tone-mapped RGBA8 frame of etxb_read_film_ldr
-  DevBuf<uint32_t> pt_info, pt_info_next, pt_stats;          // InternalData (sample count, converged, tmp); [converged this pass, error sum bits]
+  DevBuf<uint32_t> pt_info;                                  // InternalData (sample count, converged, tmp)
+  DevBuf<uint32_t> pt_mask;                                  // the noise estimate's active mask + kNoiseStats (kernels_pt.cuh)
   DevBuf<float> pt_error;
   uint32_t pixel_sampler_image = 0xffffffffu;
   float pixel_sampler_radius = 1.0f, noise_threshold = 0.0f, radiance_clamp = 0.0f;
   uint32_t scene_samples = 0;
-  uint32_t pt_pixels_processed = 0, pt_active_pixels = 0;  // active pixels of the last iteration; Film::active_pixel_count
+  uint32_t pt_pixels_processed = 0, pt_active_pixels = 0;  // active pixels of the last iteration; Film::active_pixel_count (over all ranks
+                                                           // on a context with a communicator)
   float pt_noise_level = 0.0f;                             // Film::noise_level
 
   etxb_vcm_options options = {};
@@ -257,6 +261,7 @@ struct etxb_ctx {
   bool external_iteration = false;   // etxb_set_next_iteration: the caller sets every iteration's index, it does not advance by itself
   uint32_t completed = 0;            // iterations finished since etxb_begin
   uint32_t rank = 0, world = 1;
+  bool group_lane = false;           // a lane of an etxb_group (etxb_group_create)
   bool light_full = false;           // camera-split iterations (etxb_group replicas): the partition applies to the camera pass only, the light pass traces every path
   uint32_t last_light_vertices = 0;
   uint32_t overflow_flag = 0;
@@ -1052,37 +1057,98 @@ int pt_ensure_film(etxb_ctx* ctx) {
   }
   if (int rc = film_ensure_adaptive(ctx)) return rc;
   CUDA_OK(ctx, ctx->pt_info.alloc(n));
-  CUDA_OK(ctx, ctx->pt_info_next.alloc(n));
   CUDA_OK(ctx, ctx->pt_error.alloc(n));
-  CUDA_OK(ctx, ctx->pt_stats.alloc(2));
   CUDA_OK(ctx, cudaMemsetAsync(ctx->pt_info.ptr, 0, n * 4, ctx->stream));
   CUDA_OK(ctx, cudaMemsetAsync(ctx->pt_error.ptr, 0, n * 4, ctx->stream));
   return ETXB_OK;
 }
 
-PtFilm make_pt_film(etxb_ctx* ctx) { return {ctx->film_normals.ptr, ctx->film_albedo.ptr, ctx->film_adaptive.ptr, ctx->pt_info.ptr, ctx->pt_error.ptr, ctx->pt_info_next.ptr}; }
+PtFilm make_pt_film(etxb_ctx* ctx) { return {ctx->film_normals.ptr, ctx->film_albedo.ptr, ctx->film_adaptive.ptr, ctx->pt_info.ptr, ctx->pt_error.ptr}; }
 
-// Film::estimate_noise_levels (film.cxx:233-330) after iteration `sample_index`
+// The buffers one rank's noise estimate reads and writes: its film, its history, the mask (+ kNoiseStats) and its place in the tile rule
+struct NoiseView {
+  FilmBuffers film;
+  PtFilm pf;
+  uint32_t* mask;
+  uint32_t rank, world;
+};
+
+uint32_t noise_mask_words(uint32_t width, uint32_t height) { return height * noise_mask_words_per_row(width); }
+
+int noise_level_pass(etxb_ctx* ctx, const NoiseView& v, float threshold) {
+  const uint32_t words = noise_mask_words(v.film.width, v.film.height);
+  CUDA_OK(ctx, cudaMemsetAsync(v.mask + words, 0, kNoiseStats * 4u, ctx->stream));
+  LaunchTimer t(ctx, K_FILM_NOISE);
+  k_film_noise_level<<<blocks_for(words * 32u, 256), 256, 0, ctx->stream>>>(v.film, v.pf, threshold, v.rank, v.world, v.mask, v.mask + words);
+  return ETXB_OK;
+}
+
+int noise_dilate_pass(etxb_ctx* ctx, const NoiseView& v) {
+  LaunchTimer t(ctx, K_FILM_NOISE);
+  k_film_noise_dilate<<<blocks_for(noise_mask_words(v.film.width, v.film.height) * 32u, 256), 256, 0, ctx->stream>>>(v.film.width, v.film.height, v.rank, v.world,
+                                                                                                                         v.mask, v.pf.info);
+  return ETXB_OK;
+}
+
+// The path tracer's only collective, on the context's high-priority stream fenced by events like comm_exchange: with `mask`, the active mask
+// with the converged count and pixels_processed (uint32 sums: the words of different ranks are disjoint) and the error sum (float); without,
+// pixels_processed alone.
+int comm_noise_exchange(etxb_ctx* ctx, uint32_t words, bool mask) {
+  NcclApi* n = nccl_api();
+  cudaStream_t cs = ctx->comm_stream;
+  uint32_t* m = ctx->pt_mask.ptr;
+  LaunchTimer t(ctx, mask ? K_COMM_PT_MASK : K_COMM_PT_COUNT);
+  CUDA_OK(ctx, cudaEventRecord(ctx->comm_ev_in, ctx->stream));
+  CUDA_OK(ctx, cudaStreamWaitEvent(cs, ctx->comm_ev_in, 0));
+  if (mask) {
+    NCCL_OK(ctx, n->GroupStart());
+    ncclResult_t res = n->AllReduce(m, m, size_t(words) + kNoiseStatProcessed + 1u, ncclUint32, ncclSum, ctx->comm, cs);
+    if (res == ncclSuccess) res = n->AllReduce(m + words + kNoiseStatError, m + words + kNoiseStatError, 1, ncclFloat, ncclSum, ctx->comm, cs);
+    ncclResult_t end = n->GroupEnd();
+    NCCL_OK(ctx, (res != ncclSuccess) ? res : end);
+  } else {
+    NCCL_OK(ctx, n->AllReduce(m + words + kNoiseStatProcessed, m + words + kNoiseStatProcessed, 1, ncclUint32, ncclSum, ctx->comm, cs));
+  }
+  CUDA_OK(ctx, cudaEventRecord(ctx->comm_ev_out, cs));
+  CUDA_OK(ctx, cudaStreamWaitEvent(ctx->stream, ctx->comm_ev_out, 0));
+  return ETXB_OK;
+}
+
+// Film::estimate_noise_levels (film.cxx:233-330) after iteration `sample_index`, on this context's pixels.  On a context with a communicator this
+// is also where the ranks agree on what update() reads: every iteration all-reduces pixels_processed, one with an estimate the mask and the
+// stats as well.  Which collectives a rank issues thus depends on the iteration index, the noise threshold and Scene::samples alone.
 constexpr uint32_t kFilmMinSamples = 32u;
 int pt_estimate_noise_levels(etxb_ctx* ctx, uint32_t sample_index) {
   const float threshold = ctx->noise_threshold;
-  if ((threshold == 0.0f) || (sample_index < kFilmMinSamples) || ((sample_index % 2u) != 0u)) return ETXB_OK;
-  LaunchTimer t(ctx, K_FILM_NOISE);
-  const uint32_t n = ctx->path_count;
-  FilmBuffers film = {ctx->film_camera.ptr, ctx->film_light.ptr, ctx->film_light_iteration.ptr, ctx->width, ctx->height};
-  PtFilm pf = make_pt_film(ctx);
-  CUDA_OK(ctx, cudaMemsetAsync(ctx->pt_stats.ptr, 0, 8, ctx->stream));
-  k_film_noise_level<<<blocks_for(n, 256), 256, 0, ctx->stream>>>(film, pf, threshold, ctx->pt_stats.ptr);
-  k_film_noise_rows<<<blocks_for(n, 256), 256, 0, ctx->stream>>>(film, ctx->pt_info.ptr, ctx->pt_info_next.ptr);
-  k_film_noise_columns<<<blocks_for(n, 256), 256, 0, ctx->stream>>>(film, ctx->pt_info_next.ptr, ctx->pt_info.ptr);
-  ctx->kernel_launches += 2;
-  uint32_t stats[2] = {0u, 0u};
-  CUDA_OK(ctx, cudaMemcpyAsync(stats, ctx->pt_stats.ptr, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  const bool estimate = (threshold != 0.0f) && (sample_index >= kFilmMinSamples) && ((sample_index % 2u) == 0u);
+  const bool comm = ctx->comm != nullptr;
+  if (!estimate && !comm) return ETXB_OK;
+  const uint32_t words = noise_mask_words(ctx->width, ctx->height);
+  if (ctx->pt_mask.count != size_t(words) + kNoiseStats) CUDA_OK(ctx, ctx->pt_mask.alloc(size_t(words) + kNoiseStats));
+  uint32_t* stats = ctx->pt_mask.ptr + words;
+  const NoiseView v = {{ctx->film_camera.ptr, ctx->film_light.ptr, ctx->film_light_iteration.ptr, ctx->width, ctx->height}, make_pt_film(ctx), ctx->pt_mask.ptr,
+                       ctx->rank, ctx->world};
+  if (estimate) {
+    if (int rc = noise_level_pass(ctx, v, threshold)) return rc;
+  }
+  if (comm) {
+    const uint32_t processed = ctx->pt_pixels_processed;
+    CUDA_OK(ctx, cudaMemcpyAsync(stats + kNoiseStatProcessed, &processed, 4, cudaMemcpyHostToDevice, ctx->stream));
+    if (int rc = comm_noise_exchange(ctx, words, estimate)) return rc;
+  }
+  if (estimate) {
+    if (int rc = noise_dilate_pass(ctx, v)) return rc;
+  }
+  uint32_t host[kNoiseStats] = {};
+  CUDA_OK(ctx, cudaMemcpyAsync(host, stats, sizeof(host), cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-  float total = 0.0f;
-  memcpy(&total, &stats[1], 4);
-  ctx->pt_active_pixels = stats[0];
-  ctx->pt_noise_level = (stats[0] > 0u) ? (total / float(stats[0])) : total;
+  if (comm) ctx->pt_pixels_processed = host[kNoiseStatProcessed];
+  if (estimate) {
+    float total = 0.0f;
+    memcpy(&total, &host[kNoiseStatError], 4);
+    ctx->pt_active_pixels = host[kNoiseStatConverged];
+    ctx->pt_noise_level = (host[kNoiseStatConverged] > 0u) ? (total / float(host[kNoiseStatConverged])) : total;
+  }
   return ETXB_OK;
 }
 
@@ -2278,7 +2344,10 @@ int etxb_pt_set_options(etxb_ctx* ctx, const etxb_pt_options* opt) {
 int etxb_set_integrator(etxb_ctx* ctx, uint32_t integrator) {
   if (!ctx || (integrator > ETXB_INTEGRATOR_PT)) return ETXB_ERR_INVALID_ARGUMENT;
   if (int rc = ctx_drain(ctx)) return rc;
-  if ((integrator == ETXB_INTEGRATOR_PT) && (ctx->world > 1u)) return fail(ctx, ETXB_ERR_UNSUPPORTED, "the path tracer runs on one GPU per context");
+  // pixel tiles need the ranks' noise estimates combined (a communicator), and a group's lanes would each keep their own history
+  if ((integrator == ETXB_INTEGRATOR_PT) && (ctx->world > 1u) && ((ctx->comm == nullptr) || ctx->group_lane))
+    return fail(ctx, ETXB_ERR_UNSUPPORTED, ctx->group_lane ? "the path tracer does not run on a group in pixel-tile mode: each lane would keep its own per-pixel history"
+                                                          : "the path tracer renders pixel tiles only with a communicator (etxb_comm_init)");
   ctx->integrator = integrator;
   return ETXB_OK;
 }
@@ -2338,7 +2407,7 @@ int etxb_comm_world(const etxb_ctx* ctx, uint32_t* world, uint32_t* rank) {
 // Collective: every rank calls it.  The disjoint camera tiles are summed on rank 0 (ncclReduce of the float4 film); the light layer is already
 // complete on every rank.  On rank 0 `dst_rgba` (may be null elsewhere) receives the layer like etxb_read_film.
 int etxb_comm_reduce_film(etxb_ctx* ctx, uint32_t layer, float* dst_rgba, uint64_t dst_bytes) {
-  if (!ctx || (layer > ETXB_FILM_LIGHT)) return ETXB_ERR_INVALID_ARGUMENT;
+  if (!ctx || (layer == ETXB_FILM_LIGHT_ITERATION) || (layer > ETXB_FILM_CAMERA_ADAPTIVE)) return ETXB_ERR_INVALID_ARGUMENT;
   if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
   if (ctx->comm == nullptr) return etxb_read_film(ctx, layer, dst_rgba, dst_bytes);
   if (int rc = ctx_drain(ctx)) return rc;
@@ -2346,15 +2415,28 @@ int etxb_comm_reduce_film(etxb_ctx* ctx, uint32_t layer, float* dst_rgba, uint64
   cudaSetDevice(ctx->device);
   const size_t px = ctx->path_count;
   if (ctx->film_reduced.count < px) CUDA_OK(ctx, ctx->film_reduced.alloc(px));
+  // the tiled layers: each rank holds its own tiles and zeros elsewhere (k_pt_accumulate and k_film_adaptive_vcm write owned pixels only)
+  const float4* tiles = ctx->film_camera.ptr;
+  if ((layer == ETXB_FILM_NORMALS) || (layer == ETXB_FILM_ALBEDO)) {
+    if (int rc = pt_ensure_film(ctx)) return rc;
+    tiles = (layer == ETXB_FILM_NORMALS) ? ctx->film_normals.ptr : ctx->film_albedo.ptr;
+  } else if (layer == ETXB_FILM_CAMERA_ADAPTIVE) {
+    if (int rc = film_ensure_adaptive(ctx)) return rc;
+    tiles = ctx->film_adaptive.ptr;
+  }
   if (layer != ETXB_FILM_LIGHT)
-    NCCL_OK(ctx, n->Reduce(ctx->film_camera.ptr, ctx->film_reduced.ptr, px * 4u, ncclFloat, ncclSum, 0, ctx->comm, ctx->stream));
+    NCCL_OK(ctx, n->Reduce(tiles, ctx->film_reduced.ptr, px * 4u, ncclFloat, ncclSum, 0, ctx->comm, ctx->stream));
   if (ctx->rank != 0u) {
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     return ETXB_OK;
   }
   if (!dst_rgba || (dst_bytes < px * 16u)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "film buffer too small");
-  const float4* src = ctx->film_light.ptr;
-  if (layer == ETXB_FILM_CAMERA) src = ctx->film_reduced.ptr;
+  const float4* src = (layer == ETXB_FILM_LIGHT) ? ctx->film_light.ptr : ctx->film_reduced.ptr;
+  if (layer == ETXB_FILM_NORMALS) {  // etxb_read_film's read-out (Film::layer: n * 0.5 + 0.5)
+    k_film_layer_normals<<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(ctx->film_reduced.ptr, ctx->film_out.ptr, ctx->path_count);
+    ctx->kernel_launches += 1;
+    src = ctx->film_out.ptr;
+  }
   if (layer == ETXB_FILM_RESULT) {
     FilmBuffers film = {ctx->film_reduced.ptr, ctx->film_light.ptr, ctx->film_light_iteration.ptr, ctx->width, ctx->height};
     k_film_resolve<<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(film, ctx->film_out.ptr);
@@ -2765,6 +2847,77 @@ int etxb_debug_denoise(etxb_ctx* ctx, const float* color, const float* camera, c
   return ETXB_OK;
 }
 
+// Test hook: the noise estimate of `world` pixel-tile ranks on one device (layout in include/etx_b200.h).  Each rank's view holds its own pixels
+// and zeros elsewhere, as a rank's buffers do; the all-reduce of pt_estimate_noise_levels is replaced by the same sum on the host.
+int etxb_debug_noise_estimate(etxb_ctx* ctx, uint32_t width, uint32_t height, uint32_t world, float threshold, const float* camera, const float* adaptive,
+                              const uint32_t* info_in, uint32_t* info_out, float* error_out, uint32_t* stats_out) {
+  if (!ctx || !camera || !adaptive || !info_in || !info_out || !error_out || !stats_out || !width || !height || !world) return ETXB_ERR_INVALID_ARGUMENT;
+  if (!(threshold >= 0.0f) || (uint64_t(width) * height > (1ull << 26)) || (world > 1024u)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "etxb_debug_noise_estimate: bad threshold, film size or world");
+  if (int rc = ctx_drain(ctx)) return rc;
+  cudaSetDevice(ctx->device);
+  const size_t n = size_t(width) * height;
+  const uint32_t words = noise_mask_words(width, height);
+  struct RankBuffers {
+    DevBuf<float4> camera, adaptive;
+    DevBuf<uint32_t> info, mask;
+    DevBuf<float> error;
+  };
+  std::vector<RankBuffers> ranks(world);
+  std::vector<NoiseView> views(world);
+  std::vector<float4> cam(n), ada(n);
+  std::vector<uint32_t> inf(n);
+  auto owner = [&](size_t i) { return tile_rank(width, uint32_t(i % width), height - 1u - uint32_t(i / width), world); };
+  const float4* camera4 = reinterpret_cast<const float4*>(camera);
+  const float4* adaptive4 = reinterpret_cast<const float4*>(adaptive);
+  for (uint32_t r = 0; r < world; ++r) {
+    for (size_t i = 0; i < n; ++i) {
+      const bool mine = owner(i) == r;
+      cam[i] = mine ? camera4[i] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+      ada[i] = mine ? adaptive4[i] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+      inf[i] = mine ? info_in[i] : 0u;
+    }
+    RankBuffers& b = ranks[r];
+    if (int rc = upload(ctx, b.camera, cam.data(), n)) return rc;
+    if (int rc = upload(ctx, b.adaptive, ada.data(), n)) return rc;
+    if (int rc = upload(ctx, b.info, inf.data(), n)) return rc;
+    CUDA_OK(ctx, b.error.alloc(n));
+    CUDA_OK(ctx, cudaMemsetAsync(b.error.ptr, 0, n * 4, ctx->stream));
+    CUDA_OK(ctx, b.mask.alloc(size_t(words) + kNoiseStats));
+    views[r] = {{b.camera.ptr, nullptr, nullptr, width, height}, {nullptr, nullptr, b.adaptive.ptr, b.info.ptr, b.error.ptr}, b.mask.ptr, r, world};
+    if (int rc = noise_level_pass(ctx, views[r], threshold)) return rc;
+  }
+  std::vector<uint32_t> sum(size_t(words) + kNoiseStats, 0u), part(size_t(words) + kNoiseStats);
+  float error_sum = 0.0f;
+  for (uint32_t r = 0; r < world; ++r) {
+    CUDA_OK(ctx, cudaMemcpyAsync(part.data(), ranks[r].mask.ptr, part.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    for (size_t j = 0; j < size_t(words) + kNoiseStatProcessed + 1u; ++j) sum[j] += part[j];
+    float e = 0.0f;
+    memcpy(&e, &part[words + kNoiseStatError], 4);
+    error_sum += e;
+  }
+  memcpy(&sum[words + kNoiseStatError], &error_sum, 4);
+  for (uint32_t r = 0; r < world; ++r) {
+    CUDA_OK(ctx, cudaMemcpyAsync(ranks[r].mask.ptr, sum.data(), sum.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    if (int rc = noise_dilate_pass(ctx, views[r])) return rc;
+  }
+  CUDA_OK(ctx, cudaGetLastError());
+  std::vector<float> err(n);
+  for (uint32_t r = 0; r < world; ++r) {
+    CUDA_OK(ctx, cudaMemcpyAsync(inf.data(), ranks[r].info.ptr, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(err.data(), ranks[r].error.ptr, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    for (size_t i = 0; i < n; ++i) {
+      if (owner(i) != r) continue;
+      info_out[i] = inf[i];
+      error_out[i] = err[i];
+    }
+  }
+  stats_out[0] = sum[words + kNoiseStatConverged];
+  stats_out[1] = sum[words + kNoiseStatError];
+  return ETXB_OK;
+}
+
 // Test hook: the vertex closures of dclosure.cuh, query by query (layout and outputs in include/etx_b200.h)
 int etxb_debug_closure_eval(etxb_ctx* ctx, const etxb_closure_query* queries, uint32_t count, uint32_t repetitions, double* out) {
   if (!ctx || !queries || !out || (repetitions == 0)) return ETXB_ERR_INVALID_ARGUMENT;
@@ -3046,6 +3199,7 @@ int etxb_group_create(etxb_group** out, const etxb_device_config* cfg, uint32_t 
       delete grp;
       return rc;
     }
+    ctx->group_lane = true;
     grp->lanes.push_back(ctx);
   }
   grp->plan.queues.resize(lanes);
@@ -3200,8 +3354,11 @@ int etxb_group_comm_init(etxb_group* grp, uint32_t world, uint32_t rank, const v
   if (int rc = etxb_group_wait(grp)) return rc;
   if (grp->reduce_comm != nullptr) return group_refuse(grp, "etxb_group_comm_init: the group already has a communicator");
   if ((world > 1u) && (grp->plan.split_lane != 0xffffffffu)) return group_refuse(grp, "etxb_group_comm_init: pixel tiles and a split lane exclude each other");
-  for (auto* c : grp->lanes)
+  for (auto* c : grp->lanes) {
     if (c->target_pixel_size > 1u) return group_refuse(grp, "etxb_group_comm_init: the coarse preview (film pixel size above 1) renders on one GPU", ETXB_ERR_UNSUPPORTED);
+    if ((world > 1u) && (c->integrator == ETXB_INTEGRATOR_PT))
+      return group_refuse(grp, "etxb_group_comm_init: the path tracer does not run on a group in pixel-tile mode: each lane would keep its own per-pixel history", ETXB_ERR_UNSUPPORTED);
+  }
   const uint8_t* bytes = static_cast<const uint8_t*>(ids);
   for (size_t l = 0; l < grp->lanes.size(); ++l) {
     if (int rc = etxb_comm_init(grp->lanes[l], world, rank, bytes + l * sizeof(ncclUniqueId), sizeof(ncclUniqueId))) {

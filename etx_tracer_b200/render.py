@@ -3,14 +3,15 @@
 What the reference application does between File > Open and File > Save (sources/raytracer/app.cxx: load_scene_file :318-352, the integrator
 selected by options.json "integrator" :88-99, on_save_image_selected :261-295) without its window: the scene loader (the module's C++ one by default; host/render_main.cpp is this program in C++), one of the two
 device integrators — "vcm" (CPUVCM's algorithm, the default) or "pt" (CPUPathTracing's) — pumped like IntegratorThread pumps Integrator::update,
-and the film export (OpenEXR float layer, or the tone-mapped PNG).  There is no CPU fallback: without a CUDA device this fails.
+and the film export (OpenEXR float layer, or the tone-mapped PNG).  There is no CPU fallback: without a CUDA device this fails.  With --gpus N
+the frame is split into pixel tiles over N GPUs, one process each (both integrators; the exchange runs inside the module over NCCL).
 """
 import argparse
 import sys
 import time
 
 from . import loader, structs as S
-from .api import GPUPathTracing, GPUVCM, SceneFile
+from .api import GPUPathTracing, GPUVCM, SceneFile, tonemap, write_exr, write_png
 
 LAYERS = {"result": S.FILM_RESULT, "camera": S.FILM_CAMERA, "light": S.FILM_LIGHT, "normals": S.FILM_NORMALS, "albedo": S.FILM_ALBEDO,
           "denoised": S.FILM_DENOISED}
@@ -29,16 +30,58 @@ def main(argv=None):
     ap.add_argument("--denoise", action="store_true", help="denoise the Result layer before the export (the application's Denoise button); "
                     "--layer defaults to denoised")
     ap.add_argument("--noise-threshold", type=float, default=None, help="pt: Scene::noise_threshold of the adaptive sampling (default: the scene's)")
+    ap.add_argument("--gpus", type=int, default=1, help="render pixel tiles on this many GPUs, one process each, exchanging over NCCL inside the "
+                    "module; rank 0 writes the output")
     args = ap.parse_args(argv)
+    if args.gpus < 1:
+        ap.error("--gpus must be at least 1")
+    if args.gpus == 1:
+        return _render(args)
+    if args.denoise:
+        ap.error("--denoise needs the whole film and its sample counts on one GPU: render with --gpus 1 to denoise")
+    import socket
+    import torch
+    import torch.multiprocessing as mp
+    if torch.cuda.device_count() < args.gpus:
+        ap.error(f"--gpus {args.gpus}: this machine has {torch.cuda.device_count()} CUDA devices")
+    with socket.socket() as s:
+        s.bind(("127.0.0.1", 0))
+        port = s.getsockname()[1]
+    mp.spawn(_rank, args=(args, port), nprocs=args.gpus, join=True)
+    return 0
 
+
+def _rank(rank, args, port):
+    """One process of a --gpus N render: a localhost process group hands the module's NCCL id to every rank, then each renders its tiles."""
+    import os
+    import torch
+    import torch.distributed as dist
+    from .api import comm_unique_ids
+    from .multigpu import distribute_comm_ids
+    os.environ["MASTER_ADDR"] = "127.0.0.1"
+    os.environ["MASTER_PORT"] = str(port)
+    torch.cuda.set_device(rank)
+    dist.init_process_group("nccl", rank=rank, world_size=args.gpus, device_id=torch.device("cuda", rank))
+    try:
+        comm_id = distribute_comm_ids(dist, rank, 1, comm_unique_ids, device=torch.device("cuda", rank))
+        _render(args, rank, comm_id)
+    finally:
+        dist.destroy_process_group()
+
+
+def _render(args, rank=0, comm_id=None):
+    world = args.gpus
+    log = (lambda *a: print(*a, file=sys.stderr)) if rank == 0 else (lambda *a: None)
     t0 = time.time()
     sd = SceneFile(args.scene) if args.loader == "cpp" else loader.load_scene(args.scene)
     for w in (sd.warnings if args.loader == "cpp" else sd.loader_warnings):
-        print("warning:", w, file=sys.stderr)
-    print(f"loaded {sd.triangle_count} triangles, {sd.width}x{sd.height}, in {time.time() - t0:.2f} s", file=sys.stderr)
+        log("warning:", w)
+    log(f"loaded {sd.triangle_count} triangles, {sd.width}x{sd.height}, in {time.time() - t0:.2f} s")
     if args.spp > 0:
         sd.scene["samples"] = args.spp
-    g = (GPUPathTracing if args.integrator == "pt" else GPUVCM)(sd, flavor="fast")
+    g = (GPUPathTracing if args.integrator == "pt" else GPUVCM)(sd, flavor="fast", device=rank)
+    if comm_id is not None:
+        g.comm_init(world, rank, comm_id)
     for kv in args.option:
         key, _, value = kv.partition("=")
         g.set_option(key, float(value))
@@ -50,12 +93,23 @@ def main(argv=None):
     g.wait()
     st = g.status()
     n = sd.width * sd.height * st["completed_iterations"]
-    print(f"{st['completed_iterations']} iterations in {st['total_time']:.3f} s of device time: {n / max(st['total_time'], 1e-9) / 1e6:.2f} Msamples/s", file=sys.stderr)
+    log(f"{st['completed_iterations']} iterations in {st['total_time']:.3f} s of device time{f' on rank 0 of {world}' if world > 1 else ''}: "
+        f"{n / max(st['total_time'], 1e-9) / 1e6:.2f} Msamples/s")
     if args.denoise:
         g.denoise(S.FILM_RESULT)
     layer = args.layer or ("denoised" if args.denoise else "result")
-    g.save_image(args.output, LAYERS[layer], tonemapped=args.output.lower().endswith(".png"), exposure=args.exposure)
-    print(args.output)
+    tonemapped = args.output.lower().endswith(".png")
+    if comm_id is None:
+        g.save_image(args.output, LAYERS[layer], tonemapped=tonemapped, exposure=args.exposure)
+    else:
+        film = g.comm_reduce_film(LAYERS[layer])  # collective; the frame arrives on rank 0
+        if rank == 0:
+            if tonemapped:
+                write_png(args.output, tonemap(film, args.exposure))
+            else:
+                write_exr(args.output, film)
+    if rank == 0:
+        print(args.output)
     g.close()
     return 0
 

@@ -446,13 +446,20 @@ const void* etxb_scene_file_table(const etxb_scene_file* sf, const char* name, u
  * ETXB_INTEGRATOR_PT one iteration = one path per active pixel (CPUPathTracingImpl::execute_range) followed by update()'s
  * film.estimate_noise_levels(current_iteration, samples, noise_threshold); a pixel the estimate marks converged is skipped from
  * then on (Film::active_pixel).  The coarse preview (etxb_set_film_pixel_size) applies to it as to the VCM: a path whose chosen pixel has
- * converged is skipped with its whole block. */
+ * converged is skipped with its whole block.
+ * Pixel tiles: on a context with a communicator (etxb_comm_init, either order) each rank traces its own tiles and the noise estimate is
+ * exchanged inside etxb_enqueue_iteration (see the pixel-tile section below); the ranks then render the one-GPU frame and history.
+ * etxb_set_integrator(ETXB_INTEGRATOR_PT) is refused (ETXB_ERR_UNSUPPORTED, before any collective) on a context with a pixel partition but no
+ * communicator and on the lanes of a group in pixel-tile mode (etxb_group_comm_init with world >= 2), whose lanes would each keep their own
+ * per-pixel history. */
 #define ETXB_INTEGRATOR_VCM 0u
 #define ETXB_INTEGRATOR_PT 1u
 /* PTOptions (path_tracing_shared.hxx:8-14); the reference's option ids are "nee", "direct", "mis", "bn" (path_tracing.cxx:36-39) */
 typedef struct etxb_pt_options {
   uint32_t nee, direct, mis, blue_noise; /* all default 1 */
 } etxb_pt_options;
+/* On a context with a communicator the status is global: pixels_processed is summed over the ranks at the end of every iteration,
+ * active_pixels and noise_level at every estimate — so every rank's update loop ends at the same iteration. */
 typedef struct etxb_pt_status {
   uint32_t pixels_processed; /* CPUPathTracingImpl::pixels_processed of the last finished iteration; 0 => the reference stops the run (:90-92) */
   uint32_t active_pixels;    /* Film::active_pixel_count (film.cxx:430): pixel count after a clear, pixels converged in the last estimate after one */
@@ -526,6 +533,13 @@ int etxb_debug_build_trees(etxb_ctx* ctx, const float* positions, uint32_t verte
  * out_variance may be null.  out_variance receives the smoothed per-pixel variance of the mean.  ETXB_ERR_NOT_READY where a count is below 2. */
 int etxb_debug_denoise(etxb_ctx* ctx, const float* color, const float* camera, const float* half, const uint32_t* counts, const float* normals,
                        const float* albedo, uint32_t width, uint32_t height, float* out, float* out_variance);
+/* The path tracer's noise estimate (etxb_enqueue_iteration's Film::estimate_noise_levels) on host arrays, as `world` pixel-tile ranks run it:
+ * each rank's view holds its own pixels and zeros elsewhere, the level pass runs per rank, the masks are summed (the all-reduce), the dilation
+ * runs per rank and the owned pixels are composed.  world = 1 is the one-GPU estimate.  camera / adaptive = float[4 * width * height] and
+ * info_in / info_out = uint32[width * height] (ETXB_BUF_PIXEL_INFO words), in storage order; error_out = float[width * height]
+ * (ETXB_BUF_PIXEL_ERROR, zero where a pixel was not evaluated); stats_out = uint32[2]: the converged count and the bits of the float error sum. */
+int etxb_debug_noise_estimate(etxb_ctx* ctx, uint32_t width, uint32_t height, uint32_t world, float threshold, const float* camera, const float* adaptive,
+                              const uint32_t* info_in, uint32_t* info_out, float* error_out, uint32_t* stats_out);
 /* Sampler / spectral KATs evaluated on the device (sampler.hxx:54,66; spectrum.hxx:219,234). */
 int etxb_debug_sampler(etxb_ctx* ctx, const uint32_t* a, const uint32_t* b, uint32_t count, uint32_t draws, uint32_t* out_seed, float* out_values);
 int etxb_debug_math(etxb_ctx* ctx, uint32_t fn, const float* x, const float* y, uint32_t count, float* out);
@@ -734,12 +748,20 @@ int etxb_group_read_film(etxb_group* group, uint32_t layer, float* dst_rgba, uin
  * (etxb_set_partition's rule) and runs the light and camera subpaths of its pixels; what is global is exchanged INSIDE etxb_enqueue_iteration:
  * all-reduce of the per-iteration light image (light-tracing splats land on any pixel, vcm_cpu.cxx:147-154 -> film.cxx:332-343) and an
  * all-gather of the photon records (merging queries every light path's vertices, vcm_cpu.cxx:219-221).  The host only distributes the NCCL id
- * (any transport: MPI, a file, torch.distributed) — rank 0 calls etxb_comm_unique_id, every rank calls etxb_comm_init with those bytes. */
+ * (any transport: MPI, a file, torch.distributed) — rank 0 calls etxb_comm_unique_id, every rank calls etxb_comm_init with those bytes.
+ * The path tracer (ETXB_INTEGRATOR_PT) runs over the same tiles.  Its noise estimate (Film::estimate_noise_levels) is the one global step: each
+ * rank packs a mask of its pixels that have not converged (one bit per pixel, ceil(W / 32) words per row), the ranks all-reduce the masks
+ * with the converged count, the error sum and pixels_processed, and each rank dilates the whole mask onto its own pixels.  Every other
+ * iteration only pixels_processed is all-reduced (4 bytes).  The collectives of an iteration follow from its index, the noise threshold and
+ * Scene::samples, so these, and the options, must be equal on every rank; a rank whose tiles have all converged traces no path but keeps
+ * joining the collectives until etxb_pt_status says the frame is done. */
 #define ETXB_COMM_ID_BYTES 128
 int etxb_comm_unique_id(void* out_id, uint64_t bytes);
 int etxb_comm_init(etxb_ctx* ctx, uint32_t world, uint32_t rank, const void* id, uint64_t bytes); /* collective */
 int etxb_comm_world(const etxb_ctx* ctx, uint32_t* world, uint32_t* rank);
-/* Collective: sums the disjoint camera tiles on rank 0 (ncclReduce of the float4 film); dst_rgba is written on rank 0 only. */
+/* Collective: sums the disjoint tiles of `layer` on rank 0 (ncclReduce of the float4 layer); dst_rgba is written on rank 0 only, with
+ * etxb_read_film's read-out.  Layers: Result, Camera, Light (complete on every rank), and the path tracer's Normals, Albedo and CameraAdaptive.
+ * ETXB_ERR_INVALID_ARGUMENT for LightIteration and Denoised. */
 int etxb_comm_reduce_film(etxb_ctx* ctx, uint32_t layer, float* dst_rgba, uint64_t dst_bytes);
 /* The same with several iterations in flight per GPU: ids = (lanes + 1) x ETXB_COMM_ID_BYTES (one communicator per lane + one for the frame
  * reduce); lane l renders the iteration ordinals l, l + lanes, ... on every rank.  ETXB_ERR_INVALID_ARGUMENT, before any collective, on a group
