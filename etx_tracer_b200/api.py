@@ -131,6 +131,7 @@ def load_library(flavor="fast"):
     lib.etxb_debug_bsdf_sample.argtypes = [vp, vp, u32, u32, vp]
     lib.etxb_debug_emitter.argtypes = [vp, vp, u32, u32, vp]
     lib.etxb_debug_medium.argtypes = [vp, vp, u32, u32, vp]
+    lib.etxb_debug_subsurface.argtypes = [vp, vp, u32, u32, vp]
     lib.etxb_debug_set_thresholds.argtypes = [vp, vp]
     lib.etxb_debug_get_branch_counts.argtypes = [vp, vp]
     lib.etxb_debug_merge.argtypes = [vp, vp, u32, vp, vp, u32, vp, vp]
@@ -602,6 +603,14 @@ class GPUVCM:
         queries = np.ascontiguousarray(queries, dtype=S.MEDIUM_QUERY)
         out = np.zeros((queries.shape[0], int(repetitions)), dtype=S.MEDIUM_RESULT)
         self._check(self.lib.etxb_debug_medium(self.h, _p(queries), queries.shape[0], int(repetitions), _p(out)))
+        return out
+
+    def debug_subsurface(self, queries, repetitions=1):
+        """The subsurface routines for S.SUBSURFACE_QUERY records on the uploaded scene, repetition r of each query on the sampler (seed, r);
+        returns S.SUBSURFACE_RESULT records shaped (n, repetitions), laid out as etxb_debug_subsurface documents (include/etx_b200.h)."""
+        queries = np.ascontiguousarray(queries, dtype=S.SUBSURFACE_QUERY)
+        out = np.zeros((queries.shape[0], int(repetitions)), dtype=S.SUBSURFACE_RESULT)
+        self._check(self.lib.etxb_debug_subsurface(self.h, _p(queries), queries.shape[0], int(repetitions), _p(out)))
         return out
 
     def debug_thresholds(self, **fields):

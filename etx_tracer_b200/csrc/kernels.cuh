@@ -1927,6 +1927,96 @@ __global__ void k_debug_medium(const __grid_constant__ DeviceScene sc, const etx
   out[t] = o;
 }
 
+// one thread per (etxb_subsurface_query, repetition): the subsurface routines of dsss.cuh as the bounces call them; ops and record layout
+// in include/etx_b200.h
+static_assert(sizeof(etxb_subsurface_query) == 128u && sizeof(etxb_subsurface_probe) == 96u && sizeof(etxb_subsurface_hit) == 64u &&
+                sizeof(etxb_subsurface_result) == 1920u, "etxb_subsurface_query / etxb_subsurface_result layout");
+template <bool SP>
+__global__ void k_debug_subsurface(const __grid_constant__ DeviceScene sc, const etxb_subsurface_query* queries, uint32_t count, uint32_t reps,
+                                   etxb_subsurface_result* out) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= count * reps) return;
+  const uint32_t i = t / reps, r = t % reps;
+  const etxb_subsurface_query& q = queries[i];
+  const float wavelength = SP ? q.wavelength : -1.0f;
+  const V3 origin = {q.origin[0], q.origin[1], q.origin[2]}, direction = {q.dir[0], q.dir[1], q.dir[2]};
+  const auto put = [](float* dst, V3 a) {
+    dst[0] = a.x;
+    dst[1] = a.y;
+    dst[2] = a.z;
+  };
+  const auto put_probe = [&put](etxb_subsurface_probe& dst, const SSSample& s) {
+    put(dst.o, s.ray_o);
+    put(dst.d, s.ray_d);
+    dst.min_t = s.ray_min_t;
+    dst.max_t = s.ray_max_t;
+    put(dst.u, s.u);
+    put(dst.v, s.v);
+    put(dst.w, s.w);
+    put(dst.basis_prob, s.basis_prob);
+    dst.sampled_radius = s.sampled_radius;
+  };
+  STATS_DECL;  // as every other caller: the count build's traversals are compiled for a non-null stats pointer
+  etxb_subsurface_result& o = out[t];
+  Smp smp;
+  smp.init(q.seed, r);
+  o.seed_start = smp.seed;
+  if ((q.op == ETXB_SUBSURFACE_TRACE_MATERIAL) || (q.op == ETXB_SUBSURFACE_CONTINUOUS_TRACE)) {
+    HitRec h[kSSPerDirection];
+    if (q.op == ETXB_SUBSURFACE_TRACE_MATERIAL) {
+      h[0] = trace_material(sc, origin, direction, q.t_min, q.t_max, q.material, smp, stats);
+      o.count = (h[0].tri != kInvalidIndex) ? 1u : 0u;
+    } else {
+      o.count = continuous_trace(sc, origin, direction, q.t_min, q.t_max, q.material, h, q.max_count, smp, stats);
+    }
+    for (uint32_t k = 0; k < ((q.op == ETXB_SUBSURFACE_TRACE_MATERIAL) ? 1u : o.count); ++k) {
+      o.hits[k].u = h[k].u;
+      o.hits[k].v = h[k].v;
+      o.hits[k].t = h[k].t;
+      o.hits[k].tri = h[k].tri;
+    }
+  } else if (q.op == ETXB_SUBSURFACE_REMAP) {
+    for (uint32_t k = 0; k < 3u; ++k) remap_channel(q.color[k], q.distances[k], o.albedo[k], o.extinction[k], o.scattering[k]);
+  } else {
+    const Isect in = make_intersection(sc, direction, q.triangle, q.u, q.v, 0.0f);
+    const etxb_material& mat = sc.materials[in.material_index];
+    if (q.op == ETXB_SUBSURFACE_PROFILE) {
+      o.s_r = sample_s_r(q.rnd);
+      put(o.eval, ss_evaluate<SP>(sc, wavelength, in.tex, mat, q.radius).as_v3());
+      const SSSample s = ss_sample<SP>(sc, wavelength, in, mat, q.direction, smp);
+      put_probe(o.probes[0], s);
+      o.geometric_weight = ss_geometric_weight({q.normal[0], q.normal[1], q.normal[2]}, s);
+    } else {
+      if (mat.subsurface.cls == 2u) {  // the gather's three probes are its first draws
+        Smp probe_smp = smp;
+        for (uint32_t d = 0; d < kSSDirections; ++d) put_probe(o.probes[d], ss_sample<SP>(sc, wavelength, in, mat, d, probe_smp));
+      }
+      SSGather<SP> g;
+      uint32_t rays = 0;
+      o.flag = ss_gather<SP>(sc, wavelength, in, smp, g, stats, rays) ? 1u : 0u;
+      o.rays = rays;
+      if (o.flag) {
+        o.count = g.count;
+        o.selected = g.selected;
+        o.selected_sample_weight = g.selected_sample_weight;
+        o.total_weight = g.total_weight;
+        for (uint32_t k = 0; k < g.count; ++k) {
+          const Isect e = ss_exit_intersection<SP>(sc, g, k, sc.subsurface_exit_material);
+          o.hits[k].u = g.hits[k].u;
+          o.hits[k].v = g.hits[k].v;
+          o.hits[k].t = g.hits[k].t;
+          o.hits[k].tri = g.hits[k].tri;
+          put(o.hits[k].w_i, e.w_i);
+          put(o.hits[k].weight, g.weights[k].as_v3());
+          put(o.hits[k].pos, e.pos);
+          put(o.hits[k].nrm, e.nrm);
+        }
+      }
+    }
+  }
+  o.seed_end = smp.seed;
+}
+
 // etxb_debug_merge: query i becomes path i of a one-bounce queue, staged in the columns the gather kernels read (hit record, ray
 // direction, throughput, MIS terms, sampler, depth, medium, wavelength), with the merge key k_camera_shade would give it.  Writes the
 // staged camera vertex's position and normal to pos_nrm[2 i], [2 i + 1], and i to queue slot i.

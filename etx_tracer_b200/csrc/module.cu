@@ -3105,6 +3105,70 @@ int etxb_debug_medium(etxb_ctx* ctx, const etxb_medium_query* queries, uint32_t 
   return ETXB_OK;
 }
 
+// Test hook: the subsurface routines of dsss.cuh, query by query and repetition by repetition (layout and ops in include/etx_b200.h).
+// Every loop they run is bounded (a traversal of the tree, at most 1024 random-walk steps), so the checks are on indices and finite inputs.
+int etxb_debug_subsurface(etxb_ctx* ctx, const etxb_subsurface_query* queries, uint32_t count, uint32_t repetitions, etxb_subsurface_result* out) {
+  if (!ctx || !queries || !out || (repetitions == 0)) return ETXB_ERR_INVALID_ARGUMENT;
+  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
+  if (count == 0) return ETXB_OK;
+  if (uint64_t(count) * repetitions > 0x7fffffffull) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "%u queries x %u repetitions exceed 2^31 samples", count, repetitions);
+  cudaSetDevice(ctx->device);
+  std::vector<etxb_material> mats(ctx->materials.count);
+  std::vector<DTriangle> tris(ctx->triangles.count);
+  if (!mats.empty()) CUDA_OK(ctx, cudaMemcpy(mats.data(), ctx->materials.ptr, mats.size() * sizeof(etxb_material), cudaMemcpyDeviceToHost));
+  if (!tris.empty()) CUDA_OK(ctx, cudaMemcpy(tris.data(), ctx->triangles.ptr, tris.size() * sizeof(DTriangle), cudaMemcpyDeviceToHost));
+  const auto finite = [](const float* v, int n) {
+    for (int k = 0; k < n; ++k)
+      if (!std::isfinite(v[k])) return false;
+    return true;
+  };
+  for (uint32_t i = 0; i < count; ++i) {
+    const etxb_subsurface_query& q = queries[i];
+    if (q.op > ETXB_SUBSURFACE_GATHER) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: op must be 0 to 4", i);
+    if (ctx->spectral && !std::isfinite(q.wavelength)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: non-finite wavelength", i);
+    if (q.op == ETXB_SUBSURFACE_REMAP) {
+      if (!finite(q.color, 3) || !finite(q.distances, 3)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: non-finite color or distance", i);
+      continue;
+    }
+    const float* d = q.dir;
+    if (!finite(d, 3) || ((d[0] == 0.0f) && (d[1] == 0.0f) && (d[2] == 0.0f)))
+      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: zero or non-finite direction", i);
+    if (q.op <= ETXB_SUBSURFACE_CONTINUOUS_TRACE) {
+      if ((q.material != ETXB_INVALID_INDEX) && (q.material >= mats.size())) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: material index out of range", i);
+      if (!finite(q.origin, 3) || !std::isfinite(q.t_min) || !std::isfinite(q.t_max))
+        return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: non-finite origin or ray interval", i);
+      if ((q.op == ETXB_SUBSURFACE_CONTINUOUS_TRACE) && ((q.max_count == 0) || (q.max_count > 8u)))
+        return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: max_count must be 1 to 8", i);
+      continue;
+    }
+    if (q.triangle >= tris.size()) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: triangle index out of range", i);
+    if (!std::isfinite(q.u) || !std::isfinite(q.v)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: non-finite barycentric coordinates", i);
+    if (q.op == ETXB_SUBSURFACE_PROFILE) {
+      if (q.direction > 2u) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: probe direction must be 0 to 2", i);
+      if (!std::isfinite(q.rnd) || !std::isfinite(q.radius) || !finite(q.normal, 3))
+        return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: non-finite rnd, radius or normal", i);
+    } else if (mats[tris[q.triangle].material_index].subsurface.cls == 0u) {
+      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: gather on a material without subsurface scattering", i);
+    }
+  }
+  const uint32_t total = count * repetitions;
+  DevBuf<etxb_subsurface_query> d_queries;
+  DevBuf<etxb_subsurface_result> d_out;
+  if (int rc = upload(ctx, d_queries, queries, count)) return rc;
+  CUDA_OK(ctx, d_out.alloc(total));
+  CUDA_OK(ctx, cudaMemsetAsync(d_out.ptr, 0, d_out.bytes(), ctx->stream));  // the kernel writes only the fields its op names
+  if (ctx->spectral) {
+    k_debug_subsurface<true><<<blocks_for(total, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
+  } else {
+    k_debug_subsurface<false><<<blocks_for(total, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
+  }
+  ctx->kernel_launches += 1;
+  CUDA_OK(ctx, cudaGetLastError());
+  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+  CUDA_OK(ctx, cudaMemcpy(out, d_out.ptr, d_out.bytes(), cudaMemcpyDeviceToHost));
+  return ETXB_OK;
+}
+
 // Test hook: the queue sizes from which the passes take their large-queue branches (NULL = the defaults), and what ran since etxb_begin
 int etxb_debug_set_thresholds(etxb_ctx* ctx, const etxb_debug_thresholds* thresholds) {
   if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;

@@ -159,6 +159,8 @@ class SceneData:
             spd["entries"]["power"][0] = (spd["entries"]["power"][0] * scale).astype(f32)
             spd["integrated"][0] = (spd["integrated"][0] * scale).astype(f32)
             m["subsurface"]["spectrum_index"] = self.add_spectrum(spd)
+            # an image index scales the distances per texel (apply_image of the SubsurfaceMaterial)
+            m["subsurface"]["image_index"] = subsurface.get("image", S.INVALID)
         self.materials.append(m)
         self.material_names[name] = len(self.materials) - 1
         return len(self.materials) - 1

@@ -134,6 +134,18 @@ MEDIUM_QUERY = np.dtype([("op", u4), ("medium", u4), ("seed", u4), ("reserved0",
 MEDIUM_RESULT = np.dtype([("value", f4, 3), ("pos", f4, 3), ("dir", f4, 3), ("t_min", f4), ("t_max", f4), ("t", f4), ("flag", u4),
                           ("seed_start", u4), ("seed_end", u4), ("reserved", u4)])
 MEDIUM_BOUNDS, MEDIUM_DENSITY, MEDIUM_TRANSMITTANCE, MEDIUM_SAMPLE, MEDIUM_PHASE, MEDIUM_SEGMENT = 0, 1, 2, 3, 4, 5
+# etxb_subsurface_query (128 B) and the per-sample record etxb_debug_subsurface / oracle_subsurface return (include/etx_b200.h)
+SUBSURFACE_QUERY = np.dtype([("op", u4), ("seed", u4), ("material", u4), ("triangle", u4), ("max_count", u4), ("direction", u4), ("wavelength", f4),
+                             ("u", f4), ("v", f4), ("origin", f4, 3), ("dir", f4, 3), ("t_min", f4), ("t_max", f4), ("color", f4, 3),
+                             ("distances", f4, 3), ("rnd", f4), ("radius", f4), ("normal", f4, 3), ("reserved", u4, 4)])
+SUBSURFACE_PROBE = np.dtype([("o", f4, 3), ("d", f4, 3), ("min_t", f4), ("max_t", f4), ("u", f4, 3), ("v", f4, 3), ("w", f4, 3), ("basis_prob", f4, 3),
+                             ("sampled_radius", f4), ("reserved", u4, 3)])
+SUBSURFACE_HIT = np.dtype([("u", f4), ("v", f4), ("t", f4), ("tri", u4), ("w_i", f4, 3), ("weight", f4, 3), ("pos", f4, 3), ("nrm", f4, 3)])
+SUBSURFACE_RESULT = np.dtype([("flag", u4), ("count", u4), ("selected", u4), ("rays", u4), ("seed_start", u4), ("seed_end", u4),
+                              ("selected_sample_weight", f4), ("total_weight", f4), ("albedo", f4, 3), ("extinction", f4, 3), ("scattering", f4, 3),
+                              ("s_r", f4), ("eval", f4, 3), ("geometric_weight", f4), ("reserved", u4, 2), ("probes", SUBSURFACE_PROBE, 3),
+                              ("hits", SUBSURFACE_HIT, 24)])
+SUBSURFACE_TRACE_MATERIAL, SUBSURFACE_CONTINUOUS_TRACE, SUBSURFACE_REMAP, SUBSURFACE_PROFILE, SUBSURFACE_GATHER = 0, 1, 2, 3, 4
 BSDF_DIFFUSE, BSDF_REFLECTION, BSDF_TRANSMISSION, BSDF_MEDIUM_CHANGED, BSDF_DELTA = 1, 2, 4, 8, 16
 # etxb_debug_thresholds / etxb_debug_branch_counts (include/etx_b200.h): a threshold of 0 always takes the large-queue branch, NEVER never does
 DEBUG_THRESHOLDS = np.dtype([("merge_sort_min_queries", u4), ("merge_min_warps_per_sm", u4), ("tail_queue", u4), ("sort_queue_min", u4), ("merge_qpw", u4)])
@@ -159,6 +171,8 @@ EXPECTED_SIZES = {
     "SAMPLE_QUERY": (SAMPLE_QUERY, 96), "SAMPLE_RESULT": (SAMPLE_RESULT, 48),
     "EMITTER_QUERY": (EMITTER_QUERY, 80), "EMITTER_RESULT": (EMITTER_RESULT, 104),
     "MEDIUM_QUERY": (MEDIUM_QUERY, 96), "MEDIUM_RESULT": (MEDIUM_RESULT, 64),
+    "SUBSURFACE_QUERY": (SUBSURFACE_QUERY, 128), "SUBSURFACE_PROBE": (SUBSURFACE_PROBE, 96), "SUBSURFACE_HIT": (SUBSURFACE_HIT, 64),
+    "SUBSURFACE_RESULT": (SUBSURFACE_RESULT, 1920),
     "LIGHT_VERTEX_REC": (LIGHT_VERTEX_REC, 96), "MERGE_QUERY": (MERGE_QUERY, 64), "MERGE_RESULT": (MERGE_RESULT, 48), "MERGE_GRID": (MERGE_GRID, 64),
 }
 for _name, (_dt, _size) in EXPECTED_SIZES.items():

@@ -663,6 +663,63 @@ typedef struct etxb_medium_result {
   uint32_t flag, seed_start, seed_end, reserved;
 } etxb_medium_result;
 int etxb_debug_medium(etxb_ctx* ctx, const etxb_medium_query* queries, uint32_t count, uint32_t repetitions, etxb_medium_result* out);
+/* Subsurface query (dsss.cuh, as the bounces call it) on the uploaded scene.  One query is 128 bytes: the op, a sampler seed, a material
+ * index, a triangle index, a hit-buffer size max_count, a probe direction (0 to 2), the wavelength (ignored in RGB scenes), barycentric
+ * coordinates u, v on the triangle, a ray (origin, direction, t_min, t_max), a color and scattering distances, a random number rnd, a
+ * radius and a normal.  The ops:
+ *   0 trace_material    trace_material(origin, direction, t_min, t_max, material; 0xffffffff = any material): hits[0], count 0 or 1
+ *   1 continuous_trace  continuous_trace(the same, max_count): count and hits[0, count) in buffer order
+ *   2 remap             remap_channel(color[k], distances[k]) for k = 0, 1, 2: albedo, extinction, scattering
+ *   3 profile           at the entry make_intersection(direction, triangle, u, v): s_r = sample_s_r(rnd), eval = ss_evaluate(radius)
+ *                       at the entry's texture coordinates, probes[0] = ss_sample(probe direction) on the sampler (three draws, one when
+ *                       its channel's distance is 0), geometric_weight = ss_geometric_weight(normal, probes[0])
+ *   4 gather            ss_gather at the entry make_intersection(direction, triangle, u, v) (its material is the triangle's): flag (the
+ *                       return), count, selected, selected_sample_weight, total_weight, rays, per exit hits[i] with the w_i, weight, pos
+ *                       and nrm of ss_exit_intersection; for a Christensen-Burley material, probes[0..2] are the gather's three samples
+ * Every op runs on the sampler Smp::init(seed, r) of repetition r.  The hook refuses, before any launch, an op past 4, a material index
+ * past the scene's count (ops 0 and 1; 0xffffffff is any material), a triangle index past the scene's count (ops 3 and 4), a gather on a
+ * triangle whose material has no subsurface class, a max_count of 0 or above 8 (op 1), a non-finite input the op reads, a zero
+ * direction (ops 0, 1, 3 and 4), and count x repetitions past 2^31. */
+typedef struct etxb_subsurface_query {
+  uint32_t op, seed, material, triangle, max_count, direction;
+  float wavelength, u, v;
+  float origin[3], dir[3];
+  float t_min, t_max;
+  float color[3], distances[3];
+  float rnd, radius;
+  float normal[3];
+  uint32_t reserved[4];
+} etxb_subsurface_query;
+#define ETXB_SUBSURFACE_TRACE_MATERIAL 0u
+#define ETXB_SUBSURFACE_CONTINUOUS_TRACE 1u
+#define ETXB_SUBSURFACE_REMAP 2u
+#define ETXB_SUBSURFACE_PROFILE 3u
+#define ETXB_SUBSURFACE_GATHER 4u
+/* One probe of a Christensen-Burley gather (96 bytes): the ray (origin, direction, t_min, t_max), the basis u, v, w, basis_prob and
+ * sampled_radius; an empty probe is origin 0, direction 0, [kRayEpsilon, kMaxFloat] with everything else 0. */
+typedef struct etxb_subsurface_probe {
+  float o[3], d[3], min_t, max_t, u[3], v[3], w[3], basis_prob[3], sampled_radius;
+  uint32_t reserved[3];
+} etxb_subsurface_probe;
+/* One hit (64 bytes): barycentric u, v, t and triangle (0xffffffff = none); for a gather exit also w_i, weight (rgb; a spectral value
+ * fills all three), and the pos and nrm of ss_exit_intersection. */
+typedef struct etxb_subsurface_hit {
+  float u, v, t;
+  uint32_t tri;
+  float w_i[3], weight[3], pos[3], nrm[3];
+} etxb_subsurface_hit;
+/* One 1920-byte record per (query, repetition), repetition-minor: the fields each op names above, and the sampler state Smp::init(seed,
+ * r) left and the state after the op, for every op.  Fields an op does not name are 0. */
+typedef struct etxb_subsurface_result {
+  uint32_t flag, count, selected, rays, seed_start, seed_end;
+  float selected_sample_weight, total_weight;
+  float albedo[3], extinction[3], scattering[3];
+  float s_r, eval[3], geometric_weight;
+  uint32_t reserved[2];
+  etxb_subsurface_probe probes[3];
+  etxb_subsurface_hit hits[24];
+} etxb_subsurface_result;
+int etxb_debug_subsurface(etxb_ctx* ctx, const etxb_subsurface_query* queries, uint32_t count, uint32_t repetitions, etxb_subsurface_result* out);
 /* Queue sizes from which the light and camera passes take their large-queue branches.  A pass of a long queue runs the same paths as
  * one of a short queue, in another order; these let a small film take either branch.  Each field is a queue size: 0 = always the
  * large-queue branch, 0xffffffff = never.

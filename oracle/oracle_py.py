@@ -52,6 +52,8 @@ def load(flavor="parity"):
         lib.oracle_emitter.argtypes = [vp, vp, u32, u32, u32, vp]
     if hasattr(lib, "oracle_medium"):
         lib.oracle_medium.argtypes = [vp, vp, u32, u32, u32, vp]
+    if hasattr(lib, "oracle_subsurface"):
+        lib.oracle_subsurface.argtypes = [vp, vp, u32, u32, u32, vp]
     if hasattr(lib, "oracle_merge"):
         lib.oracle_merge.argtypes = [vp, vp, u32, vp, vp, u32, u32, u32, vp, vp]
     lib.oracle_sampler.argtypes = [vp, vp, u32, u32, vp, vp]
@@ -93,6 +95,11 @@ def has_emitter(flavor="parity"):
 def has_medium(flavor="parity"):
     """Whether the built oracle exports oracle_medium."""
     return hasattr(load(flavor), "oracle_medium")
+
+
+def has_subsurface(flavor="parity"):
+    """Whether the built oracle exports oracle_subsurface."""
+    return hasattr(load(flavor), "oracle_subsurface")
 
 
 def has_merge(flavor="parity"):
@@ -294,6 +301,14 @@ class Oracle:
         queries = np.ascontiguousarray(queries, dtype=self.S.MEDIUM_QUERY)
         out = np.zeros((queries.shape[0], int(repetitions)), dtype=self.S.MEDIUM_RESULT)
         self.lib.oracle_medium(self.h, _p(queries), queries.shape[0], int(repetitions), int(threads or os.cpu_count() or 1), _p(out))
+        return out
+
+    def subsurface(self, queries, repetitions=1, threads=None):
+        """The reference's subsurface routines for S.SUBSURFACE_QUERY records, repetition r of each query on Sampler(seed, r);
+        S.SUBSURFACE_RESULT records shaped (n, repetitions), in the layout of GPUVCM.debug_subsurface."""
+        queries = np.ascontiguousarray(queries, dtype=self.S.SUBSURFACE_QUERY)
+        out = np.zeros((queries.shape[0], int(repetitions)), dtype=self.S.SUBSURFACE_RESULT)
+        self.lib.oracle_subsurface(self.h, _p(queries), queries.shape[0], int(repetitions), int(threads or os.cpu_count() or 1), _p(out))
         return out
 
     def merge(self, records, light_wavelengths, queries, repetitions=1, threads=None):

@@ -143,8 +143,12 @@ bool Raytracing::trace(const Scene& scene, const Ray& r, Intersection& result_in
   return true;
 }
 
+// the rays trace_material and continuous_trace have traced on this thread: oracle_subsurface reports a gather's count as the device does
+static thread_local uint32_t g_material_rays = 0;
+
 // rt.cxx:327-371 — closest hit restricted to one material
 bool Raytracing::trace_material(const Scene& scene, const Ray& r, const uint32_t material_id, Intersection& result_intersection, Sampler& smp) const {
+  g_material_rays += 1;
   IntersectionBase best = {{}, kInvalidIndex, 0.0f};
   auto visit = [&](uint32_t triangle_index, float u, float v, float t) -> int {
     const auto& tri = scene.triangles[triangle_index];
@@ -167,6 +171,7 @@ bool Raytracing::trace_material(const Scene& scene, const Ray& r, const uint32_t
 
 // rt.cxx:373-426 — collect up to N hits along the ray
 uint32_t Raytracing::continuous_trace(const Scene& scene, const Ray& r, const ContinousTraceOptions& options, Sampler& smp) const {
+  g_material_rays += 1;
   uint32_t count = 0;
   auto visit = [&](uint32_t triangle_index, float u, float v, float t) -> int {
     const auto& tri = scene.triangles[triangle_index];
@@ -1271,6 +1276,102 @@ void oracle_medium(void* h, const etxb_medium_query* queries, uint32_t count, ui
       }
       dst.seed_end = smp.seed;
       out[t] = dst;
+    }
+  });
+}
+
+// The reference's own subsurface routines (scene_bssrdf_subsurface.hxx and subsurface::gather of path_tracing_shared.hxx, compiled in
+// place) for etxb_subsurface_query records (include/etx_b200.h), with Raytracing::trace_material and continuous_trace above for ops 0 and
+// 1.  Entries are make_intersection(scene, dir, {{u, v}, triangle, 0}), as etxb_debug_subsurface builds them.  One etxb_subsurface_result
+// per (query, repetition r) on Sampler(seed, r).  The caller keeps to the hook's checks, except that a zero direction is traced as given.
+static_assert(sizeof(etxb_subsurface_query) == 128);
+static_assert(sizeof(etxb_subsurface_result) == 1920);
+void oracle_subsurface(void* h, const etxb_subsurface_query* queries, uint32_t count, uint32_t repetitions, uint32_t threads, etxb_subsurface_result* out) {
+  auto* o = static_cast<Oracle*>(h);
+  const Scene& scene = o->scene;
+  parallel_ranges(count * repetitions, threads, [&](uint32_t begin, uint32_t end, uint32_t, uint32_t) {
+    for (uint32_t t = begin; t < end; ++t) {
+      const etxb_subsurface_query& q = queries[t / repetitions];
+      const SpectralQuery spect = scene.spectral() ? SpectralQuery{q.wavelength, SpectralQuery::Spectral} : SpectralQuery::sample();
+      const float3 origin = {q.origin[0], q.origin[1], q.origin[2]}, direction = {q.dir[0], q.dir[1], q.dir[2]};
+      const auto put = [](float* d, const float3& a) {
+        d[0] = a.x;
+        d[1] = a.y;
+        d[2] = a.z;
+      };
+      const auto put_spectral = [&](float* d, const SpectralResponse& s) { put(d, s.spectral() ? float3{s.value, s.value, s.value} : s.integrated); };
+      const auto put_probe = [&](etxb_subsurface_probe& d, const subsurface::Sample& s) {
+        put(d.o, s.ray.o);
+        put(d.d, s.ray.d);
+        d.min_t = s.ray.min_t;
+        d.max_t = s.ray.max_t;
+        put(d.u, s.u);
+        put(d.v, s.v);
+        put(d.w, s.w);
+        put(d.basis_prob, s.basis_prob);
+        d.sampled_radius = s.sampled_radius;
+      };
+      etxb_subsurface_result& dst = out[t];
+      dst = {};
+      Sampler smp(q.seed, t % repetitions);
+      dst.seed_start = smp.seed;
+      const Ray ray = {origin, direction, q.t_min, q.t_max};
+      if (q.op == ETXB_SUBSURFACE_TRACE_MATERIAL) {
+        Intersection i;
+        const bool found = o->rt.trace_material(scene, ray, q.material, i, smp);
+        dst.count = found ? 1u : 0u;
+        dst.hits[0].tri = kInvalidIndex;
+        if (found) {
+          dst.hits[0] = {i.barycentric.y, i.barycentric.z, i.t, i.triangle_index};
+        }
+      } else if (q.op == ETXB_SUBSURFACE_CONTINUOUS_TRACE) {
+        IntersectionBase buffer[subsurface::kIntersectionsPerDirection] = {};
+        dst.count = o->rt.continuous_trace(scene, ray, ContinousTraceOptions{buffer, q.max_count, q.material}, smp);
+        for (uint32_t k = 0; k < dst.count; ++k)
+          dst.hits[k] = {buffer[k].barycentric.x, buffer[k].barycentric.y, buffer[k].t, buffer[k].triangle_index};
+      } else if (q.op == ETXB_SUBSURFACE_REMAP) {
+        for (uint32_t k = 0; k < 3u; ++k)
+          subsurface::remap_channel(q.color[k], q.distances[k], dst.albedo[k], dst.extinction[k], dst.scattering[k]);
+      } else {
+        const Intersection in = make_intersection(scene, direction, IntersectionBase{{q.u, q.v}, q.triangle, 0.0f});
+        const auto& sss = scene.materials[in.material_index].subsurface;
+        if (q.op == ETXB_SUBSURFACE_PROFILE) {
+          dst.s_r = subsurface::sample_s_r(q.rnd);
+          put_spectral(dst.eval, subsurface::evaluate(spect, scene, in, sss, q.radius));
+          const subsurface::Sample s = subsurface::sample(spect, scene, in, sss, q.direction, smp);
+          put_probe(dst.probes[0], s);
+          dst.geometric_weight = subsurface::geometric_weigth({q.normal[0], q.normal[1], q.normal[2]}, s);
+        } else {
+          if (sss.cls == SubsurfaceMaterial::Class::ChristensenBurley) {  // the gather's three probes are its first draws
+            Sampler probe_smp = smp;
+            for (uint32_t d = 0; d < subsurface::kIntersectionDirections; ++d)
+              put_probe(dst.probes[d], subsurface::sample(spect, scene, in, sss, d, probe_smp));
+          }
+          subsurface::Gather g = {};
+          const uint32_t rays_before = g_material_rays;
+          dst.flag = (subsurface::gather(spect, scene, in, o->rt, smp, g) == subsurface::GatherResult::Succeedded) ? 1u : 0u;
+          dst.rays = g_material_rays - rays_before;
+          if (dst.flag) {
+            dst.count = g.intersection_count;
+            dst.selected = g.selected_intersection;
+            dst.selected_sample_weight = g.selected_sample_weight;
+            dst.total_weight = g.total_weight;
+            for (uint32_t k = 0; k < g.intersection_count; ++k) {
+              const Intersection& e = g.intersections[k];
+              etxb_subsurface_hit& hk = dst.hits[k];
+              hk.u = e.barycentric.y;
+              hk.v = e.barycentric.z;
+              hk.t = e.t;
+              hk.tri = e.triangle_index;
+              put(hk.w_i, e.w_i);
+              put_spectral(hk.weight, g.weights[k]);
+              put(hk.pos, e.pos);
+              put(hk.nrm, e.nrm);
+            }
+          }
+        }
+      }
+      dst.seed_end = smp.seed;
     }
   });
 }
