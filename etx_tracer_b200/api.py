@@ -6,6 +6,7 @@ EtxbError with the module's message when the device path cannot do what was aske
 """
 import ctypes as C
 import os
+import warnings
 
 import numpy as np
 
@@ -53,6 +54,7 @@ def load_library(flavor="fast"):
     lib.etxb_options_file_string.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, u64]
     lib.etxb_mesh_tangents.argtypes = [vp, u64, vp, u64]
     lib.etxb_image_file_read.argtypes = [C.c_char_p, vp, vp, vp, vp, u64, C.c_char_p, u64]
+    lib.etxb_reference_image_file_read.argtypes = [C.c_char_p, vp, vp, vp, u64, C.c_char_p, u64]
     lib.etxb_nvdb_density.argtypes = [C.c_char_p, vp, vp, u64, C.c_char_p, u64]
     for fn in (lib.etxb_scene_file_scene, lib.etxb_scene_file_camera):
         fn.argtypes = [vp]
@@ -112,6 +114,13 @@ def load_library(flavor="fast"):
     lib.etxb_denoise.argtypes = [vp, u32]
     lib.etxb_debug_denoise.argtypes = [vp, vp, vp, vp, vp, vp, vp, u32, u32, vp, vp]
     lib.etxb_debug_noise_estimate.argtypes = [vp, u32, u32, u32, C.c_float, vp, vp, vp, vp, vp, vp]
+    lib.etxb_set_reference_image.argtypes = [vp, vp, u32, u32]
+    lib.etxb_use_film_as_reference.argtypes = [vp, u32]
+    lib.etxb_clear_reference.argtypes = [vp]
+    lib.etxb_read_film_view.argtypes = [vp, u32, vp, vp, u64]
+    lib.etxb_film_error.argtypes = [vp, u32, vp]
+    lib.etxb_debug_film_view.argtypes = [vp, vp, vp, u32, vp, vp]
+    lib.etxb_debug_film_error.argtypes = [vp, vp, vp, u32, u32, vp]
     lib.etxb_save_film.argtypes = [vp, u32, C.c_char_p, u32, C.c_float]
     lib.etxb_write_exr.argtypes = [C.c_char_p, vp, u32, u32]
     lib.etxb_write_png.argtypes = [C.c_char_p, vp, u32, u32]
@@ -166,6 +175,23 @@ def read_image(file_name, flavor="fast"):
     out = np.zeros((h.value, w.value, 4), dtype=np.uint8 if eight.value else np.float32)
     if lib.etxb_image_file_read(os.fsencode(file_name), C.byref(w), C.byref(h), C.byref(eight), _p(out), out.nbytes, err, len(err)) != 0:
         raise EtxbError(-4, err.value.decode(errors="replace"))
+    return out
+
+
+def read_reference_image(file_name, flavor="fast"):
+    """The viewer's reference image from a file (Open Reference Image): (H, W, 4) float32, rows in file order, as the reference's image pool
+    holds it.  A file that cannot be read gives the 1 x 1 white placeholder, with a warning."""
+    lib = load_library(flavor)
+    w, h = C.c_uint32(0), C.c_uint32(0)
+    err = C.create_string_buffer(512)
+    name = os.fsencode(file_name)
+    lib.etxb_reference_image_file_read(name, C.byref(w), C.byref(h), None, 0, err, len(err))
+    out = np.zeros((h.value, w.value, 4), dtype=np.float32)
+    rc = lib.etxb_reference_image_file_read(name, C.byref(w), C.byref(h), _p(out), out.nbytes, err, len(err))
+    if rc != 0:
+        raise EtxbError(rc, f"could not read {file_name}")
+    if err.value:
+        warnings.warn(err.value.decode(errors="replace"))
     return out
 
 
@@ -448,6 +474,54 @@ class GPUVCM:
     def save_image(self, file_name, layer=S.FILM_RESULT, tonemapped=False, exposure=1.0):
         """RTApplication::on_save_image_selected (app.cxx:261-295): the float layer as OpenEXR, or tone-mapped as PNG."""
         self._check(self.lib.etxb_save_film(self.h, layer, os.fsencode(file_name), 1 if tonemapped else 0, C.c_float(exposure)))
+
+    # -- the viewer (DESIGN §14) ----------------------------------------------------------------------------
+    def set_reference(self, rgba):
+        """The viewer's reference image (ImagePool::add_from_data): a float (H, W, 4) array in film storage order, of the film's size."""
+        rgba = np.ascontiguousarray(rgba, dtype=np.float32)
+        if rgba.ndim != 3 or rgba.shape[2] != 4:
+            raise ValueError(f"reference must be (H, W, 4), got {rgba.shape}")
+        self._check(self.lib.etxb_set_reference_image(self.h, _p(rgba), rgba.shape[1], rgba.shape[0]))
+
+    def use_as_reference(self, layer=S.FILM_RESULT):
+        """Use as Reference: the layer as it stands becomes the reference, copied on the device."""
+        self._check(self.lib.etxb_use_film_as_reference(self.h, layer))
+
+    def clear_reference(self):
+        self._check(self.lib.etxb_clear_reference(self.h))
+
+    def view(self, layer=S.FILM_RESULT, view=S.VIEW_TONEMAPPED, options=S.VIEW_OPT_TONEMAPPING | S.VIEW_OPT_SRGB, exposure=1.0, rgba8=False):
+        """One of the viewer's six output views of a layer, computed on the device: (H, W, 4) float32 as the shader returns it, or (rgba8=True)
+        uint8 as an 8-bit window stores it.  The reference views need set_reference() or use_as_reference() first."""
+        v = np.zeros(1, dtype=S.VIEW)
+        v["view"], v["options"], v["exposure"], v["rgba8"] = view, options, exposure, 1 if rgba8 else 0
+        out = np.zeros((self.height, self.width, 4), dtype=np.uint8 if rgba8 else np.float32)
+        self._check(self.lib.etxb_read_film_view(self.h, layer, _p(v), _p(out), out.nbytes))
+        return out
+
+    def film_error(self, layer=S.FILM_RESULT):
+        """The layer's error against the reference, after the iterations in flight (etxb_film_error_info fields as a dict)."""
+        e = np.zeros(1, dtype=S.FILM_ERROR)
+        self._check(self.lib.etxb_film_error(self.h, layer, _p(e)))
+        return {k: v for k, v in _fields(e).items() if k != "pad"}
+
+    def debug_film_view(self, layer_rgba, reference_rgba, view, options, exposure, rgba8=False):
+        """etxb_read_film_view's kernel on host float4 arrays of any shape (..., 4); reference_rgba may be None for views 0-2."""
+        layer_rgba = np.ascontiguousarray(layer_rgba, dtype=np.float32)
+        ref = None if reference_rgba is None else np.ascontiguousarray(reference_rgba, dtype=np.float32)
+        v = np.zeros(1, dtype=S.VIEW)
+        v["view"], v["options"], v["exposure"], v["rgba8"] = view, options, exposure, 1 if rgba8 else 0
+        out = np.zeros(layer_rgba.shape, dtype=np.uint8 if rgba8 else np.float32)
+        self._check(self.lib.etxb_debug_film_view(self.h, _p(layer_rgba), None if ref is None else _p(ref), layer_rgba.size // 4, _p(v), _p(out)))
+        return out
+
+    def debug_film_error(self, layer_rgba, reference_rgba):
+        """etxb_film_error's kernels on host (H, W, 4) arrays."""
+        layer_rgba = np.ascontiguousarray(layer_rgba, dtype=np.float32)
+        ref = np.ascontiguousarray(reference_rgba, dtype=np.float32)
+        e = np.zeros(1, dtype=S.FILM_ERROR)
+        self._check(self.lib.etxb_debug_film_error(self.h, _p(layer_rgba), _p(ref), layer_rgba.shape[1], layer_rgba.shape[0], _p(e)))
+        return {k: v for k, v in _fields(e).items() if k != "pad"}
 
     def denoise(self, layer=S.FILM_RESULT):
         """Film::denoise(layer): filters the Result or Camera layer into S.FILM_DENOISED on the device (DESIGN §13: non-local means with a

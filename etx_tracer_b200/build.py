@@ -11,7 +11,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SOURCES = ["module.cu", "bvh_build.cpp", "bvh_build_device.cu", "film_io.cpp", "scene_loader.cpp"]
-HEADERS = ["bvh.h", "bvh_build.h", "bvh_build_device.h", "dcore.cuh", "dscene.cuh", "dimage.cuh", "dbsdf.cuh", "dclosure.cuh", "dtrace.cuh", "dtrav.cuh", "dwide.cuh", "dmedium.cuh", "dsss.cuh", "dvcm.cuh", "dpt.cuh", "kernels.cuh", "kernels_pt.cuh", "kernels_denoise.cuh", "portable_math.h", "scene_loader_formats.inl", "scene_loader_build.inl", "scene_loader_atmosphere.inl", "scene_loader_tangents.inl", "scene_loader_nvdb.inl", "scene_loader_jpeg.inl",
+HEADERS = ["bvh.h", "bvh_build.h", "bvh_build_device.h", "dcore.cuh", "dscene.cuh", "dimage.cuh", "dbsdf.cuh", "dclosure.cuh", "dtrace.cuh", "dtrav.cuh", "dwide.cuh", "dmedium.cuh", "dsss.cuh", "dvcm.cuh", "dpt.cuh", "kernels.cuh", "kernels_pt.cuh", "kernels_denoise.cuh", "kernels_view.cuh", "portable_math.h", "scene_loader_formats.inl", "scene_loader_build.inl", "scene_loader_atmosphere.inl", "scene_loader_tangents.inl", "scene_loader_nvdb.inl", "scene_loader_jpeg.inl",
            os.path.join("..", "..", "include", "etx_b200.h")]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared", "--expt-relaxed-constexpr", "-Wno-deprecated-gpu-targets"]

@@ -3,7 +3,7 @@
 // tone-mapped layer as an 8-bit PNG (stb_image_write).  Neither third-party writer is used here: an EXR scan-line file without compression
 // and a PNG with stored (uncompressed) deflate blocks are a few dozen lines each and every reader accepts them — tests/test_film_io.py reads
 // them back with the reference's own tinyexr / stb_image (compiled into oracle/_ref/libreference_loader.so) and with zlib.
-// Host-only code: no CUDA here; the tone-mapping itself runs on the device (k_film_tonemap, kernels_pt.cuh) or through etxb_tonemap_rgba8.
+// Host-only code: no CUDA here; the tone-mapping itself runs on the device (k_film_tonemap, kernels_view.cuh) or through etxb_tonemap_rgba8.
 #include <algorithm>
 #include <cmath>
 #include <cstdint>

@@ -344,22 +344,4 @@ __global__ void __launch_bounds__(256) k_film_layer_normals(const float4* normal
   out[i] = make_float4(n.x * 0.5f + 0.5f, n.y * 0.5f + 0.5f, n.z * 0.5f + 0.5f, 1.0f);
 }
 
-// The tone map of the application's LDR export and viewer (app.cxx:268-282, render.cxx:307-320) on the device: 1 - exp(-exposure * c), sRGB
-// transfer curve, 8 bits, alpha 255 — a preview frame leaves the GPU as 4 bytes per pixel instead of 16.
-__global__ void __launch_bounds__(256) k_film_tonemap(const float4* layer, uint32_t* out_rgba8, uint32_t count, float exposure) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= count) return;
-  float4 v = layer[i];
-  float c[3] = {v.x, v.y, v.z};
-  uint32_t packed = 0xff000000u;
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    float tm = 1.0f - expf(-exposure * c[k]);
-    float g = (tm <= 0.0031308f) ? (12.92f * tm) : (1.055f * powf(tm, 1.0f / 2.4f) - 0.055f);
-    g = (g > 0.0f) ? fminf(g, 1.0f) : 0.0f;
-    packed |= uint32_t(255.0f * g) << (8 * k);
-  }
-  out_rgba8[i] = packed;
-}
-
 }  // namespace etxb

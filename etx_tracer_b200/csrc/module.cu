@@ -28,6 +28,7 @@
 #include "kernels.cuh"
 #include "kernels_pt.cuh"
 #include "kernels_denoise.cuh"
+#include "kernels_view.cuh"
 
 using namespace etxb;
 
@@ -246,6 +247,10 @@ struct etxb_ctx {
   DevBuf<float4> denoise_u, denoise_var_raw, denoise_var;   // etxb_denoise scratch: colour with its flags, variance, smoothed variance
   DevBuf<uint32_t> denoise_flag;                            // set by k_denoise_variance where a pixel has fewer than two samples
   DevBuf<uint32_t> film_ldr;                                 // the tone-mapped RGBA8 frame of etxb_read_film_ldr
+  DevBuf<float4> film_view;                                  // the float4 frame of etxb_read_film_view (the RGBA8 one goes to film_ldr)
+  DevBuf<float4> reference;                                  // the viewer's reference image: W x H in storage order, empty when none is set
+  double reference_mean_rgb = 0.0;                           // its mean over pixels and RGB channels, the scale of rel_mse's epsilon
+  DevBuf<ErrorSums> error_blocks;                            // etxb_film_error: one record per block, then the final record
   DevBuf<uint32_t> pt_info;                                  // InternalData (sample count, converged, tmp)
   DevBuf<uint32_t> pt_mask;                                  // the noise estimate's active mask + kNoiseStats (kernels_pt.cuh)
   DevBuf<float> pt_error;
@@ -1666,7 +1671,10 @@ int commit_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, Sce
     allocations += 1;
     return b.alloc(count);
   };
-  if ((ctx->width != cam.film_size[0]) || (ctx->height != cam.film_size[1])) ctx->film_denoised.release();  // Denoised starts over at a new film size
+  if ((ctx->width != cam.film_size[0]) || (ctx->height != cam.film_size[1])) {  // Denoised starts over at a new film size; the reference no longer fits
+    ctx->film_denoised.release();
+    ctx->reference.release();
+  }
   ctx->width = cam.film_size[0];
   ctx->height = cam.film_size[1];
   ctx->path_count = ctx->width * ctx->height;
@@ -1920,6 +1928,93 @@ int run_denoise(etxb_ctx* ctx, const DenoiseInputs& in, float4* out, float4* out
   CUDA_OK(ctx, cudaGetLastError());
   CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
   resolve_timers(ctx);
+  return ETXB_OK;
+}
+
+// ---- the viewer (DESIGN §14) -------------------------------------------------------------------------------------------------------------
+int check_view(etxb_ctx* ctx, const etxb_view* v) {
+  if (!v) return ETXB_ERR_INVALID_ARGUMENT;
+  if ((v->view > ETXB_VIEW_ABSOLUTE) || (v->options & ~(ETXB_VIEW_OPT_TONEMAPPING | ETXB_VIEW_OPT_SRGB | ETXB_VIEW_OPT_SKIP_COLOR_CONVERSION)) ||
+      !std::isfinite(v->exposure) || (v->rgba8 > 1u))
+    return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "film view: view %u (0-5), options 0x%x (bits 0-2), exposure %g (finite), rgba8 %u (0 or 1)", v->view, v->options,
+                double(v->exposure), v->rgba8);
+  return ETXB_OK;
+}
+
+int check_whole_film(etxb_ctx* ctx, const char* what) {
+  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
+  if ((ctx->comm != nullptr) || (ctx->world > 1u)) return fail(ctx, ETXB_ERR_UNSUPPORTED, "%s: the film of a context with pixel tiles holds only its own tiles", what);
+  return ETXB_OK;
+}
+
+bool has_reference(const etxb_ctx* ctx) { return (ctx->reference.ptr != nullptr) && (ctx->reference.count == ctx->path_count); }
+
+// k_film_view over n pixels into the context's own frame buffer, then to `dst`; synchronous
+int run_film_view(etxb_ctx* ctx, const float4* layer, const float4* ref, size_t n, const etxb_view& v, void* dst) {
+  float4* out_f = nullptr;
+  uint32_t* out_rgba8 = nullptr;
+  if (v.rgba8) {
+    if (ctx->film_ldr.count != n) CUDA_OK(ctx, ctx->film_ldr.alloc(n));
+    out_rgba8 = ctx->film_ldr.ptr;
+  } else {
+    if (ctx->film_view.count != n) CUDA_OK(ctx, ctx->film_view.alloc(n));
+    out_f = ctx->film_view.ptr;
+  }
+  k_film_view<<<blocks_for(uint32_t(n), 256), 256, 0, ctx->stream>>>(layer, ref, uint32_t(n), v.view, v.options, v.exposure, out_f, out_rgba8);
+  ctx->kernel_launches += 1;
+  const void* src = v.rgba8 ? static_cast<const void*>(out_rgba8) : static_cast<const void*>(out_f);
+  CUDA_OK(ctx, cudaMemcpyAsync(dst, src, n * (v.rgba8 ? 4u : 16u), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+  return ETXB_OK;
+}
+
+// the two passes of the error reduction over n > 0 pixels (MeanOnly: the reference's r + g + b); synchronous
+template <bool MeanOnly>
+int run_film_error(etxb_ctx* ctx, const float4* layer, const float4* ref, uint32_t n, double eps, ErrorSums* out) {
+  const uint32_t blocks = (n + kErrorChunk - 1u) / kErrorChunk;
+  if (ctx->error_blocks.count < blocks + 1u) CUDA_OK(ctx, ctx->error_blocks.alloc(blocks + 1u));
+  ErrorSums* final_record = ctx->error_blocks.ptr + blocks;
+  k_film_error_blocks<MeanOnly><<<blocks, kErrorThreads, 0, ctx->stream>>>(layer, ref, n, eps, ctx->error_blocks.ptr);
+  k_film_error_final<<<1, kErrorThreads, 0, ctx->stream>>>(ctx->error_blocks.ptr, blocks, final_record);
+  ctx->kernel_launches += 2;
+  CUDA_OK(ctx, cudaMemcpyAsync(out, final_record, sizeof(ErrorSums), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+  return ETXB_OK;
+}
+
+// mean_rgb of a reference of n pixels
+int reference_mean_rgb(etxb_ctx* ctx, const float4* ref, uint32_t n, double* out) {
+  ErrorSums s = {};
+  if (int rc = run_film_error<true>(ctx, nullptr, ref, n, 0.0, &s)) return rc;
+  *out = s.se / (3.0 * double(n));
+  return ETXB_OK;
+}
+
+// the reference slot has just been filled: its mean, or the slot emptied again when that fails
+int commit_reference(etxb_ctx* ctx) {
+  if (int rc = reference_mean_rgb(ctx, ctx->reference.ptr, ctx->path_count, &ctx->reference_mean_rgb)) {
+    ctx->reference.release();
+    return rc;
+  }
+  return ETXB_OK;
+}
+
+int film_error_of(etxb_ctx* ctx, const float4* layer, const float4* ref, uint32_t n, double mean_rgb, etxb_film_error_info* out) {
+  ErrorSums s = {};
+  const double eps = (0.01 * mean_rgb) * (0.01 * mean_rgb);
+  if (int rc = run_film_error<false>(ctx, layer, ref, n, eps, &s)) return rc;
+  const double finite = double(s.finite);
+  memset(out, 0, sizeof(*out));
+  out->pixels = n;
+  out->nonfinite = s.nonfinite;
+  out->negative = s.negative;
+  out->lum_above = s.above;
+  out->lum_below = s.below;
+  out->mse = s.se / (3.0 * finite);
+  out->rel_mse = s.rel / (3.0 * finite);
+  out->mean_abs_lum = s.abs_lum / finite;
+  out->mean_lum = s.lum / finite;
+  out->reference_mean_lum = s.ref_lum / finite;
   return ETXB_OK;
 }
 
@@ -2562,6 +2657,63 @@ int etxb_save_film(etxb_ctx* ctx, uint32_t layer, const char* file_name, uint32_
   return (rc == ETXB_OK) ? ETXB_OK : fail(ctx, rc, "could not write %s", file_name);
 }
 
+// ImagePool::add_from_data into the viewer's reference slot (app.cxx:243-250 with a file read by the caller)
+int etxb_set_reference_image(etxb_ctx* ctx, const float* rgba, uint32_t width, uint32_t height) {
+  if (!ctx || !rgba) return ETXB_ERR_INVALID_ARGUMENT;
+  if (int rc = check_whole_film(ctx, "etxb_set_reference_image")) return rc;
+  // the reference's HLSL and Metal shaders disagree on a reference of another size (a zero Load against a bilinear uv sample): neither is taken
+  if ((width != ctx->width) || (height != ctx->height))
+    return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "etxb_set_reference_image: a %ux%u image for a %ux%u film", width, height, ctx->width, ctx->height);
+  cudaSetDevice(ctx->device);
+  if (ctx->reference.count != ctx->path_count) CUDA_OK(ctx, ctx->reference.alloc(ctx->path_count));
+  CUDA_OK(ctx, cudaMemcpyAsync(ctx->reference.ptr, rgba, ctx->reference.bytes(), cudaMemcpyHostToDevice, ctx->stream));
+  return commit_reference(ctx);
+}
+
+// Use as Reference (app.cxx:252-259): the layer as it stands, copied on the device
+int etxb_use_film_as_reference(etxb_ctx* ctx, uint32_t layer) {
+  if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;
+  if (int rc = check_whole_film(ctx, "etxb_use_film_as_reference")) return rc;
+  const float4* src = nullptr;
+  if (int rc = film_layer_source(ctx, layer, &src)) return rc;
+  if (ctx->reference.count != ctx->path_count) CUDA_OK(ctx, ctx->reference.alloc(ctx->path_count));
+  CUDA_OK(ctx, cudaMemcpyAsync(ctx->reference.ptr, src, ctx->reference.bytes(), cudaMemcpyDeviceToDevice, ctx->stream));
+  return commit_reference(ctx);
+}
+
+int etxb_clear_reference(etxb_ctx* ctx) {
+  if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;
+  if ((ctx->comm != nullptr) || (ctx->world > 1u)) return fail(ctx, ETXB_ERR_UNSUPPORTED, "etxb_clear_reference: the film of a context with pixel tiles holds only its own tiles");
+  cudaSetDevice(ctx->device);
+  ctx->reference.release();
+  return ETXB_OK;
+}
+
+// RenderContext's fragment shader (render.cxx:252-388) over the whole layer
+int etxb_read_film_view(etxb_ctx* ctx, uint32_t layer, const etxb_view* view, void* dst, uint64_t dst_bytes) {
+  if (!ctx || !dst) return ETXB_ERR_INVALID_ARGUMENT;
+  if (int rc = check_view(ctx, view)) return rc;
+  if (int rc = check_whole_film(ctx, "etxb_read_film_view")) return rc;
+  if ((view->view >= ETXB_VIEW_REFERENCE) && !has_reference(ctx)) return fail(ctx, ETXB_ERR_NOT_READY, "etxb_read_film_view: view %u needs a reference image", view->view);
+  const size_t n = ctx->path_count;
+  if (dst_bytes < n * (view->rgba8 ? 4u : 16u)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "film buffer too small");
+  const float4* src = nullptr;
+  if (int rc = film_layer_source(ctx, layer, &src)) return rc;
+  return run_film_view(ctx, src, (view->view >= ETXB_VIEW_REFERENCE) ? ctx->reference.ptr : nullptr, n, *view, dst);
+}
+
+int etxb_film_error(etxb_ctx* ctx, uint32_t layer, etxb_film_error_info* out) {
+  if (!ctx || !out) return ETXB_ERR_INVALID_ARGUMENT;
+  if (int rc = check_whole_film(ctx, "etxb_film_error")) return rc;
+  if (!has_reference(ctx)) return fail(ctx, ETXB_ERR_NOT_READY, "etxb_film_error: no reference image");
+  if (int rc = ctx_drain(ctx)) return rc;
+  const float4* src = nullptr;
+  if (int rc = film_layer_source(ctx, layer, &src)) return rc;
+  if (int rc = film_error_of(ctx, src, ctx->reference.ptr, ctx->path_count, ctx->reference_mean_rgb, out)) return rc;
+  out->iterations = ctx->completed;
+  return ETXB_OK;
+}
+
 int etxb_get_counters(etxb_ctx* ctx, etxb_counters* out) {
   if (!ctx || !out) return ETXB_ERR_INVALID_ARGUMENT;
   cudaSetDevice(ctx->device);
@@ -2845,6 +2997,33 @@ int etxb_debug_denoise(etxb_ctx* ctx, const float* color, const float* camera, c
   CUDA_OK(ctx, cudaMemcpy(out, dout.ptr, n * 16, cudaMemcpyDeviceToHost));
   if (out_variance) CUDA_OK(ctx, cudaMemcpy(out_variance, dvar.ptr, n * 16, cudaMemcpyDeviceToHost));
   return ETXB_OK;
+}
+
+// Test hook: etxb_read_film_view's kernel on host arrays
+int etxb_debug_film_view(etxb_ctx* ctx, const float* layer, const float* reference, uint32_t count, const etxb_view* view, void* out) {
+  if (!ctx || !layer || !out || !count) return ETXB_ERR_INVALID_ARGUMENT;
+  if (int rc = check_view(ctx, view)) return rc;
+  if ((view->view >= ETXB_VIEW_REFERENCE) && !reference) return fail(ctx, ETXB_ERR_NOT_READY, "etxb_debug_film_view: view %u needs a reference image", view->view);
+  cudaSetDevice(ctx->device);
+  DevBuf<float4> dl, dr;
+  if (int rc = upload(ctx, dl, reinterpret_cast<const float4*>(layer), count)) return rc;
+  if (reference)
+    if (int rc = upload(ctx, dr, reinterpret_cast<const float4*>(reference), count)) return rc;
+  return run_film_view(ctx, dl.ptr, reference ? dr.ptr : nullptr, count, *view, out);
+}
+
+// Test hook: etxb_film_error's kernels on host arrays (the reference's mean taken as etxb_set_reference_image takes it)
+int etxb_debug_film_error(etxb_ctx* ctx, const float* layer, const float* reference, uint32_t width, uint32_t height, etxb_film_error_info* out) {
+  if (!ctx || !layer || !reference || !out || !width || !height) return ETXB_ERR_INVALID_ARGUMENT;
+  if (uint64_t(width) * height > (1ull << 26)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "etxb_debug_film_error: film too large");
+  cudaSetDevice(ctx->device);
+  const uint32_t n = width * height;
+  DevBuf<float4> dl, dr;
+  if (int rc = upload(ctx, dl, reinterpret_cast<const float4*>(layer), n)) return rc;
+  if (int rc = upload(ctx, dr, reinterpret_cast<const float4*>(reference), n)) return rc;
+  double mean_rgb = 0.0;
+  if (int rc = reference_mean_rgb(ctx, dr.ptr, n, &mean_rgb)) return rc;
+  return film_error_of(ctx, dl.ptr, dr.ptr, n, mean_rgb, out);
 }
 
 // Test hook: the noise estimate of `world` pixel-tile ranks on one device (layout in include/etx_b200.h).  Each rank's view holds its own pixels

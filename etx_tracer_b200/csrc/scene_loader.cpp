@@ -487,6 +487,29 @@ int etxb_image_file_read(const char* file_name, uint32_t* width, uint32_t* heigh
   return ETXB_OK;
 }
 
+// The viewer's reference image as ImagePool::add_from_file(file, 0, {}, {1, 1}) leaves it (image_pool.cxx:51-67, 162-224, 271-385): float4 per
+// pixel, rows in file order, 8-bit files read back as UNORM after the pool's sRGB -> linear and truncation.  A file that cannot be read is the
+// 1 x 1 white placeholder, with the reason in `err`, and ETXB_OK, as the pool takes it.  Call with rgba = NULL for the size.
+int etxb_reference_image_file_read(const char* file_name, uint32_t* width, uint32_t* height, float* rgba, uint64_t capacity, char* err, uint64_t err_bytes) {
+  if (file_name == nullptr || width == nullptr || height == nullptr) return ETXB_ERR_INVALID_ARGUMENT;
+  put_error(err, err_bytes, "");
+  Pixels px;
+  std::string problem;
+  if (!pool_read(file_name, px, problem)) put_error(err, err_bytes, problem + "; using the 1x1 white placeholder");
+  pool_convert(px, true, exr_file(file_name));
+  *width = px.w, *height = px.h;
+  if (rgba != nullptr) {
+    const size_t n = size_t(px.w) * px.h;
+    if (capacity < uint64_t(n) * 16u) return ETXB_ERR_OVERFLOW;
+    if (px.eight_bit) {
+      for (size_t i = 0; i < n * 4u; ++i) rgba[i] = px.u8[i] / 255.0f;
+    } else {
+      memcpy(rgba, px.f32.data(), n * 16u);
+    }
+  }
+  return ETXB_OK;
+}
+
 // The tangent-space generator and the NanoVDB reader on their own, for a caller that assembles the scene itself (the Python twin)
 int etxb_mesh_tangents(etxb_vertex* vertices, uint64_t vertex_count, const etxb_triangle* triangles, uint64_t triangle_count) {
   if ((vertices == nullptr && vertex_count != 0) || (triangles == nullptr && triangle_count != 0)) return ETXB_ERR_INVALID_ARGUMENT;

@@ -109,6 +109,13 @@ class IntegratorAdapter {
   // Film::denoise (film.cxx:420-423, the application's Denoise button): `layer` (RESULT or CAMERA) into ETXB_FILM_DENOISED, on the device; waits for
   // the iteration in flight.  The filter is the module's own (DESIGN §13), not OpenImageDenoise.
   int denoise(uint32_t layer) { return enabled() ? etxb_denoise(_ctx, layer) : _create_result; }
+  // The viewer (DESIGN §14): its reference image (Open Reference Image / Use as Reference), its six output views, and the error against the
+  // reference (waits for the iteration in flight)
+  int set_reference(const float* rgba, uint32_t width, uint32_t height) { return enabled() ? etxb_set_reference_image(_ctx, rgba, width, height) : _create_result; }
+  int use_as_reference(uint32_t layer = ETXB_FILM_RESULT) { return enabled() ? etxb_use_film_as_reference(_ctx, layer) : _create_result; }
+  int clear_reference() { return enabled() ? etxb_clear_reference(_ctx) : _create_result; }
+  int view(uint32_t layer, const etxb_view& v, void* dst, uint64_t bytes) { return enabled() ? etxb_read_film_view(_ctx, layer, &v, dst, bytes) : _create_result; }
+  int film_error(uint32_t layer, etxb_film_error_info* out) { return enabled() ? etxb_film_error(_ctx, layer, out) : _create_result; }
   etxb_ctx* context() { return _ctx; }
 
  protected:

@@ -7,11 +7,12 @@ and the film export (OpenEXR float layer, or the tone-mapped PNG).  There is no 
 the frame is split into pixel tiles over N GPUs, one process each (both integrators; the exchange runs inside the module over NCCL).
 """
 import argparse
+import json
 import sys
 import time
 
 from . import loader, structs as S
-from .api import GPUPathTracing, GPUVCM, SceneFile, tonemap, write_exr, write_png
+from .api import GPUPathTracing, GPUVCM, SceneFile, read_reference_image, tonemap, write_exr, write_png
 
 LAYERS = {"result": S.FILM_RESULT, "camera": S.FILM_CAMERA, "light": S.FILM_LIGHT, "normals": S.FILM_NORMALS, "albedo": S.FILM_ALBEDO,
           "denoised": S.FILM_DENOISED}
@@ -32,9 +33,18 @@ def main(argv=None):
     ap.add_argument("--noise-threshold", type=float, default=None, help="pt: Scene::noise_threshold of the adaptive sampling (default: the scene's)")
     ap.add_argument("--gpus", type=int, default=1, help="render pixel tiles on this many GPUs, one process each, exchanging over NCCL inside the "
                     "module; rank 0 writes the output")
+    ap.add_argument("--reference", default=None, metavar="FILE", help="the viewer's reference image (EXR / HDR / PFM / PNG / JPEG, the film's size): "
+                    "prints the final error against it as one JSON line")
+    ap.add_argument("--view", choices=S.VIEW_NAMES, default=None, help="write this output view of the layer instead of the layer itself: 8-bit to a .png, "
+                    "float to an .exr (tone mapping and sRGB on, --exposure)")
+    ap.add_argument("--error-every", type=int, default=0, metavar="N", help="with --reference: one JSON error line per N completed iterations")
     args = ap.parse_args(argv)
     if args.gpus < 1:
         ap.error("--gpus must be at least 1")
+    if args.error_every < 0 or (args.error_every and not args.reference):
+        ap.error("--error-every needs --reference and N >= 1")
+    if args.gpus > 1 and (args.reference or args.view):
+        ap.error("--reference and --view need the whole film on one GPU: render with --gpus 1")
     if args.gpus == 1:
         return _render(args)
     if args.denoise:
@@ -87,10 +97,17 @@ def _render(args, rank=0, comm_id=None):
         g.set_option(key, float(value))
     if args.integrator == "pt" and args.noise_threshold is not None:
         g.set_scene_settings(args.noise_threshold, float(sd.scene["radiance_clamp"][0]))
+    if args.reference:
+        g.set_reference(read_reference_image(args.reference))
     g.run()
-    while g.update():  # non-blocking like Integrator::update; a UI would draw a preview here (g.film_ldr)
+    reported = 0
+    while g.update():  # non-blocking like Integrator::update; a UI would draw a preview here (g.film_ldr or g.view)
+        if args.error_every and g.status()["completed_iterations"] >= reported + args.error_every:
+            reported = _print_error(g)
         time.sleep(0.002)
     g.wait()
+    if args.reference:
+        _print_error(g)
     st = g.status()
     n = sd.width * sd.height * st["completed_iterations"]
     log(f"{st['completed_iterations']} iterations in {st['total_time']:.3f} s of device time{f' on rank 0 of {world}' if world > 1 else ''}: "
@@ -99,7 +116,10 @@ def _render(args, rank=0, comm_id=None):
         g.denoise(S.FILM_RESULT)
     layer = args.layer or ("denoised" if args.denoise else "result")
     tonemapped = args.output.lower().endswith(".png")
-    if comm_id is None:
+    if args.view:
+        out = g.view(LAYERS[layer], S.VIEW_NAMES.index(args.view), S.VIEW_OPT_TONEMAPPING | S.VIEW_OPT_SRGB, args.exposure, rgba8=tonemapped)
+        (write_png if tonemapped else write_exr)(args.output, out)
+    elif comm_id is None:
         g.save_image(args.output, LAYERS[layer], tonemapped=tonemapped, exposure=args.exposure)
     else:
         film = g.comm_reduce_film(LAYERS[layer])  # collective; the frame arrives on rank 0
@@ -112,6 +132,13 @@ def _render(args, rank=0, comm_id=None):
         print(args.output)
     g.close()
     return 0
+
+
+def _print_error(g):
+    """One JSON line: the Result layer's error against the reference after the iterations in flight, with the device time they took."""
+    e = g.film_error(S.FILM_RESULT)
+    print(json.dumps({"iteration": e["iterations"], "seconds": g.status()["total_time"], **e}), flush=True)
+    return e["iterations"]
 
 
 if __name__ == "__main__":

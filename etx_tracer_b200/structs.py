@@ -106,6 +106,14 @@ UPDATE_INFO = np.dtype({"names": ["kept", "images_kept", "images_uploaded", "gri
                                   "bytes_hashed"],
                         "formats": [u4, u4, u4, u4, u4, np.float64, np.float64, np.float64, u8], "offsets": [0, 4, 8, 12, 16, 24, 32, 40, 48], "itemsize": 56})
 KEPT_GEOMETRY, KEPT_WIDE_TREE, KEPT_PATH_STATE = 1, 2, 4
+# the viewer (etxb_read_film_view, etxb_film_error; DESIGN §14): OutputView, ViewOptions, etxb_view (16 B) and etxb_film_error_info (88 B)
+VIEW_TONEMAPPED, VIEW_ALPHA, VIEW_HDR, VIEW_REFERENCE, VIEW_RELATIVE, VIEW_ABSOLUTE = range(6)
+VIEW_NAMES = ("tonemapped", "alpha", "hdr", "reference", "relative", "absolute")
+VIEW_OPT_TONEMAPPING, VIEW_OPT_SRGB, VIEW_OPT_SKIP_COLOR_CONVERSION = 1, 2, 4
+VIEW = np.dtype([("view", u4), ("options", u4), ("exposure", f4), ("rgba8", u4)])
+FILM_ERROR = np.dtype([("pixels", u8), ("nonfinite", u8), ("negative", u8), ("lum_above", u8), ("lum_below", u8), ("mse", np.float64),
+                       ("rel_mse", np.float64), ("mean_abs_lum", np.float64), ("mean_lum", np.float64), ("reference_mean_lum", np.float64),
+                       ("iterations", u4), ("pad", u4)])
 # etxb_closure_query (96 B) and the per-query statistics etxb_debug_closure_eval / oracle_bsdf_eval return (include/etx_b200.h)
 CLOSURE_QUERY = np.dtype([
     ("nrm", f4, 3), ("tan", f4, 3), ("btn", f4, 3), ("w_i", f4, 3), ("w_o", f4, 3), ("uv", f4, 2), ("wavelength", f4),

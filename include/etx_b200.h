@@ -394,6 +394,59 @@ int etxb_write_exr(const char* file_name, const float* rgba, uint32_t width, uin
 int etxb_write_png(const char* file_name, const uint8_t* rgba8, uint32_t width, uint32_t height);
 int etxb_tonemap_rgba8(const float* rgba, uint64_t pixel_count, float exposure, uint8_t* out_rgba8);
 
+/* ---- the viewer (DESIGN §14): RenderContext's fragment shader (sources/raytracer/render.cxx:252-388) and its reference image ------------
+ * etxb_read_film_view computes one of the six OutputViews of a film layer on the device: float4 as the shader returns it (unclamped), or the
+ * RGBA8 an 8-bit UNORM window stores (clamp to [0, 1], floor(255 x + 0.5), NaN -> 0).  Like etxb_read_film_ldr it does not wait for
+ * iterations in flight.  The reference views (Reference, Relative / Absolute Difference) and etxb_film_error need a reference:
+ * ETXB_ERR_NOT_READY without one.  All the calls below are ETXB_ERR_UNSUPPORTED on a context with a communicator or a pixel partition (its
+ * film holds only its own tiles). */
+#define ETXB_VIEW_TONEMAPPED 0u /* OutputView::TonemappedImage */
+#define ETXB_VIEW_ALPHA 1u      /* AlphaChannel */
+#define ETXB_VIEW_HDR 2u        /* HDRImage */
+#define ETXB_VIEW_REFERENCE 3u  /* ReferenceImage */
+#define ETXB_VIEW_RELATIVE 4u   /* RelativeDifference */
+#define ETXB_VIEW_ABSOLUTE 5u   /* AbsoluteDifference */
+#define ETXB_VIEW_OPT_TONEMAPPING 1u /* ViewOptions (raytracer/options.hxx:40-45) */
+#define ETXB_VIEW_OPT_SRGB 2u
+#define ETXB_VIEW_OPT_SKIP_COLOR_CONVERSION 4u
+typedef struct etxb_view {
+  uint32_t view;    /* ETXB_VIEW_*; ETXB_ERR_INVALID_ARGUMENT past 5 */
+  uint32_t options; /* ETXB_VIEW_OPT_* bits; ETXB_ERR_INVALID_ARGUMENT for any other bit */
+  float exposure;   /* finite */
+  uint32_t rgba8;   /* 0: float4 per pixel (16 bytes), 1: RGBA8 (4 bytes) */
+} etxb_view;
+/* The film's error against the reference (float64 sums in a reduction whose shape depends on the pixel count alone: the same bits on every
+ * call).  Pixels whose RGB has a NaN or inf are counted in `nonfinite` and left out of every sum and every other count. */
+typedef struct etxb_film_error_info {
+  uint64_t pixels;          /* W * H */
+  uint64_t nonfinite;       /* pixels with a NaN / inf in RGB */
+  uint64_t negative;        /* finite pixels with a negative RGB channel */
+  uint64_t lum_above;       /* finite pixels where the reference's float32 luminance exceeds the layer's by more than 1/8192 (the Absolute
+                               Difference view's red) */
+  uint64_t lum_below;       /* ... the layer's exceeds the reference's (its green) */
+  double mse;               /* mean over finite pixels and RGB of (c - r)^2 */
+  double rel_mse;           /* mean of (c - r)^2 / (r^2 + eps), eps = (0.01 mean_rgb(reference))^2; not finite when eps is 0 (an all-zero
+                               reference) or not finite (a reference with a NaN / inf pixel).  Every mean is NaN when no pixel is finite. */
+  double mean_abs_lum;      /* means over finite pixels of |c_lum - r_lum|, c_lum, r_lum (float64, the view's weights) */
+  double mean_lum;
+  double reference_mean_lum;
+  uint32_t iterations;      /* completed iterations the film held */
+  uint32_t pad;
+} etxb_film_error_info;
+/* ImagePool::add_from_data: host float4 pixels (film storage order, W x H of the film) into the reference slot.  ETXB_ERR_INVALID_ARGUMENT for
+ * another size.  The slot is kept across etxb_begin / etxb_update_scene / etxb_upload_scene at the same film size and dropped at another. */
+int etxb_set_reference_image(etxb_ctx* ctx, const float* rgba, uint32_t width, uint32_t height);
+/* Use as Reference (app.cxx:252-259): the layer, copied on the device into the reference slot. */
+int etxb_use_film_as_reference(etxb_ctx* ctx, uint32_t layer);
+int etxb_clear_reference(etxb_ctx* ctx);
+int etxb_read_film_view(etxb_ctx* ctx, uint32_t layer, const etxb_view* view, void* dst, uint64_t dst_bytes);
+/* Waits for the iterations in flight first, so that the numbers belong to a whole number of iterations. */
+int etxb_film_error(etxb_ctx* ctx, uint32_t layer, etxb_film_error_info* out);
+/* Open Reference Image (app.cxx:243-250): the float4 pixels ImagePool::add_from_file(file, 0, {}, {1, 1}) holds, host code.  Rows in file
+ * order; 8-bit files through sRGB -> linear, 8-bit truncation and back to [0, 1]; OpenEXR with inf -> 65504 and NaN / negatives -> 0; HDR
+ * and PFM as read.  A file that cannot be read gives the 1 x 1 white placeholder and a warning in `err` (ETXB_OK).  rgba = NULL: the size. */
+int etxb_reference_image_file_read(const char* file_name, uint32_t* width, uint32_t* height, float* rgba, uint64_t capacity, char* err, uint64_t err_bytes);
+
 /* ---- scene files (SURVEY 8(f) N2): SceneRepresentation::load_from_file (render/host/scene_representation.cxx:679-838) ------------------
  * Reads the reference's `.json` + `.obj` + `.mtl` scene dialect (et::camera / et::medium / et::dir / et::env / et::spectrum blocks, the material
  * directives of parse_material :1682-2079, PNG / JPEG / TGA / BMP / EXR / HDR / PFM textures) into the Scene / Camera PODs etxb_create takes: host C++, no CUDA, no
@@ -533,6 +586,11 @@ int etxb_debug_build_trees(etxb_ctx* ctx, const float* positions, uint32_t verte
  * out_variance may be null.  out_variance receives the smoothed per-pixel variance of the mean.  ETXB_ERR_NOT_READY where a count is below 2. */
 int etxb_debug_denoise(etxb_ctx* ctx, const float* color, const float* camera, const float* half, const uint32_t* counts, const float* normals,
                        const float* albedo, uint32_t width, uint32_t height, float* out, float* out_variance);
+/* etxb_read_film_view's kernel on host arrays: layer / reference = float[4 * count] (reference may be null for views 0-2); out = float[4 * count]
+ * or uint8[4 * count] as view->rgba8 says. */
+int etxb_debug_film_view(etxb_ctx* ctx, const float* layer, const float* reference, uint32_t count, const etxb_view* view, void* out);
+/* etxb_film_error's kernels on host arrays (float[4 * width * height] each); `iterations` comes back 0. */
+int etxb_debug_film_error(etxb_ctx* ctx, const float* layer, const float* reference, uint32_t width, uint32_t height, etxb_film_error_info* out);
 /* The path tracer's noise estimate (etxb_enqueue_iteration's Film::estimate_noise_levels) on host arrays, as `world` pixel-tile ranks run it:
  * each rank's view holds its own pixels and zeros elsewhere, the level pass runs per rank, the masks are summed (the all-reduce), the dilation
  * runs per rank and the owned pixels are composed.  world = 1 is the one-GPU estimate.  camera / adaptive = float[4 * width * height] and
