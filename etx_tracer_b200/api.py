@@ -647,45 +647,37 @@ class GPUVCM:
         self._check(self.lib.etxb_debug_math(self.h, fn, _p(x), _p(yy) if yy is not None else None, x.shape[0], _p(out)))
         return out
 
+    def _debug_queries(self, fn, queries, query_dtype, repetitions, result_dtype, stats=None):
+        """Runs a query hook of the C interface over `queries`: one result record per query and repetition, or `stats` values per query."""
+        queries = np.ascontiguousarray(queries, dtype=query_dtype)
+        out = np.zeros((queries.shape[0], int(repetitions) if stats is None else stats), dtype=result_dtype)
+        self._check(fn(self.h, _p(queries), queries.shape[0], int(repetitions), _p(out)))
+        return out
+
     def debug_closure(self, queries, repetitions):
         """The vertex closures (make_closure + closure_evaluate) for S.CLOSURE_QUERY records on the uploaded scene, `repetitions` fresh
         samplers per query; returns float64 (n, S.CLOSURE_STATS), laid out as etxb_debug_closure_eval documents (include/etx_b200.h)."""
-        queries = np.ascontiguousarray(queries, dtype=S.CLOSURE_QUERY)
-        out = np.zeros((queries.shape[0], S.CLOSURE_STATS), dtype=np.float64)
-        self._check(self.lib.etxb_debug_closure_eval(self.h, _p(queries), queries.shape[0], int(repetitions), _p(out)))
-        return out
+        return self._debug_queries(self.lib.etxb_debug_closure_eval, queries, S.CLOSURE_QUERY, repetitions, np.float64, S.CLOSURE_STATS)
 
     def debug_bsdf_sample(self, queries, repetitions):
         """bsdf_sample for S.SAMPLE_QUERY records on the uploaded scene, repetition r of each on the sampler (seed, r); returns
         S.SAMPLE_RESULT records shaped (n, repetitions), laid out as etxb_debug_bsdf_sample documents (include/etx_b200.h)."""
-        queries = np.ascontiguousarray(queries, dtype=S.SAMPLE_QUERY)
-        out = np.zeros((queries.shape[0], int(repetitions)), dtype=S.SAMPLE_RESULT)
-        self._check(self.lib.etxb_debug_bsdf_sample(self.h, _p(queries), queries.shape[0], int(repetitions), _p(out)))
-        return out
+        return self._debug_queries(self.lib.etxb_debug_bsdf_sample, queries, S.SAMPLE_QUERY, repetitions, S.SAMPLE_RESULT)
 
     def debug_emitter(self, queries, repetitions=1):
         """The emitter routines for S.EMITTER_QUERY records on the uploaded scene, repetition r of each emission query on the sampler (seed, r);
         returns S.EMITTER_RESULT records shaped (n, repetitions), laid out as etxb_debug_emitter documents (include/etx_b200.h)."""
-        queries = np.ascontiguousarray(queries, dtype=S.EMITTER_QUERY)
-        out = np.zeros((queries.shape[0], int(repetitions)), dtype=S.EMITTER_RESULT)
-        self._check(self.lib.etxb_debug_emitter(self.h, _p(queries), queries.shape[0], int(repetitions), _p(out)))
-        return out
+        return self._debug_queries(self.lib.etxb_debug_emitter, queries, S.EMITTER_QUERY, repetitions, S.EMITTER_RESULT)
 
     def debug_medium(self, queries, repetitions=1):
         """The media routines for S.MEDIUM_QUERY records on the uploaded scene, repetition r of each query on the sampler (seed, r); returns
         S.MEDIUM_RESULT records shaped (n, repetitions), laid out as etxb_debug_medium documents (include/etx_b200.h)."""
-        queries = np.ascontiguousarray(queries, dtype=S.MEDIUM_QUERY)
-        out = np.zeros((queries.shape[0], int(repetitions)), dtype=S.MEDIUM_RESULT)
-        self._check(self.lib.etxb_debug_medium(self.h, _p(queries), queries.shape[0], int(repetitions), _p(out)))
-        return out
+        return self._debug_queries(self.lib.etxb_debug_medium, queries, S.MEDIUM_QUERY, repetitions, S.MEDIUM_RESULT)
 
     def debug_subsurface(self, queries, repetitions=1):
         """The subsurface routines for S.SUBSURFACE_QUERY records on the uploaded scene, repetition r of each query on the sampler (seed, r);
         returns S.SUBSURFACE_RESULT records shaped (n, repetitions), laid out as etxb_debug_subsurface documents (include/etx_b200.h)."""
-        queries = np.ascontiguousarray(queries, dtype=S.SUBSURFACE_QUERY)
-        out = np.zeros((queries.shape[0], int(repetitions)), dtype=S.SUBSURFACE_RESULT)
-        self._check(self.lib.etxb_debug_subsurface(self.h, _p(queries), queries.shape[0], int(repetitions), _p(out)))
-        return out
+        return self._debug_queries(self.lib.etxb_debug_subsurface, queries, S.SUBSURFACE_QUERY, repetitions, S.SUBSURFACE_RESULT)
 
     def debug_thresholds(self, **fields):
         """The queue sizes from which the passes take their large-queue branches (etxb_debug_set_thresholds): keyword fields of

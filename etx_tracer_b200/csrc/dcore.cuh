@@ -11,7 +11,9 @@
 #include "portable_math.h"
 
 #define DEV __device__ __forceinline__
-#define DEVN __device__ __noinline__
+// out of line, and `inline` for the linker: nvcc gives a non-inline __device__ function an external host symbol, and the units that include
+// these headers (module.cu, test_hooks.cu) would each define it
+#define DEVN __device__ __noinline__ inline
 // experiment switches (default: out of line)
 #if defined(ETXB_BSDF_INLINE)
 #define DEVG_BSDF DEV

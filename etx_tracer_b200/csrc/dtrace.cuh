@@ -5,6 +5,17 @@
 #pragma once
 #include "dscene.cuh"
 
+// A kernel's traversal counters (TraverseStats, bvh.h): real ones in the count build, a null `stats` pointer in the others
+#ifdef ETXB_COUNT_TRAVERSAL
+#define STATS_DECL TraverseStats stats_obj; TraverseStats* stats = &stats_obj
+#define STATS_NODES stats_obj.nodes
+#define STATS_TRIS stats_obj.tris
+#else
+#define STATS_DECL TraverseStats* stats = nullptr
+#define STATS_NODES 0u
+#define STATS_TRIS 0u
+#endif
+
 namespace etxb {
 
 struct DevNodeLoad {

@@ -1,4 +1,4 @@
-// kernels.cuh — the wavefront kernels of one VCM iteration (included once, by module.cu).
+// kernels.cuh — the wavefront kernels of one VCM iteration (included once, by module.cu; test_hooks.cu has its own kernels).
 //
 // Stage list (reference decomposition: bin/optix/vcm/*.cu + vcm_cpu.cxx:95-241, redesigned for sm_90a):
 //   light pass : k_light_begin -> { k_trace_closest -> k_light_bounce }*          (queues of path ids, ping-pong)
@@ -100,16 +100,6 @@ struct LaunchParams {
                                  //    light-to-camera connections go to the shadow list with their target address; k_shadow_resolve adds the unoccluded ones
   uint32_t merge_material_major; // 1 (scenes with stochastic BSDFs): the gather queue is ordered by (material, Morton code) instead of the Morton code alone
 };
-
-#ifdef ETXB_COUNT_TRAVERSAL
-#define STATS_DECL TraverseStats stats_obj; TraverseStats* stats = &stats_obj
-#define STATS_NODES stats_obj.nodes
-#define STATS_TRIS stats_obj.tris
-#else
-#define STATS_DECL TraverseStats* stats = nullptr
-#define STATS_NODES 0u
-#define STATS_TRIS 0u
-#endif
 
 // PLAIN (template parameter of the bounce kernels): compile-time promise that the scene has no media, Boundary surfaces or subsurface
 // materials — what C1-C3-class scenes otherwise pay for in registers, stack and instruction footprint (measured +4 % C2, +6 % on C3's bounce
@@ -1657,366 +1647,9 @@ __global__ void __launch_bounds__(256) k_film_resolve(const __grid_constant__ Fi
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// debug / known-answer kernels
+// test hook kernels: the one that stages queries for the product's own gather (etxb_debug_merge); the kernels of the hooks that run the
+// d*.cuh routines on host-given queries are in test_hooks.cu
 // ---------------------------------------------------------------------------------------------------------------------
-// closest hits of rays (origin, tmin, direction, tmax: 8 floats each), as k_trace_closest finds them; through the 4-wide quantised tree, as
-// k_trace_closest_wide finds them, when `wide` (product build, scenes that have one)
-__global__ void k_debug_trace(const __grid_constant__ DeviceScene sc, const float* rays, uint32_t* seeds, uint32_t count, uint32_t wide, float* hits_uv_t,
-                              uint32_t* hits_tri) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= count) return;
-  const float* r = rays + size_t(i) * 8;
-  const V3 o = {r[0], r[1], r[2]}, d = {r[4], r[5], r[6]};
-  Smp smp = Smp::resume(seeds[i]);
-  uint32_t n_nodes = 0, n_tris = 0;
-  const HitRec h = wide ? trace_closest_wide(sc, o, d, r[3], r[7], smp, n_nodes, n_tris) : trace_closest(sc, o, d, r[3], r[7], smp, nullptr);
-  seeds[i] = smp.seed;
-  hits_tri[i] = h.tri;
-  bool hit = h.tri != kInvalidIndex;
-  hits_uv_t[size_t(i) * 3 + 0] = hit ? h.u : 0.0f;
-  hits_uv_t[size_t(i) * 3 + 1] = hit ? h.v : 0.0f;
-  hits_uv_t[size_t(i) * 3 + 2] = hit ? h.t : 0.0f;
-}
-
-// occlusion of segments (p0, p1: 6 floats each), as k_shadow_resolve tests them: any non-Void surface in between; through the 4-wide
-// quantised tree when `wide` (product build, scenes that have one), the BVH2 otherwise
-__global__ void k_debug_occluded(const __grid_constant__ DeviceScene sc, const float* segments, uint32_t count, uint32_t wide, uint32_t* occluded) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= count) return;
-  const float* s = segments + size_t(i) * 6;
-  const V3 p0 = {s[0], s[1], s[2]}, p1 = {s[3], s[4], s[5]};
-  if (!wide) {
-    occluded[i] = trace_occluded(sc, p0, p1) ? 1u : 0u;
-    return;
-  }
-  V3 direction;
-  float t_max;
-  if (!shadow_segment(p0, p1, direction, t_max)) {
-    occluded[i] = 0u;  // a degenerate segment is unoccluded
-    return;
-  }
-  OcclusionVisitor visit{sc, false};
-  uint32_t n_nodes = 0, n_tris = 0;
-  wide_trace(sc, p0, direction, kRayEpsilon, t_max, visit, n_nodes, n_tris);
-  occluded[i] = visit.occluded ? 1u : 0u;
-}
-
-__global__ void k_debug_sampler(const uint32_t* a, const uint32_t* b, uint32_t count, uint32_t draws, uint32_t* out_seed, float* out_values) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= count) return;
-  Smp s;
-  s.init(a[i], b[i]);
-  out_seed[size_t(i) * (draws + 1u)] = s.seed;
-  for (uint32_t d = 0; d < draws; ++d) {
-    out_values[size_t(i) * draws + d] = s.next();
-    out_seed[size_t(i) * (draws + 1u) + d + 1u] = s.seed;
-  }
-}
-
-__global__ void k_debug_math(const __grid_constant__ DeviceScene sc, uint32_t fn, const float* x, const float* y, uint32_t count, float* out) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= count) return;
-  float a = x[i], b = y ? y[i] : 0.0f, r = 0.0f;
-  switch (fn) {
-    case 0: r = m_sin(a); break;
-    case 1: r = m_cos(a); break;
-    case 2: r = m_exp(a); break;
-    case 3: r = m_log(a); break;
-    case 4: r = m_pow(a, b); break;
-    case 5: r = m_acos(a); break;
-    case 6: r = m_atan2(a, b); break;
-    case 7: r = spectral_sample_wavelength(a); break;
-    case 8: r = spectral_sampling_pdf(a); break;
-    case 9: r = spec_to_rgb<true>(sc, Spec<true>{1.0f}, a).x; break;
-    case 10: r = spec_to_rgb<true>(sc, Spec<true>{1.0f}, a).y; break;
-    case 11: r = spec_to_rgb<true>(sc, Spec<true>{1.0f}, a).z; break;
-    case 12: r = m_atan(a); break;
-    case 13: r = m_asin(a); break;
-    case 14: r = sample_blue_noise(sc, uint32_t(a) & 127u, uint32_t(a) >> 7, uint32_t(b), 0).x; break;
-    case 15: r = sample_blue_noise(sc, uint32_t(a) & 127u, uint32_t(a) >> 7, uint32_t(b), 4).y; break;
-    default: break;
-  }
-  out[i] = r;
-}
-
-// one thread per etxb_closure_query: `reps` times make_closure + closure_evaluate on a fresh sampler Smp::init(seed, r), as the photon gather
-// and the vertex connections call them; float64 running moments (Welford: a constant output keeps a variance of exactly 0) of
-// {func.rgb, bsdf.rgb, pdf, rev_pdf}, repetition 0's raw values and the counters of include/etx_b200.h (ETXB_CLOSURE_STATS per query)
-template <bool SP>
-__global__ void k_debug_closure(const __grid_constant__ DeviceScene sc, const etxb_closure_query* queries, uint32_t count, uint32_t reps, double* out) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= count) return;
-  const etxb_closure_query& q = queries[i];
-  const V3 nrm = {q.nrm[0], q.nrm[1], q.nrm[2]}, tan = {q.tan[0], q.tan[1], q.tan[2]}, btn = {q.btn[0], q.btn[1], q.btn[2]};
-  const V3 w_i = {q.w_i[0], q.w_i[1], q.w_i[2]}, w_o = {q.w_o[0], q.w_o[1], q.w_o[2]};
-  const BData d = {{0.0f, 0.0f, 0.0f}, nrm, tan, btn, {q.uv[0], q.uv[1]}, w_i, SP ? q.wavelength : -1.0f, q.path_source, kInvalidIndex};
-  double mean[8], m2[8];
-  double* o = out + size_t(i) * ETXB_CLOSURE_STATS;
-  for (uint32_t k = 0; k < 8; ++k) mean[k] = m2[k] = 0.0;
-  uint32_t finite = 0, nonfinite = 0, negative = 0, unsupported = 0;
-  for (uint32_t r = 0; r < reps; ++r) {
-    Smp smp;
-    smp.init(q.seed, r);
-    const Closure<SP> c = make_closure<SP>(sc, d, q.material, smp);
-    const CEval<SP> e = closure_evaluate<SP>(sc, c, w_o, smp);
-    const V3 f = e.func.as_v3(), b = e.bsdf.as_v3();
-    const float v[8] = {f.x, f.y, f.z, b.x, b.y, b.z, e.pdf, e.rev_pdf};
-    if (r == 0) {
-      for (uint32_t k = 0; k < 8; ++k) o[16 + k] = v[k];
-    }
-    bool ok = true;
-    for (uint32_t k = 0; k < 8; ++k) ok = ok && isfinite(v[k]);
-    negative += ((e.pdf < 0.0f) || (e.rev_pdf < 0.0f)) ? 1u : 0u;
-    unsupported += ((e.pdf == 0.0f) && ((f.x != 0.0f) || (f.y != 0.0f) || (f.z != 0.0f) || (b.x != 0.0f) || (b.y != 0.0f) || (b.z != 0.0f))) ? 1u : 0u;
-    if (!ok) {
-      nonfinite += 1u;
-      continue;
-    }
-    finite += 1u;
-    for (uint32_t k = 0; k < 8; ++k) {
-      const double delta = double(v[k]) - mean[k];
-      mean[k] += delta / double(finite);
-      m2[k] += delta * (double(v[k]) - mean[k]);
-    }
-  }
-  for (uint32_t k = 0; k < 8; ++k) {
-    o[k] = mean[k];
-    o[8 + k] = (finite > 0) ? m2[k] / double(finite) : 0.0;
-  }
-  o[24] = double(nonfinite);
-  o[25] = double(negative);
-  o[26] = double(unsupported);
-  for (uint32_t k = 27; k < ETXB_CLOSURE_STATS; ++k) o[k] = 0.0;
-}
-
-// one thread per (etxb_sample_query, repetition): bsdf_sample on the sampler Smp::init(seed, r) with the fixed values a bounce pushes
-// (mode 0, kernels.cuh / dpt.cuh at every bsdf_sample call) or the query's own (mode 1); record layout in include/etx_b200.h
-template <bool SP>
-__global__ void k_debug_bsdf_sample(const __grid_constant__ DeviceScene sc, const etxb_sample_query* queries, uint32_t count, uint32_t reps, etxb_sample_result* out) {
-  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= count * reps) return;
-  const uint32_t i = t / reps, r = t % reps;
-  const etxb_sample_query& q = queries[i];
-  const V3 nrm = {q.nrm[0], q.nrm[1], q.nrm[2]}, tan = {q.tan[0], q.tan[1], q.tan[2]}, btn = {q.btn[0], q.btn[1], q.btn[2]};
-  const V3 w_i = {q.w_i[0], q.w_i[1], q.w_i[2]};
-  const BData d = {{0.0f, 0.0f, 0.0f}, nrm, tan, btn, {q.uv[0], q.uv[1]}, w_i, SP ? q.wavelength : -1.0f, q.path_source, q.medium};
-  Smp smp;
-  smp.init(q.seed, r);
-  etxb_sample_result& o = out[t];
-  o.seed_start = smp.seed;
-  if (q.mode == 0u) {
-    const V2 rnd_bsdf = smp.next_2d();
-    smp.next_2d();  // rnd_connection
-    const V2 rnd_support = smp.next_2d();
-    smp.push_fixed(rnd_bsdf.x, rnd_bsdf.y, rnd_support.x);
-  } else {
-    smp.push_fixed(q.fixed[0], q.fixed[1], q.fixed[2]);
-  }
-  const BSample<SP> s = bsdf_sample<SP>(sc, d, sc.materials[q.material], smp);
-  smp.pop_fixed();
-  const V3 w = s.weight.as_v3();
-  o.w_o[0] = s.w_o.x;
-  o.w_o[1] = s.w_o.y;
-  o.w_o[2] = s.w_o.z;
-  o.pdf = s.pdf;
-  o.weight[0] = w.x;
-  o.weight[1] = w.y;
-  o.weight[2] = w.z;
-  o.eta = s.eta;
-  o.properties = s.properties;
-  o.medium_index = s.medium_index;
-  o.seed_end = smp.seed;
-}
-
-// one thread per (etxb_emitter_query, repetition): the emitter routines of dvcm.cuh as the passes call them; ops and record layout in
-// include/etx_b200.h
-static_assert(sizeof(etxb_emitter_query) == 80u && sizeof(etxb_emitter_result) == 104u, "etxb_emitter_query / etxb_emitter_result layout");
-template <bool SP>
-__global__ void k_debug_emitter(const __grid_constant__ DeviceScene sc, const etxb_emitter_query* queries, uint32_t count, uint32_t reps, etxb_emitter_result* out) {
-  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= count * reps) return;
-  const uint32_t i = t / reps, r = t % reps;
-  const etxb_emitter_query& q = queries[i];
-  const float wavelength = SP ? q.wavelength : -1.0f;
-  const V3 source = {q.source[0], q.source[1], q.source[2]};
-  etxb_emitter_result o = {};
-  EmitterSample<SP> s = {};
-  s.value = Spec<SP>::make(0.0f);
-  s.emitter_index = s.triangle_index = s.medium_index = kInvalidIndex;
-  if (q.op == ETXB_EMITTER_SELECT) {
-    s.emitter_index = distribution_sample(sc.emitter_dist, sc.emitter_count + 1u, q.rnd[0]);
-    s.pdf_sample = emitter_discrete_pdf(sc, sc.emitters[s.emitter_index]);
-  } else if (q.op == ETXB_EMITTER_SAMPLE_IN) {
-    s = sample_emitter<SP>(sc, wavelength, q.emitter, {q.rnd[0], q.rnd[1]}, source);
-  } else if (q.op == ETXB_EMITTER_EMISSION) {
-    Smp smp;
-    smp.init(q.seed, r);
-    o.seed_start = smp.seed;
-    s = sample_emission<SP>(sc, wavelength, smp);
-    o.seed_end = smp.seed;
-  } else {
-    const V3 target = {q.target[0], q.target[1], q.target[2]}, direction = {q.direction[0], q.direction[1], q.direction[2]};
-    s.emitter_index = q.emitter;
-    s.value = emitter_get_radiance<SP>(sc, sc.emitters[q.emitter], wavelength, source, target, direction, {q.uv[0], q.uv[1]}, q.directly_visible != 0u, s.pdf_area,
-      s.pdf_dir, s.pdf_dir_out);
-  }
-  const auto put = [](float* dst, V3 a) {
-    dst[0] = a.x;
-    dst[1] = a.y;
-    dst[2] = a.z;
-  };
-  put(o.value, s.value.as_v3());
-  put(o.origin, s.origin);
-  put(o.normal, s.normal);
-  put(o.direction, s.direction);
-  put(o.barycentric, s.barycentric);
-  o.pdf_sample = s.pdf_sample;
-  o.pdf_area = s.pdf_area;
-  o.pdf_dir = s.pdf_dir;
-  o.pdf_dir_out = s.pdf_dir_out;
-  o.emitter_index = s.emitter_index;
-  o.triangle_index = s.triangle_index;
-  o.medium_index = s.medium_index;
-  o.flags = (s.is_delta ? 1u : 0u) | (s.is_distant ? 2u : 0u);
-  out[t] = o;
-}
-
-// one thread per (etxb_medium_query, repetition): the media routines of dmedium.cuh and the shadow-ray walk of dtrace.cuh as the passes
-// call them; ops and record layout in include/etx_b200.h
-static_assert(sizeof(etxb_medium_query) == 96u && sizeof(etxb_medium_result) == 64u, "etxb_medium_query / etxb_medium_result layout");
-template <bool SP>
-__global__ void k_debug_medium(const __grid_constant__ DeviceScene sc, const etxb_medium_query* queries, uint32_t count, uint32_t reps, etxb_medium_result* out) {
-  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= count * reps) return;
-  const uint32_t i = t / reps, r = t % reps;
-  const etxb_medium_query& q = queries[i];
-  const float wavelength = SP ? q.wavelength : -1.0f;
-  const V3 origin = {q.origin[0], q.origin[1], q.origin[2]}, direction = {q.direction[0], q.direction[1], q.direction[2]};
-  const auto put = [](float* dst, V3 a) {
-    dst[0] = a.x;
-    dst[1] = a.y;
-    dst[2] = a.z;
-  };
-  etxb_medium_result o = {};
-  Smp smp;
-  smp.init(q.seed, r);
-  o.seed_start = smp.seed;
-  if (q.op == ETXB_MEDIUM_BOUNDS) {
-    V3 pos = origin, dir = direction;
-    o.flag = medium_intersects_bounds(sc.mediums[q.medium], origin, direction, q.max_t, pos, dir, o.t_min, o.t_max) ? 1u : 0u;
-    put(o.pos, pos);
-    put(o.dir, dir);
-  } else if (q.op == ETXB_MEDIUM_DENSITY) {
-    o.value[0] = medium_sample_density(sc.mediums[q.medium], origin);
-  } else if (q.op == ETXB_MEDIUM_TRANSMITTANCE) {
-    put(o.value, medium_transmittance<SP>(sc, sc.mediums[q.medium], wavelength, smp, origin, direction, q.max_t).as_v3());
-  } else if (q.op == ETXB_MEDIUM_SAMPLE) {
-    const Spec<SP> throughput = Spec<SP>::make3({q.throughput[0], q.throughput[1], q.throughput[2]});
-    const MediumSample<SP> s = sample_medium<SP>(sc, sc.mediums[q.medium], wavelength, throughput, smp, origin, direction, q.max_t);
-    put(o.value, s.weight.as_v3());
-    put(o.pos, s.pos);
-    o.t = s.sampled_medium_t;
-  } else if (q.op == ETXB_MEDIUM_PHASE) {
-    o.value[0] = phase_function(direction, {q.w_o[0], q.w_o[1], q.w_o[2]}, q.g);
-    put(o.dir, sample_phase_function(direction, q.g, {q.rnd[0], q.rnd[1]}));
-  } else {
-    STATS_DECL;  // as every other caller: the count build's trace_transmittance is compiled for a non-null stats pointer
-    put(o.value, trace_transmittance<SP, false>(sc, wavelength, origin, {q.end[0], q.end[1], q.end[2]}, q.medium, smp, stats).as_v3());
-  }
-  o.seed_end = smp.seed;
-  out[t] = o;
-}
-
-// one thread per (etxb_subsurface_query, repetition): the subsurface routines of dsss.cuh as the bounces call them; ops and record layout
-// in include/etx_b200.h
-static_assert(sizeof(etxb_subsurface_query) == 128u && sizeof(etxb_subsurface_probe) == 96u && sizeof(etxb_subsurface_hit) == 64u &&
-                sizeof(etxb_subsurface_result) == 1920u, "etxb_subsurface_query / etxb_subsurface_result layout");
-template <bool SP>
-__global__ void k_debug_subsurface(const __grid_constant__ DeviceScene sc, const etxb_subsurface_query* queries, uint32_t count, uint32_t reps,
-                                   etxb_subsurface_result* out) {
-  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= count * reps) return;
-  const uint32_t i = t / reps, r = t % reps;
-  const etxb_subsurface_query& q = queries[i];
-  const float wavelength = SP ? q.wavelength : -1.0f;
-  const V3 origin = {q.origin[0], q.origin[1], q.origin[2]}, direction = {q.dir[0], q.dir[1], q.dir[2]};
-  const auto put = [](float* dst, V3 a) {
-    dst[0] = a.x;
-    dst[1] = a.y;
-    dst[2] = a.z;
-  };
-  const auto put_probe = [&put](etxb_subsurface_probe& dst, const SSSample& s) {
-    put(dst.o, s.ray_o);
-    put(dst.d, s.ray_d);
-    dst.min_t = s.ray_min_t;
-    dst.max_t = s.ray_max_t;
-    put(dst.u, s.u);
-    put(dst.v, s.v);
-    put(dst.w, s.w);
-    put(dst.basis_prob, s.basis_prob);
-    dst.sampled_radius = s.sampled_radius;
-  };
-  STATS_DECL;  // as every other caller: the count build's traversals are compiled for a non-null stats pointer
-  etxb_subsurface_result& o = out[t];
-  Smp smp;
-  smp.init(q.seed, r);
-  o.seed_start = smp.seed;
-  if ((q.op == ETXB_SUBSURFACE_TRACE_MATERIAL) || (q.op == ETXB_SUBSURFACE_CONTINUOUS_TRACE)) {
-    HitRec h[kSSPerDirection];
-    if (q.op == ETXB_SUBSURFACE_TRACE_MATERIAL) {
-      h[0] = trace_material(sc, origin, direction, q.t_min, q.t_max, q.material, smp, stats);
-      o.count = (h[0].tri != kInvalidIndex) ? 1u : 0u;
-    } else {
-      o.count = continuous_trace(sc, origin, direction, q.t_min, q.t_max, q.material, h, q.max_count, smp, stats);
-    }
-    for (uint32_t k = 0; k < ((q.op == ETXB_SUBSURFACE_TRACE_MATERIAL) ? 1u : o.count); ++k) {
-      o.hits[k].u = h[k].u;
-      o.hits[k].v = h[k].v;
-      o.hits[k].t = h[k].t;
-      o.hits[k].tri = h[k].tri;
-    }
-  } else if (q.op == ETXB_SUBSURFACE_REMAP) {
-    for (uint32_t k = 0; k < 3u; ++k) remap_channel(q.color[k], q.distances[k], o.albedo[k], o.extinction[k], o.scattering[k]);
-  } else {
-    const Isect in = make_intersection(sc, direction, q.triangle, q.u, q.v, 0.0f);
-    const etxb_material& mat = sc.materials[in.material_index];
-    if (q.op == ETXB_SUBSURFACE_PROFILE) {
-      o.s_r = sample_s_r(q.rnd);
-      put(o.eval, ss_evaluate<SP>(sc, wavelength, in.tex, mat, q.radius).as_v3());
-      const SSSample s = ss_sample<SP>(sc, wavelength, in, mat, q.direction, smp);
-      put_probe(o.probes[0], s);
-      o.geometric_weight = ss_geometric_weight({q.normal[0], q.normal[1], q.normal[2]}, s);
-    } else {
-      if (mat.subsurface.cls == 2u) {  // the gather's three probes are its first draws
-        Smp probe_smp = smp;
-        for (uint32_t d = 0; d < kSSDirections; ++d) put_probe(o.probes[d], ss_sample<SP>(sc, wavelength, in, mat, d, probe_smp));
-      }
-      SSGather<SP> g;
-      uint32_t rays = 0;
-      o.flag = ss_gather<SP>(sc, wavelength, in, smp, g, stats, rays) ? 1u : 0u;
-      o.rays = rays;
-      if (o.flag) {
-        o.count = g.count;
-        o.selected = g.selected;
-        o.selected_sample_weight = g.selected_sample_weight;
-        o.total_weight = g.total_weight;
-        for (uint32_t k = 0; k < g.count; ++k) {
-          const Isect e = ss_exit_intersection<SP>(sc, g, k, sc.subsurface_exit_material);
-          o.hits[k].u = g.hits[k].u;
-          o.hits[k].v = g.hits[k].v;
-          o.hits[k].t = g.hits[k].t;
-          o.hits[k].tri = g.hits[k].tri;
-          put(o.hits[k].w_i, e.w_i);
-          put(o.hits[k].weight, g.weights[k].as_v3());
-          put(o.hits[k].pos, e.pos);
-          put(o.hits[k].nrm, e.nrm);
-        }
-      }
-    }
-  }
-  o.seed_end = smp.seed;
-}
-
 // etxb_debug_merge: query i becomes path i of a one-bounce queue, staged in the columns the gather kernels read (hit record, ray
 // direction, throughput, MIS terms, sampler, depth, medium, wavelength), with the merge key k_camera_shade would give it.  Writes the
 // staged camera vertex's position and normal to pos_nrm[2 i], [2 i + 1], and i to queue slot i.

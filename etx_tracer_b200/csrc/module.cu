@@ -1,36 +1,25 @@
 // module.cu — C ABI (include/etx_b200.h) over the wavefront kernels: context, scene upload, iteration driver.
 // Host-side counterpart of CPUVCMImpl (sources/etx/rt/integrators/vcm_cpu.cxx:30-241) and of
-// Raytracing::commit_changes (sources/etx/rt/rt.cxx:58-88).
+// Raytracing::commit_changes (sources/etx/rt/rt.cxx:58-88).  The context is declared in context.cuh; the test hooks that run the d*.cuh
+// routines on host-given queries are in test_hooks.cu.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
-#include <algorithm>
-#include <chrono>
-#include <condition_variable>
-#include <mutex>
-#include <thread>
 #include <cmath>
-#include <cstdarg>
-#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <ctime>
 #include <deque>
-#include <string>
-#include <utility>
-#include <vector>
 
 #include <dlfcn.h>
-#include <nccl.h>
 
 #include "bvh_build.h"
 #include "bvh_build_device.h"
+#include "context.cuh"
 #include "kernels.cuh"
 #include "kernels_pt.cuh"
 #include "kernels_denoise.cuh"
 #include "kernels_view.cuh"
-
-using namespace etxb;
 
 #if defined(ETXB_PARITY) && ETXB_PARITY
 static const char* kFlavor = "parity";
@@ -40,105 +29,9 @@ static const char* kFlavor = "fast";
 
 namespace {
 
-enum KernelId : uint32_t {
-  K_LIGHT_BEGIN,
-  K_TRACE_LIGHT,
-  K_LIGHT_BOUNCE,
-  K_LV_SCAN,
-  K_LV_REORDER,
-  K_GRID_BBOX,
-  K_GRID_KEYS,
-  K_GRID_SORT,
-  K_GRID_BUILD,
-  K_CAMERA_BEGIN,
-  K_TRACE_CAMERA,
-  K_CAMERA_SHADE,
-  K_CAMERA_CONNECT,
-  K_SHADOW_TRACE,
-  K_QUEUE_SORT,
-  K_CAMERA_MERGE_SORT,
-  K_CAMERA_MERGE,
-  K_CAMERA_MERGE_GENERIC,
-  K_CAMERA_CONTINUE,
-  K_FILM_COMMIT,
-  K_COMM_LIGHT_IMAGE,
-  K_COMM_PHOTONS,
-  K_PT_BEGIN,
-  K_PT_SHADE,
-  K_PT_ACCUMULATE,
-  K_FILM_NOISE,
-  K_BVH_BUILD,
-  K_BVH_WIDE,
-  K_FILM_ADAPTIVE,
-  K_DENOISE_VARIANCE,
-  K_DENOISE_SMOOTH,
-  K_DENOISE_NLM,
-  K_COMM_PT_MASK,
-  K_COMM_PT_COUNT,
-  K_COUNT
-};
-const char* kKernelNames[K_COUNT] = {"light_begin", "trace_closest(light)", "light_bounce", "lv_scan", "lv_reorder", "grid_bbox", "grid_keys", "grid_sort", "grid_build",
-  "camera_begin", "trace_closest(camera)", "camera_shade", "camera_connect", "shadow_trace", "queue_sort", "camera_merge_sort", "camera_merge", "camera_merge_generic", "camera_continue", "film_commit_light", "nccl_allreduce_light_image", "nccl_allgather_photons",
-  "pt_begin", "pt_shade", "pt_accumulate", "film_noise_levels", "bvh_build", "bvh_collapse_wide",
-  "film_adaptive_vcm", "denoise_variance", "denoise_smooth", "denoise_nlm", "nccl_allreduce_pt_mask", "nccl_allreduce_pt_count"};
-
-// Queue sizes from which a pass takes its large-queue branches (the context's `thresholds`; etxb_debug_set_thresholds overrides them):
-//   merge_sort_min_queries  the gather queue is sorted by its merge keys (below it, a latency-bound tail, the sort launches cost more than they save)
-//   merge_min_warps_per_sm  the gather gives each warp up to 32 queries while the queue still fills this many warps per SM
-//   tail_queue              vertex connections go through the host-sized, material-pair-sorted list, and the queue count is read every bounce
-//   sort_queue_min          path queues and connection lists are grouped by material (scenes with stochastic BSDFs)
-constexpr etxb_debug_thresholds kDefaultThresholds = {16384u, 32u, 8192u, 1024u, 0u};
-
-// A device allocation with one owner: it is freed when the buffer is destroyed, on the device that is current then.
-template <class T>
-struct DevBuf {
-  T* ptr = nullptr;
-  size_t count = 0;
-  DevBuf() = default;
-  DevBuf(const DevBuf&) = delete;
-  DevBuf& operator=(const DevBuf&) = delete;
-  DevBuf(DevBuf&& o) noexcept : ptr(std::exchange(o.ptr, nullptr)), count(std::exchange(o.count, size_t(0))) {}
-  DevBuf& operator=(DevBuf&& o) noexcept {
-    if (this != &o) {
-      release();
-      ptr = std::exchange(o.ptr, nullptr);
-      count = std::exchange(o.count, size_t(0));
-    }
-    return *this;
-  }
-  ~DevBuf() { release(); }
-  cudaError_t alloc(size_t n) {
-    release();
-    count = n;
-    if (n == 0) return cudaSuccess;
-    return cudaMalloc(&ptr, n * sizeof(T));
-  }
-  // alloc that keeps the allocation when it already holds n elements; counts the allocations it makes
-  cudaError_t ensure(size_t n, uint32_t& allocations) {
-    if (ptr && (count == n)) return cudaSuccess;
-    allocations += 1;
-    return alloc(n);
-  }
-  void release() {
-    if (ptr) cudaFree(ptr);
-    ptr = nullptr;
-    count = 0;
-  }
-  size_t bytes() const { return count * sizeof(T); }
-};
-
-struct TimedLaunch {
-  uint32_t kernel;
-  cudaEvent_t start, stop;
-};
-
 // 128-bit content hash of a byte range, chained through `seed`: four independent 64-bit multiply-rotate lanes over 32-byte stripes (the
 // round of xxHash64), a zero-padded tail, and two differently mixed 64-bit digests of the lanes and the length.  It detects edits, not
 // adversaries.
-struct Hash128 {
-  uint64_t lo = 0, hi = 0;
-  bool operator==(const Hash128& o) const { return (lo == o.lo) && (hi == o.hi); }
-};
 constexpr uint64_t kHashP1 = 0x9E3779B185EBCA87ull, kHashP2 = 0xC2B2AE3D27D4EB4Full, kHashP3 = 0x165667B19E3779F9ull, kHashP4 = 0x85EBCA77C2B2AE63ull;
 inline uint64_t rotl64(uint64_t x, int r) { return (x << r) | (x >> (64 - r)); }
 inline uint64_t hash_round(uint64_t acc, uint64_t w) { return rotl64(acc + w * kHashP2, 31) * kHashP1; }
@@ -165,146 +58,7 @@ Hash128 hash128(const void* data, size_t bytes, Hash128 seed) {
   const uint64_t b = (v[0] * kHashP4) ^ rotl64(v[1], 29) ^ (v[2] * kHashP3) ^ rotl64(v[3], 43);
   return {hash_mix(a ^ (uint64_t(bytes) * kHashP4)), hash_mix(b + uint64_t(bytes) * kHashP1)};
 }
-
-// what the last upload / update of a context copied, by content (etxb_update_scene keeps what did not change)
-struct SceneHashes {
-  bool valid = false;  // set once the whole scene is on the device
-  Hash128 geometry;    // vertex array + triangle array: device vertices, triangles, BVH2 (+ the 4-wide tree)
-  std::vector<Hash128> images, grids;  // per image; per medium (zero for media without a density grid)
-};
-
 }  // namespace
-
-struct etxb_ctx {
-  int device = 0;
-  uint32_t sm_count = 132;  // the device's multiprocessors (set at creation): persistent and grid-stride launches are sized by it
-  cudaStream_t stream = nullptr;
-  std::string error;
-  bool scene_ready = false;
-  bool spectral = false;
-  bool profile = false;
-  bool has_stochastic_merge = false;  // some material that can be merged at is not Lambert (needs the generic gather)
-  bool plain_scene = false;           // set at upload: no media, Boundary surfaces or subsurface (the bounce kernels' PLAIN instantiation)
-  bool opaque_scene = false;          // set at upload: no alpha test can reject a hit (every opacity 1, no alpha images), no Boundary surfaces / media
-
-  // scene in HBM
-  DevBuf<DVertex> vertices;
-  DevBuf<DTriangle> triangles;
-  DevBuf<uint32_t> tri_emitter;
-  DevBuf<etxb_material> materials;
-  DevBuf<etxb_emitter_profile> profiles;
-  DevBuf<etxb_emitter> emitters;
-  DevBuf<DSpectrum> spectra;
-  DevBuf<DImage> images;
-  DevBuf<DMedium> mediums;
-  std::vector<DevBuf<float>> medium_density;
-  std::vector<DevBuf<uint8_t>> image_pixels, image_dists;
-  DevBuf<etxb_distribution_entry> emitter_dist;
-  DevBuf<BvhNode> bvh_nodes;
-  DevBuf<WideNode> wide_nodes;
-  bool wide_rejected = false;         // the committed geometry's 4-wide tree exceeds kWideStackSize (the scene walks the BVH2)
-  bool debug_trace_wide = false;      // etxb_debug_select_tree: etxb_debug_trace walks the 4-wide tree when the scene has one
-  DevBuf<float4> bvh_tris;
-  DevBuf<float> xyz_table, rgb_response_table;
-  DevBuf<uint8_t> bn_sobol, bn_scrambling, bn_ranking;
-  float y_integral = 0.0f;
-  DeviceScene dscene = {};
-  double bvh_build_seconds = 0.0;
-  SceneHashes hashes;
-
-  // per-path state + queues.  path_count = W * H sizes the film and every path-indexed buffer; launch_count = Film::pixel_count() is the
-  // number of paths an iteration traces: W * H at pixel size 1, ceil(W / s) * ceil(H / s) in the coarse preview
-  uint32_t width = 0, height = 0, path_count = 0, launch_count = 0;
-  uint32_t pixel_size = 1, target_pixel_size = 1;  // Film::pixel_size, and the one etxb_set_film_pixel_size stored for the next etxb_begin
-  DevBuf<float4> ray_o, ray_d, thr, mis, hit, gathered, merged, camera_value, bs_weight_pdf, bs_wo_eta;
-  DevBuf<uint4> misc;
-  DevBuf<uint2> bs_props;
-  DevBuf<float> wavelength;
-  DevBuf<uint32_t> queue_sorted, queue_keys, queue_keys_sorted;  // path queue grouped by hit material (scenes with stochastic BSDFs)
-  DevBuf<uint2> conn_list_sorted;
-  DevBuf<uint32_t> lv_count, lp_offset, queue_a, queue_b, queue_counts, sampler_end_light, sampler_end_camera, merge_key, conn_count;
-  DevBuf<float4> conn_rec;  // product build, scenes with a connection stage: kConnRecRows rows per path (kernels.cuh)
-  DevBuf<uint2> conn_list, shadow_span;
-  DevBuf<float4> shadow_p0, shadow_p1, shadow_value;
-  DevBuf<uint32_t> shadow_result, shadow_count, trace_cursor;  // trace_cursor: work cursor of k_shadow_resolve
-  // light vertices + grid
-  uint32_t lv_capacity = 0, max_light_vertices_cfg = 0;
-  DevBuf<LightVertexRec> lv_tmp, lv_final;
-  DevBuf<uint32_t> lv_tmp_count, overflow, grid_bbox, keys_in, keys_out, vals_in, vals_out;
-  DevBuf<uint2> cell_range;
-  DevBuf<float4> g_pos, g_nrm, g_win, g_thr;
-  DevBuf<uint8_t> cub_temp;
-  DevBuf<DeviceCounters> counters;
-  // film
-  DevBuf<float4> film_camera, film_light, film_light_iteration, film_out;
-
-  // unidirectional path tracer (SURVEY 8(f) N3): the same context renders with CPUPathTracing's algorithm once etxb_set_integrator selects it
-  uint32_t integrator = ETXB_INTEGRATOR_VCM;
-  etxb_pt_options pt_options = {1u, 1u, 1u, 1u};
-  DevBuf<float4> film_normals, film_albedo, film_adaptive;  // Film's Normals / Albedo / CameraAdaptive layers (allocated with the first PT run;
-                                                           // CameraAdaptive also with the first VCM camera pass)
-  DevBuf<float4> film_denoised;                             // Film's Denoised layer: the last etxb_denoise, zeros before it (StorageDenoised)
-  DevBuf<float4> denoise_u, denoise_var_raw, denoise_var;   // etxb_denoise scratch: colour with its flags, variance, smoothed variance
-  DevBuf<uint32_t> denoise_flag;                            // set by k_denoise_variance where a pixel has fewer than two samples
-  DevBuf<uint32_t> film_ldr;                                 // the tone-mapped RGBA8 frame of etxb_read_film_ldr
-  DevBuf<float4> film_view;                                  // the float4 frame of etxb_read_film_view (the RGBA8 one goes to film_ldr)
-  DevBuf<float4> reference;                                  // the viewer's reference image: W x H in storage order, empty when none is set
-  double reference_mean_rgb = 0.0;                           // its mean over pixels and RGB channels, the scale of rel_mse's epsilon
-  DevBuf<ErrorSums> error_blocks;                            // etxb_film_error: one record per block, then the final record
-  DevBuf<uint32_t> pt_info;                                  // InternalData (sample count, converged, tmp)
-  DevBuf<uint32_t> pt_mask;                                  // the noise estimate's active mask + kNoiseStats (kernels_pt.cuh)
-  DevBuf<float> pt_error;
-  uint32_t pixel_sampler_image = 0xffffffffu;
-  float pixel_sampler_radius = 1.0f, noise_threshold = 0.0f, radiance_clamp = 0.0f;
-  uint32_t scene_samples = 0;
-  uint32_t pt_pixels_processed = 0, pt_active_pixels = 0;  // active pixels of the last iteration; Film::active_pixel_count (over all ranks
-                                                           // on a context with a communicator)
-  float pt_noise_level = 0.0f;                             // Film::noise_level
-
-  etxb_vcm_options options = {};
-  uint32_t iteration = 0;            // absolute iteration index (VCMIteration::iteration)
-  bool external_iteration = false;   // etxb_set_next_iteration: the caller sets every iteration's index, it does not advance by itself
-  uint32_t completed = 0;            // iterations finished since etxb_begin
-  uint32_t rank = 0, world = 1;
-  bool group_lane = false;           // a lane of an etxb_group (etxb_group_create)
-  bool light_full = false;           // camera-split iterations (etxb_group replicas): the partition applies to the camera pass only, the light pass traces every path
-  uint32_t last_light_vertices = 0;
-  uint32_t overflow_flag = 0;
-  double last_iteration_time = 0.0, total_time = 0.0;
-  uint64_t kernel_launches = 0;
-  GridData grid = {};
-  // queue sizes from which a pass takes its large-queue branches (etxb_debug_set_thresholds; 0 = always, 0xffffffff = never), and what ran
-  etxb_debug_thresholds thresholds = kDefaultThresholds;
-  etxb_debug_branch_counts branch_counts = {};
-
-  // pixel-tile sharding across processes (one per GPU): NCCL communicator over NVLink, created by etxb_comm_init
-  ncclComm_t comm = nullptr;
-  cudaStream_t comm_stream = nullptr;  // highest priority: a collective's few CTAs start as soon as ANY slot frees up instead of queueing behind the
-                                       // tens of thousands of blocks of another lane's kernel (measured, 2 GPUs x 4 lanes: 43 ms per all-reduce waiting otherwise)
-  cudaEvent_t comm_ev_in = nullptr, comm_ev_out = nullptr;
-  DevBuf<uint32_t> comm_counts;   // [world] stored light vertices per rank (all-gathered every iteration)
-  DevBuf<float4> film_reduced;    // rank 0: sum of every rank's camera tiles (etxb_comm_reduce_film)
-  double comm_ms = 0.0;           // device time of the collectives of the iterations since etxb_begin
-
-  // etxb_enqueue_iteration is asynchronous (CPUVCM::update returns at once, vcm_cpu.cxx:264-276): the iteration's host loop — it reads queue
-  // sizes back between bounces — runs on this context's own worker thread; etxb_poll never blocks, etxb_wait drains
-  std::thread worker;
-  std::mutex worker_m;
-  std::condition_variable worker_cv, worker_idle;
-  uint32_t worker_queued = 0;
-  bool worker_busy = false, worker_quit = false;
-  int worker_error = ETXB_OK;
-
-  cudaEvent_t ev_iter_start = nullptr, ev_iter_stop = nullptr;
-  std::vector<TimedLaunch> timed;
-  std::vector<cudaEvent_t> event_pool;
-  size_t event_cursor = 0;
-  float kernel_ms[K_COUNT] = {};
-  uint32_t kernel_count[K_COUNT] = {};
-
-  // frees the device buffers; a C++ symbol, kept out of the library's exports (the interface is etxb_destroy)
-  __attribute__((visibility("hidden"))) ~etxb_ctx() = default;
-};
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Iterations in flight (etxb_group): L contexts on one device, one host thread each, pulling iteration indices from per-lane
@@ -452,25 +206,6 @@ NcclApi* nccl_api() {
   return api.handle ? &api : nullptr;
 }
 
-int fail(etxb_ctx* ctx, int code, const char* fmt, ...) {
-  char buf[1024];
-  va_list args;
-  va_start(args, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, args);
-  va_end(args);
-  if (ctx) ctx->error = buf;
-  return code;
-}
-
-#define CUDA_OK(ctx, call)                                                                                   \
-  do {                                                                                                       \
-    cudaError_t err__ = (call);                                                                              \
-    if (err__ != cudaSuccess) {                                                                              \
-      return fail(ctx, (err__ == cudaErrorMemoryAllocation) ? ETXB_ERR_OUT_OF_MEMORY : ETXB_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(err__), \
-        __FILE__, __LINE__);                                                                                 \
-    }                                                                                                        \
-  } while (0)
-
 #define NCCL_OK(ctx, call)                                                                                                 \
   do {                                                                                                                     \
     ncclResult_t res__ = (call);                                                                                           \
@@ -492,13 +227,6 @@ cudaError_t create_priority_stream(cudaStream_t* stream) {
   int prio_low = 0, prio_high = 0;
   if (cudaError_t err = cudaDeviceGetStreamPriorityRange(&prio_low, &prio_high)) return err;
   return cudaStreamCreateWithPriority(stream, cudaStreamNonBlocking, prio_high);
-}
-
-template <class T>
-int upload(etxb_ctx* ctx, DevBuf<T>& buf, const T* host, size_t n) {
-  CUDA_OK(ctx, buf.alloc(std::max<size_t>(n, 1)));
-  if (n) CUDA_OK(ctx, cudaMemcpyAsync(buf.ptr, host, n * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
-  return ETXB_OK;
 }
 
 cudaEvent_t next_event(etxb_ctx* ctx) {
@@ -620,8 +348,6 @@ LaunchParams make_params(etxb_ctx* ctx) {
   v.vm_normalization = 1.0f / eta_vcm;
   return p;
 }
-
-uint32_t blocks_for(uint32_t n, uint32_t block) { return (n + block - 1u) / block; }
 
 int read_u32(etxb_ctx* ctx, const uint32_t* dptr, uint32_t& out) {
   CUDA_OK(ctx, cudaMemcpyAsync(&out, dptr, 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1230,8 +956,6 @@ struct ScenePrep {
   bool have_wide = false;
 };
 
-double seconds_since(std::chrono::steady_clock::time_point t0) { return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(); }
-
 bool image_has_table(const etxb_image& im) {
   return (im.y_distribution.values.a != nullptr) && distribution_covers(im.y_distribution.values.count, im.isize[1]) && (im.x_distributions.count == im.isize[1]);
 }
@@ -1401,14 +1125,6 @@ int prepare_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, Sc
   h.valid = true;
   p.fingerprint_seconds = seconds_since(t0);
   return ETXB_OK;
-}
-
-// takes ownership of a cudaMalloc'd array of n elements
-template <class T>
-void adopt(DevBuf<T>& buf, T* ptr, size_t n) {
-  buf.release();
-  buf.ptr = ptr;
-  buf.count = n;
 }
 
 // a device-to-device copy into `dst`, sized as `src`
@@ -2838,142 +2554,6 @@ int etxb_read_buffer(etxb_ctx* ctx, uint32_t buffer_id, void* dst, uint64_t dst_
 
 void* etxb_stream(etxb_ctx* ctx) { return ctx ? (void*)ctx->stream : nullptr; }
 
-int etxb_debug_trace(etxb_ctx* ctx, const float* rays, uint32_t* seeds, uint32_t count, float* hits_uv_t, uint32_t* hits_tri) {
-  if (!ctx || !rays || !seeds || !hits_uv_t || !hits_tri) return ETXB_ERR_INVALID_ARGUMENT;
-  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
-  cudaSetDevice(ctx->device);
-  DevBuf<float> d_rays, d_uvt;
-  DevBuf<uint32_t> d_seeds, d_tri;
-  if (int rc = upload(ctx, d_rays, rays, size_t(count) * 8)) return rc;
-  if (int rc = upload(ctx, d_seeds, seeds, count)) return rc;
-  CUDA_OK(ctx, d_uvt.alloc(size_t(count) * 3));
-  CUDA_OK(ctx, d_tri.alloc(count));
-  const uint32_t wide = (ctx->debug_trace_wide && (ctx->dscene.wide_nodes != nullptr)) ? 1u : 0u;
-  k_debug_trace<<<blocks_for(count, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_rays.ptr, d_seeds.ptr, count, wide, d_uvt.ptr, d_tri.ptr);
-  ctx->kernel_launches += 1;
-  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-  CUDA_OK(ctx, cudaMemcpy(seeds, d_seeds.ptr, size_t(count) * 4, cudaMemcpyDeviceToHost));
-  CUDA_OK(ctx, cudaMemcpy(hits_uv_t, d_uvt.ptr, d_uvt.bytes(), cudaMemcpyDeviceToHost));
-  CUDA_OK(ctx, cudaMemcpy(hits_tri, d_tri.ptr, d_tri.bytes(), cudaMemcpyDeviceToHost));
-  return ETXB_OK;
-}
-
-int etxb_debug_occluded(etxb_ctx* ctx, const float* segments, uint32_t count, uint32_t* occluded) {
-  if (!ctx || !segments || !occluded) return ETXB_ERR_INVALID_ARGUMENT;
-  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
-  if (count == 0) return ETXB_OK;
-  cudaSetDevice(ctx->device);
-  DevBuf<float> d_segments;
-  DevBuf<uint32_t> d_occluded;
-  if (int rc = upload(ctx, d_segments, segments, size_t(count) * 6)) return rc;
-  CUDA_OK(ctx, d_occluded.alloc(count));
-  const uint32_t wide = (ctx->debug_trace_wide && (ctx->dscene.wide_nodes != nullptr)) ? 1u : 0u;
-  k_debug_occluded<<<blocks_for(count, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_segments.ptr, count, wide, d_occluded.ptr);
-  ctx->kernel_launches += 1;
-  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-  CUDA_OK(ctx, cudaMemcpy(occluded, d_occluded.ptr, d_occluded.bytes(), cudaMemcpyDeviceToHost));
-  return ETXB_OK;
-}
-
-// Test hook: both trees of a triangle soup from the host builder (the specification) or from the device builder, nothing committed
-int etxb_debug_build_trees(etxb_ctx* ctx, const float* positions, uint32_t vertex_count, const uint32_t* indices, uint32_t triangle_count, uint32_t device,
-  etxb_debug_trees* out) {
-  if (!ctx || !out || !out->bvh_nodes || !out->tri_pos || !out->tri_index || !out->wide_nodes || (device > 1u)) return ETXB_ERR_INVALID_ARGUMENT;
-  if ((triangle_count && !indices) || (vertex_count && !positions)) return ETXB_ERR_INVALID_ARGUMENT;
-  for (uint64_t i = 0; i < uint64_t(triangle_count) * 3u; ++i)
-    if (indices[i] >= vertex_count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "triangle %llu: vertex index out of range", (unsigned long long)(i / 3u));
-  const size_t cap = std::max<uint32_t>(triangle_count, 1u);
-  auto t0 = std::chrono::steady_clock::now();
-  if (device == 0u) {
-    Bvh bvh;
-    build_bvh(positions, 12u, indices, 12u, triangle_count, bvh);
-    WideBvh wide;
-    build_wide_bvh(bvh, wide);
-    out->seconds = seconds_since(t0);
-    memcpy(out->bvh_nodes, bvh.nodes.data(), bvh.nodes.size() * sizeof(BvhNode));
-    memcpy(out->tri_pos, bvh.tri_pos.data(), bvh.tri_pos.size() * sizeof(F4));
-    memcpy(out->tri_index, bvh.tri_index.data(), bvh.tri_index.size() * 4u);
-    memcpy(out->wide_nodes, wide.nodes.data(), wide.nodes.size() * sizeof(WideNode));
-    out->bvh_node_count = uint32_t(bvh.nodes.size());
-    out->slot_count = uint32_t(bvh.tri_index.size());
-    out->wide_node_count = uint32_t(wide.nodes.size());
-    out->max_depth = bvh.max_depth;
-    out->max_stack = wide.max_stack;
-    return ETXB_OK;
-  }
-  cudaSetDevice(ctx->device);
-  DevBuf<float> d_pos;
-  DevBuf<uint32_t> d_idx;
-  if (int rc = upload(ctx, d_pos, positions, size_t(vertex_count) * 3u)) return rc;
-  if (int rc = upload(ctx, d_idx, indices, size_t(triangle_count) * 3u)) return rc;
-  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-  t0 = std::chrono::steady_clock::now();
-  DeviceBvhOut bvh;
-  CUDA_OK(ctx, build_bvh_device(d_pos.ptr, 12u, d_idx.ptr, 12u, triangle_count, true, ctx->stream, bvh));
-  DevBuf<BvhNode> nodes;
-  DevBuf<F4> tri_pos;
-  DevBuf<uint32_t> tri_index;
-  adopt(nodes, bvh.nodes, cap);
-  adopt(tri_pos, bvh.tri_pos, cap * 3u);
-  adopt(tri_index, bvh.tri_index, cap);
-  DevBuf<WideNode> wide;
-  WideNode* w = nullptr;
-  uint32_t wide_count = 0, max_stack = 0;
-  CUDA_OK(ctx, build_wide_bvh_device(bvh.nodes, bvh.node_count, ctx->stream, &w, &wide_count, &max_stack));
-  adopt(wide, w, wide_count);
-  out->seconds = seconds_since(t0);
-  CUDA_OK(ctx, cudaMemcpy(out->bvh_nodes, bvh.nodes, size_t(bvh.node_count) * sizeof(BvhNode), cudaMemcpyDeviceToHost));
-  CUDA_OK(ctx, cudaMemcpy(out->tri_pos, bvh.tri_pos, size_t(bvh.slot_count) * 3u * sizeof(F4), cudaMemcpyDeviceToHost));
-  CUDA_OK(ctx, cudaMemcpy(out->tri_index, bvh.tri_index, size_t(bvh.slot_count) * 4u, cudaMemcpyDeviceToHost));
-  CUDA_OK(ctx, cudaMemcpy(out->wide_nodes, w, size_t(wide_count) * sizeof(WideNode), cudaMemcpyDeviceToHost));
-  out->bvh_node_count = bvh.node_count;
-  out->slot_count = bvh.slot_count;
-  out->wide_node_count = wide_count;
-  out->max_depth = bvh.max_depth;
-  out->max_stack = max_stack;
-  return ETXB_OK;
-}
-
-// Test hook: which tree etxb_debug_trace and etxb_debug_occluded walk (0: the BVH2 shared with the oracle; 1: the 4-wide quantised tree of the product build).  Returns 1
-// when the requested tree exists for the uploaded scene.
-int etxb_debug_select_tree(etxb_ctx* ctx, int wide) {
-  if (!ctx) return ETXB_ERR_INVALID_ARGUMENT;
-  ctx->debug_trace_wide = wide != 0;
-  return (!wide || (ctx->dscene.wide_nodes != nullptr)) ? 1 : 0;
-}
-
-int etxb_debug_sampler(etxb_ctx* ctx, const uint32_t* a, const uint32_t* b, uint32_t count, uint32_t draws, uint32_t* out_seed, float* out_values) {
-  if (!ctx || !a || !b || !out_seed || !out_values) return ETXB_ERR_INVALID_ARGUMENT;
-  cudaSetDevice(ctx->device);
-  DevBuf<uint32_t> da, db, ds;
-  DevBuf<float> dv;
-  if (int rc = upload(ctx, da, a, count)) return rc;
-  if (int rc = upload(ctx, db, b, count)) return rc;
-  CUDA_OK(ctx, ds.alloc(size_t(count) * (draws + 1)));
-  CUDA_OK(ctx, dv.alloc(size_t(count) * std::max(draws, 1u)));
-  k_debug_sampler<<<blocks_for(count, 128), 128, 0, ctx->stream>>>(da.ptr, db.ptr, count, draws, ds.ptr, dv.ptr);
-  ctx->kernel_launches += 1;
-  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-  CUDA_OK(ctx, cudaMemcpy(out_seed, ds.ptr, ds.bytes(), cudaMemcpyDeviceToHost));
-  if (draws) CUDA_OK(ctx, cudaMemcpy(out_values, dv.ptr, size_t(count) * draws * 4, cudaMemcpyDeviceToHost));
-  return ETXB_OK;
-}
-
-int etxb_debug_math(etxb_ctx* ctx, uint32_t fn, const float* x, const float* y, uint32_t count, float* out) {
-  if (!ctx || !x || !out) return ETXB_ERR_INVALID_ARGUMENT;
-  cudaSetDevice(ctx->device);
-  DevBuf<float> dx, dy, dout;
-  if (int rc = upload(ctx, dx, x, count)) return rc;
-  if (y)
-    if (int rc = upload(ctx, dy, y, count)) return rc;
-  CUDA_OK(ctx, dout.alloc(count));
-  k_debug_math<<<blocks_for(count, 128), 128, 0, ctx->stream>>>(ctx->dscene, fn, dx.ptr, y ? dy.ptr : nullptr, count, dout.ptr);
-  ctx->kernel_launches += 1;
-  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-  CUDA_OK(ctx, cudaMemcpy(out, dout.ptr, dout.bytes(), cudaMemcpyDeviceToHost));
-  return ETXB_OK;
-}
-
 // Test hook: etxb_denoise's kernels on host arrays (RGBA float per pixel, storage order; `counts` per pixel; guides may be null)
 int etxb_debug_denoise(etxb_ctx* ctx, const float* color, const float* camera, const float* half, const uint32_t* counts, const float* normals, const float* albedo,
                        uint32_t width, uint32_t height, float* out, float* out_variance) {
@@ -3094,257 +2674,6 @@ int etxb_debug_noise_estimate(etxb_ctx* ctx, uint32_t width, uint32_t height, ui
   }
   stats_out[0] = sum[words + kNoiseStatConverged];
   stats_out[1] = sum[words + kNoiseStatError];
-  return ETXB_OK;
-}
-
-// Test hook: the vertex closures of dclosure.cuh, query by query (layout and outputs in include/etx_b200.h)
-int etxb_debug_closure_eval(etxb_ctx* ctx, const etxb_closure_query* queries, uint32_t count, uint32_t repetitions, double* out) {
-  if (!ctx || !queries || !out || (repetitions == 0)) return ETXB_ERR_INVALID_ARGUMENT;
-  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
-  if (count == 0) return ETXB_OK;
-  for (uint32_t i = 0; i < count; ++i) {
-    if (queries[i].material >= ctx->materials.count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "closure query material index out of range");
-  }
-  cudaSetDevice(ctx->device);
-  DevBuf<etxb_closure_query> d_queries;
-  DevBuf<double> d_out;
-  if (int rc = upload(ctx, d_queries, queries, count)) return rc;
-  CUDA_OK(ctx, d_out.alloc(size_t(count) * ETXB_CLOSURE_STATS));
-  if (ctx->spectral) {
-    k_debug_closure<true><<<blocks_for(count, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
-  } else {
-    k_debug_closure<false><<<blocks_for(count, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
-  }
-  ctx->kernel_launches += 1;
-  CUDA_OK(ctx, cudaGetLastError());
-  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-  CUDA_OK(ctx, cudaMemcpy(out, d_out.ptr, d_out.bytes(), cudaMemcpyDeviceToHost));
-  return ETXB_OK;
-}
-
-// Test hook: bsdf_sample of dbsdf.cuh, query by query and repetition by repetition (layout and modes in include/etx_b200.h)
-int etxb_debug_bsdf_sample(etxb_ctx* ctx, const etxb_sample_query* queries, uint32_t count, uint32_t repetitions, etxb_sample_result* out) {
-  if (!ctx || !queries || !out || (repetitions == 0)) return ETXB_ERR_INVALID_ARGUMENT;
-  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
-  if (count == 0) return ETXB_OK;
-  if (uint64_t(count) * repetitions > 0x7fffffffull) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "%u queries x %u repetitions exceed 2^31 samples", count, repetitions);
-  for (uint32_t i = 0; i < count; ++i) {
-    if (queries[i].material >= ctx->materials.count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "sample query %u: material index out of range", i);
-    if (queries[i].mode > 1u) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "sample query %u: mode must be 0 or 1", i);
-  }
-  cudaSetDevice(ctx->device);
-  const uint32_t total = count * repetitions;
-  DevBuf<etxb_sample_query> d_queries;
-  DevBuf<etxb_sample_result> d_out;
-  if (int rc = upload(ctx, d_queries, queries, count)) return rc;
-  CUDA_OK(ctx, d_out.alloc(total));
-  if (ctx->spectral) {
-    k_debug_bsdf_sample<true><<<blocks_for(total, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
-  } else {
-    k_debug_bsdf_sample<false><<<blocks_for(total, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
-  }
-  ctx->kernel_launches += 1;
-  CUDA_OK(ctx, cudaGetLastError());
-  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-  CUDA_OK(ctx, cudaMemcpy(out, d_out.ptr, d_out.bytes(), cudaMemcpyDeviceToHost));
-  return ETXB_OK;
-}
-
-// Test hook: the emitter routines of dvcm.cuh, query by query and repetition by repetition (layout and ops in include/etx_b200.h)
-int etxb_debug_emitter(etxb_ctx* ctx, const etxb_emitter_query* queries, uint32_t count, uint32_t repetitions, etxb_emitter_result* out) {
-  if (!ctx || !queries || !out || (repetitions == 0)) return ETXB_ERR_INVALID_ARGUMENT;
-  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
-  if (count == 0) return ETXB_OK;
-  if (uint64_t(count) * repetitions > 0x7fffffffull) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "%u queries x %u repetitions exceed 2^31 samples", count, repetitions);
-  if (ctx->emitters.count == 0) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "the scene has no emitter");
-  for (uint32_t i = 0; i < count; ++i) {
-    if (queries[i].op > ETXB_EMITTER_RADIANCE) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "emitter query %u: op must be 0 to 3", i);
-    const bool indexed = (queries[i].op == ETXB_EMITTER_SAMPLE_IN) || (queries[i].op == ETXB_EMITTER_RADIANCE);
-    if (indexed && (queries[i].emitter >= ctx->emitters.count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "emitter query %u: emitter index out of range", i);
-  }
-  cudaSetDevice(ctx->device);
-  const uint32_t total = count * repetitions;
-  DevBuf<etxb_emitter_query> d_queries;
-  DevBuf<etxb_emitter_result> d_out;
-  if (int rc = upload(ctx, d_queries, queries, count)) return rc;
-  CUDA_OK(ctx, d_out.alloc(total));
-  if (ctx->spectral) {
-    k_debug_emitter<true><<<blocks_for(total, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
-  } else {
-    k_debug_emitter<false><<<blocks_for(total, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
-  }
-  ctx->kernel_launches += 1;
-  CUDA_OK(ctx, cudaGetLastError());
-  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-  CUDA_OK(ctx, cudaMemcpy(out, d_out.ptr, d_out.bytes(), cudaMemcpyDeviceToHost));
-  return ETXB_OK;
-}
-
-// Test hook: the media routines of dmedium.cuh and the shadow-ray walk of dtrace.cuh, query by query and repetition by repetition (layout
-// and ops in include/etx_b200.h).  Every query is checked before the launch against what makes those loops end: a finite local segment,
-// tracking steps that still advance t in float32, and a free-flight redraw loop that ends in a few thousand draws on average.
-namespace {
-constexpr double kMediumCoordMax = 1e15;       // |world coordinate| of an origin or an end point
-constexpr double kMediumLocalSegmentMax = 1e18;  // local segment length: its float32 square stays finite
-constexpr double kMediumTrackingMax = 65536.0;   // max_sigma x (|local origin| + 2): a mean tracking step of ~1000 float32 ulps of t or more
-constexpr double kMediumRedrawMax = 8.0;         // extinction x kRayEpsilon: the homogeneous redraw loop runs exp(8) ~ 3000 times on average
-
-// A heterogeneous medium's tracking from a to b (world points; b = nullptr: a only) ends: finite local points, a local segment whose
-// float32 length is finite, and steps of 1 / max_sigma well above an ulp of the local t.
-bool tracking_bounded(const DMedium& m, const double* a, const double* b) {
-  if ((m.cls != 1u) || !(m.max_sigma > 0.0f)) return true;
-  const double lo[3] = {m.bounds_min.x, m.bounds_min.y, m.bounds_min.z}, hi[3] = {m.bounds_max.x, m.bounds_max.y, m.bounds_max.z};
-  double magnitude = 0.0, length2 = 0.0;
-  for (int k = 0; k < 3; ++k) {
-    const double ext = hi[k] - lo[k];
-    if (!(ext > 0.0)) return false;
-    const double pa = (a[k] - lo[k]) / ext, pb = b ? (b[k] - lo[k]) / ext : pa;
-    if (!std::isfinite(pa) || !std::isfinite(pb)) return false;
-    magnitude = std::max(magnitude, std::fabs(pa));
-    length2 += (pb - pa) * (pb - pa);
-  }
-  return (std::sqrt(length2) <= kMediumLocalSegmentMax) && (double(m.max_sigma) * (magnitude + 2.0) <= kMediumTrackingMax);
-}
-
-double spectrum_max(const std::vector<DSpectrum>& spectra, uint32_t index) {
-  if (index >= spectra.size()) return 0.0;
-  const DSpectrum& s = spectra[index];
-  double v = std::max({double(s.rgb[0]), double(s.rgb[1]), double(s.rgb[2])});
-  for (float p : s.power) v = std::max(v, double(p));
-  return v;
-}
-}  // namespace
-
-int etxb_debug_medium(etxb_ctx* ctx, const etxb_medium_query* queries, uint32_t count, uint32_t repetitions, etxb_medium_result* out) {
-  if (!ctx || !queries || !out || (repetitions == 0)) return ETXB_ERR_INVALID_ARGUMENT;
-  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
-  if (count == 0) return ETXB_OK;
-  if (uint64_t(count) * repetitions > 0x7fffffffull) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "%u queries x %u repetitions exceed 2^31 samples", count, repetitions);
-  cudaSetDevice(ctx->device);
-  std::vector<DMedium> meds(ctx->mediums.count);
-  std::vector<DSpectrum> spectra(ctx->spectra.count);
-  if (!meds.empty()) CUDA_OK(ctx, cudaMemcpy(meds.data(), ctx->mediums.ptr, meds.size() * sizeof(DMedium), cudaMemcpyDeviceToHost));
-  if (!spectra.empty()) CUDA_OK(ctx, cudaMemcpy(spectra.data(), ctx->spectra.ptr, spectra.size() * sizeof(DSpectrum), cudaMemcpyDeviceToHost));
-  const auto bounded3 = [](const float* v) {
-    return (std::fabs(double(v[0])) <= kMediumCoordMax) && (std::fabs(double(v[1])) <= kMediumCoordMax) && (std::fabs(double(v[2])) <= kMediumCoordMax);
-  };
-  for (uint32_t i = 0; i < count; ++i) {
-    const etxb_medium_query& q = queries[i];
-    if (q.op > ETXB_MEDIUM_SEGMENT) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: op must be 0 to 5", i);
-    if (ctx->spectral && !std::isfinite(q.wavelength)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: non-finite wavelength", i);
-    const bool unset = (q.op == ETXB_MEDIUM_SEGMENT) && (q.medium == ETXB_INVALID_INDEX);
-    if ((q.op != ETXB_MEDIUM_PHASE) && !unset && (q.medium >= meds.size())) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: medium index out of range", i);
-    if ((q.op == ETXB_MEDIUM_DENSITY) && (ctx->medium_density[q.medium].count == 0)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: density of a homogeneous medium", i);
-    if ((q.op != ETXB_MEDIUM_PHASE) && !bounded3(q.origin)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: origin not finite or past 1e15", i);
-    const double o[3] = {q.origin[0], q.origin[1], q.origin[2]};
-    if (q.op == ETXB_MEDIUM_SEGMENT) {
-      if (!bounded3(q.end)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: segment end not finite or past 1e15", i);
-      // every medium the walk can track through starts from a point of the segment: bound both ends in each heterogeneous medium
-      const double e[3] = {q.end[0], q.end[1], q.end[2]};
-      for (const DMedium& m : meds) {
-        if (!tracking_bounded(m, o, e) || !tracking_bounded(m, e, o)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: segment too far from a heterogeneous medium to track", i);
-      }
-      continue;
-    }
-    if (q.op == ETXB_MEDIUM_DENSITY) continue;
-    const float* d = q.direction;
-    if (!std::isfinite(d[0]) || !std::isfinite(d[1]) || !std::isfinite(d[2]) || ((d[0] == 0.0f) && (d[1] == 0.0f) && (d[2] == 0.0f)))
-      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: zero or non-finite direction", i);
-    if (q.op == ETXB_MEDIUM_PHASE) continue;
-    if (!std::isfinite(q.max_t) && (q.max_t != kMaxFloat)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: non-finite max_t", i);
-    if ((q.op == ETXB_MEDIUM_SAMPLE) && !(q.max_t >= kRayEpsilon)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: sample needs max_t >= kRayEpsilon", i);
-    if (!std::isfinite(q.throughput[0]) || !std::isfinite(q.throughput[1]) || !std::isfinite(q.throughput[2]))
-      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: non-finite throughput", i);
-    const DMedium& m = meds[q.medium];
-    if (q.max_t < kMaxFloat) {  // medium_intersects_bounds refuses max_t = kMaxFloat before any arithmetic
-      double e[3];
-      for (int k = 0; k < 3; ++k) e[k] = o[k] + double(d[k]) * double(q.max_t);
-      if (!(std::fabs(e[0]) <= 1e30) || !(std::fabs(e[1]) <= 1e30) || !(std::fabs(e[2]) <= 1e30))
-        return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: the segment's end overflows", i);
-      if (!tracking_bounded(m, o, e)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: segment too long or too far from the medium to track", i);
-    }
-    if ((q.op == ETXB_MEDIUM_SAMPLE) && (m.cls == 0u) &&
-        ((spectrum_max(spectra, m.absorption_index) + spectrum_max(spectra, m.scattering_index)) * kRayEpsilon > kMediumRedrawMax))
-      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium query %u: extinction too high for the free-flight redraw loop", i);
-  }
-  const uint32_t total = count * repetitions;
-  DevBuf<etxb_medium_query> d_queries;
-  DevBuf<etxb_medium_result> d_out;
-  if (int rc = upload(ctx, d_queries, queries, count)) return rc;
-  CUDA_OK(ctx, d_out.alloc(total));
-  if (ctx->spectral) {
-    k_debug_medium<true><<<blocks_for(total, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
-  } else {
-    k_debug_medium<false><<<blocks_for(total, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
-  }
-  ctx->kernel_launches += 1;
-  CUDA_OK(ctx, cudaGetLastError());
-  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-  CUDA_OK(ctx, cudaMemcpy(out, d_out.ptr, d_out.bytes(), cudaMemcpyDeviceToHost));
-  return ETXB_OK;
-}
-
-// Test hook: the subsurface routines of dsss.cuh, query by query and repetition by repetition (layout and ops in include/etx_b200.h).
-// Every loop they run is bounded (a traversal of the tree, at most 1024 random-walk steps), so the checks are on indices and finite inputs.
-int etxb_debug_subsurface(etxb_ctx* ctx, const etxb_subsurface_query* queries, uint32_t count, uint32_t repetitions, etxb_subsurface_result* out) {
-  if (!ctx || !queries || !out || (repetitions == 0)) return ETXB_ERR_INVALID_ARGUMENT;
-  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
-  if (count == 0) return ETXB_OK;
-  if (uint64_t(count) * repetitions > 0x7fffffffull) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "%u queries x %u repetitions exceed 2^31 samples", count, repetitions);
-  cudaSetDevice(ctx->device);
-  std::vector<etxb_material> mats(ctx->materials.count);
-  std::vector<DTriangle> tris(ctx->triangles.count);
-  if (!mats.empty()) CUDA_OK(ctx, cudaMemcpy(mats.data(), ctx->materials.ptr, mats.size() * sizeof(etxb_material), cudaMemcpyDeviceToHost));
-  if (!tris.empty()) CUDA_OK(ctx, cudaMemcpy(tris.data(), ctx->triangles.ptr, tris.size() * sizeof(DTriangle), cudaMemcpyDeviceToHost));
-  const auto finite = [](const float* v, int n) {
-    for (int k = 0; k < n; ++k)
-      if (!std::isfinite(v[k])) return false;
-    return true;
-  };
-  for (uint32_t i = 0; i < count; ++i) {
-    const etxb_subsurface_query& q = queries[i];
-    if (q.op > ETXB_SUBSURFACE_GATHER) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: op must be 0 to 4", i);
-    if (ctx->spectral && !std::isfinite(q.wavelength)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: non-finite wavelength", i);
-    if (q.op == ETXB_SUBSURFACE_REMAP) {
-      if (!finite(q.color, 3) || !finite(q.distances, 3)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: non-finite color or distance", i);
-      continue;
-    }
-    const float* d = q.dir;
-    if (!finite(d, 3) || ((d[0] == 0.0f) && (d[1] == 0.0f) && (d[2] == 0.0f)))
-      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: zero or non-finite direction", i);
-    if (q.op <= ETXB_SUBSURFACE_CONTINUOUS_TRACE) {
-      if ((q.material != ETXB_INVALID_INDEX) && (q.material >= mats.size())) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: material index out of range", i);
-      if (!finite(q.origin, 3) || !std::isfinite(q.t_min) || !std::isfinite(q.t_max))
-        return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: non-finite origin or ray interval", i);
-      if ((q.op == ETXB_SUBSURFACE_CONTINUOUS_TRACE) && ((q.max_count == 0) || (q.max_count > 8u)))
-        return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: max_count must be 1 to 8", i);
-      continue;
-    }
-    if (q.triangle >= tris.size()) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: triangle index out of range", i);
-    if (!std::isfinite(q.u) || !std::isfinite(q.v)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: non-finite barycentric coordinates", i);
-    if (q.op == ETXB_SUBSURFACE_PROFILE) {
-      if (q.direction > 2u) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: probe direction must be 0 to 2", i);
-      if (!std::isfinite(q.rnd) || !std::isfinite(q.radius) || !finite(q.normal, 3))
-        return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: non-finite rnd, radius or normal", i);
-    } else if (mats[tris[q.triangle].material_index].subsurface.cls == 0u) {
-      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "subsurface query %u: gather on a material without subsurface scattering", i);
-    }
-  }
-  const uint32_t total = count * repetitions;
-  DevBuf<etxb_subsurface_query> d_queries;
-  DevBuf<etxb_subsurface_result> d_out;
-  if (int rc = upload(ctx, d_queries, queries, count)) return rc;
-  CUDA_OK(ctx, d_out.alloc(total));
-  CUDA_OK(ctx, cudaMemsetAsync(d_out.ptr, 0, d_out.bytes(), ctx->stream));  // the kernel writes only the fields its op names
-  if (ctx->spectral) {
-    k_debug_subsurface<true><<<blocks_for(total, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
-  } else {
-    k_debug_subsurface<false><<<blocks_for(total, 128), 128, 0, ctx->stream>>>(ctx->dscene, d_queries.ptr, count, repetitions, d_out.ptr);
-  }
-  ctx->kernel_launches += 1;
-  CUDA_OK(ctx, cudaGetLastError());
-  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-  CUDA_OK(ctx, cudaMemcpy(out, d_out.ptr, d_out.bytes(), cudaMemcpyDeviceToHost));
   return ETXB_OK;
 }
 
