@@ -10,7 +10,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["module.cu", "test_hooks.cu", "bvh_build.cpp", "bvh_build_device.cu", "film_io.cpp", "scene_loader.cpp"]
+SOURCES = ["module.cu", "scene_upload.cu", "group.cu", "test_hooks.cu", "bvh_build.cpp", "bvh_build_device.cu", "film_io.cpp", "scene_loader.cpp"]
 HEADERS = ["bvh.h", "bvh_build.h", "bvh_build_device.h", "context.cuh", "dcore.cuh", "dscene.cuh", "dimage.cuh", "dbsdf.cuh", "dclosure.cuh", "dtrace.cuh", "dtrav.cuh", "dwide.cuh", "dmedium.cuh", "dsss.cuh", "dvcm.cuh", "dpt.cuh", "kernels.cuh", "kernels_pt.cuh", "kernels_denoise.cuh", "kernels_view.cuh", "portable_math.h", "scene_loader_formats.inl", "scene_loader_build.inl", "scene_loader_atmosphere.inl", "scene_loader_tangents.inl", "scene_loader_nvdb.inl", "scene_loader_jpeg.inl",
            os.path.join("..", "..", "include", "etx_b200.h")]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
@@ -30,10 +30,13 @@ def lib_path(flavor="fast"):
     return FLAVORS[flavor][0]
 
 
-# what each translation unit includes (the per-flavour objects are rebuilt when one of these is newer)
+# what each translation unit includes (the per-flavour objects are rebuilt when one of these is newer); only module.cu includes kernels*.cuh
+_CONTEXT_HEADERS = [h for h in HEADERS if not h.endswith(".inl") and not h.startswith("kernels")]
 UNIT_DEPS = {
     "module.cu": [h for h in HEADERS if not h.endswith(".inl")],
-    "test_hooks.cu": [h for h in HEADERS if not h.endswith(".inl") and not h.startswith("kernels")],
+    "scene_upload.cu": _CONTEXT_HEADERS,
+    "group.cu": _CONTEXT_HEADERS,
+    "test_hooks.cu": _CONTEXT_HEADERS,
     "bvh_build.cpp": ["bvh.h", "bvh_build.h"],
     "bvh_build_device.cu": ["bvh.h", "bvh_build_device.h"],
     "film_io.cpp": [os.path.join("..", "..", "include", "etx_b200.h")],

@@ -1,7 +1,7 @@
-// context.cuh — the context behind the C interface (struct etxb_ctx) and the host helpers of the two units that drive it: module.cu (the
-// product: context, scene upload, passes, film, group, NCCL) and test_hooks.cu (the test hooks that run the d*.cuh routines on host-given
-// queries).  No kernels*.cuh here: their non-template kernels have host stubs with external linkage, and a second unit that included them
-// would not link; etxb_ctx names two of their types by declaration only.
+// context.cuh — the context behind the C interface (struct etxb_ctx) and the host helpers of the units that drive it: module.cu (the
+// product: context, passes, film, NCCL), scene_upload.cu (the scene upload and update), group.cu (the iteration group, etxb_group) and
+// test_hooks.cu (the test hooks that run the d*.cuh routines on host-given queries).  No kernels*.cuh here: their non-template kernels have
+// host stubs with external linkage, and a second unit that included them would not link; etxb_ctx names two of their types by declaration only.
 #pragma once
 #include <algorithm>
 #include <chrono>
@@ -118,7 +118,7 @@ struct TimedLaunch {
   cudaEvent_t start, stop;
 };
 
-// a 128-bit content hash (hash128, module.cu)
+// a 128-bit content hash (hash128, scene_upload.cu)
 struct Hash128 {
   uint64_t lo = 0, hi = 0;
   bool operator==(const Hash128& o) const { return (lo == o.lo) && (hi == o.hi); }
@@ -308,5 +308,94 @@ void adopt(DevBuf<T>& buf, T* ptr, size_t n) {
 inline uint32_t blocks_for(uint32_t n, uint32_t block) { return (n + block - 1u) / block; }
 
 inline double seconds_since(std::chrono::steady_clock::time_point t0) { return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(); }
+
+// ---- the scene upload and update (scene_upload.cu) ----------------------------------------------------------------------------------------
+// etxb_upload_scene, etxb_update_scene and etxb_group_update_scene run the same stages: validate_scene makes every check and touches nothing
+// on the device, prepare_scene hashes the bulk arrays (prepare_bvh uploads a new geometry and builds its BVH2 on the device), commit_scene
+// commits to the device.  An update keeps the device copies whose content hashes did not change; everything small is derived from the PODs
+// again on every call.
+struct SceneClass {
+  bool stochastic = false;  // has_stochastic_merge
+  bool boundaries = false, subsurface = false, deferred = false, opaque = false, plain = false;
+};
+
+struct ScenePrep {
+  SceneClass cls;
+  SceneHashes hashes;
+  double fingerprint_seconds = 0.0, bvh_seconds = 0.0;
+  uint64_t bytes_hashed = 0;
+  // a new geometry's device copies and BVH2 (prepare_bvh: built once, copied into each context that commits it)
+  DevBuf<DVertex> vertices;
+  DevBuf<DTriangle> triangles;
+  DevBuf<BvhNode> bvh_nodes;
+  DevBuf<float4> bvh_tris;
+  uint32_t max_depth = 0;
+  bool have_bvh = false;
+  DevBuf<WideNode> wide;  // the 4-wide tree collapsed from the first committing context's BVH2
+  uint32_t max_stack = 0;
+  bool have_wide = false;
+};
+
+int check_scene_args(etxb_ctx* ctx, uint64_t scene_bytes, uint64_t camera_bytes);
+int prepare_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, ScenePrep& p);
+int prepare_bvh(etxb_ctx* ctx, const etxb_scene& s, ScenePrep& p);
+bool geometry_kept(const etxb_ctx* ctx, const ScenePrep& p, bool reuse);
+int commit_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, ScenePrep& p, bool reuse, etxb_update_info* info);
+
+// ---- the driver (module.cu) ------------------------------------------------------------------------------------------------------------------
+// commit_scene's last step: the film and path-state buffers for the committed scene class and film size (Film::allocate), counting the
+// allocations it makes (none: an update kept the path state)
+int commit_path_state(etxb_ctx* ctx, const etxb_camera& cam, bool reuse, uint32_t* allocations);
+// one whole iteration on the calling thread; returns when it has finished (the bounce loops read queue sizes back)
+int run_iteration_blocking(etxb_ctx* ctx);
+// blocks until every queued iteration of the context's worker has finished; returns (and clears) the first error one of them hit
+int ctx_drain(etxb_ctx* ctx);
+// Film::layer's read-out of `layer` (film.cxx:381-418) from `raw`, the buffer the layer is made from: Result = max(0, raw + light) and
+// Normals = raw * 0.5 + 0.5 are written to `out`, which is returned; every other layer is `raw` as it is.  Asynchronous on `stream`.
+const float4* film_layer_finish(uint32_t layer, float4* raw, float4* light, uint32_t width, uint32_t height, float4* out, cudaStream_t stream);
+
+// NCCL is bound at run time: a single-GPU host needs no libnccl, and a torch host that already loaded its bundled libnccl.so.2 shares it.
+struct NcclApi {
+  void* handle = nullptr;
+  ncclResult_t (*GetUniqueId)(ncclUniqueId*) = nullptr;
+  ncclResult_t (*CommInitRank)(ncclComm_t*, int, ncclUniqueId, int) = nullptr;
+  ncclResult_t (*CommDestroy)(ncclComm_t) = nullptr;
+  ncclResult_t (*AllReduce)(const void*, void*, size_t, ncclDataType_t, ncclRedOp_t, ncclComm_t, cudaStream_t) = nullptr;
+  ncclResult_t (*AllGather)(const void*, void*, size_t, ncclDataType_t, ncclComm_t, cudaStream_t) = nullptr;
+  ncclResult_t (*Reduce)(const void*, void*, size_t, ncclDataType_t, ncclRedOp_t, int, ncclComm_t, cudaStream_t) = nullptr;
+  ncclResult_t (*Broadcast)(const void*, void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
+  ncclResult_t (*GroupStart)() = nullptr;
+  ncclResult_t (*GroupEnd)() = nullptr;
+  const char* (*GetErrorString)(ncclResult_t) = nullptr;
+};
+// the bound library, or null where it could not be loaded
+NcclApi* nccl_api();
+
+#define NCCL_OK(ctx, call)                                                                                                 \
+  do {                                                                                                                     \
+    ncclResult_t res__ = (call);                                                                                           \
+    if (res__ != ncclSuccess) return fail(ctx, ETXB_ERR_CUDA, "%s failed: %s (%s:%d)", #call, nccl_api()->GetErrorString(res__), __FILE__, __LINE__); \
+  } while (0)
+
+// Joins rank `rank` of a `world`-rank communicator on the current device; `id` holds the ncclUniqueId rank 0 made.  Collective.
+int comm_init_rank(etxb_ctx* ctx, ncclComm_t* comm, uint32_t world, uint32_t rank, const void* id);
+// A stream at the device's highest priority, so that its few blocks do not queue behind the lanes' large kernels
+cudaError_t create_priority_stream(cudaStream_t* stream);
+
+// The end of a film reduce to rank 0 on `stream`: a rank other than 0 waits for its part and returns; rank 0 checks the host buffer, finishes
+// the layer (`finish(&src)` leaves the device buffer that holds it in src) and copies it to `dst`.  Errors go to `ctx`.
+template <class Finish>
+int end_rank0_reduce(etxb_ctx* ctx, cudaStream_t stream, uint32_t rank, float* dst, uint64_t dst_bytes, size_t pixels, Finish&& finish) {
+  if (rank != 0u) {
+    CUDA_OK(ctx, cudaStreamSynchronize(stream));
+    return ETXB_OK;
+  }
+  if (!dst || (dst_bytes < pixels * 16u)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "film buffer too small");
+  const float4* src = nullptr;
+  if (int rc = finish(&src)) return rc;
+  CUDA_OK(ctx, cudaMemcpyAsync(dst, src, pixels * 16u, cudaMemcpyDeviceToHost, stream));
+  CUDA_OK(ctx, cudaStreamSynchronize(stream));
+  return ETXB_OK;
+}
 
 }  // namespace etxb_internal

@@ -1,7 +1,7 @@
-// module.cu — C ABI (include/etx_b200.h) over the wavefront kernels: context, scene upload, iteration driver.
-// Host-side counterpart of CPUVCMImpl (sources/etx/rt/integrators/vcm_cpu.cxx:30-241) and of
-// Raytracing::commit_changes (sources/etx/rt/rt.cxx:58-88).  The context is declared in context.cuh; the test hooks that run the d*.cuh
-// routines on host-given queries are in test_hooks.cu.
+// module.cu — C ABI (include/etx_b200.h) over the wavefront kernels: context, iteration driver, film, NCCL.
+// Host-side counterpart of CPUVCMImpl (sources/etx/rt/integrators/vcm_cpu.cxx:30-241).  The context is declared in context.cuh; the scene
+// upload and update are in scene_upload.cu (its last step, the path-state buffers the kernels size, is commit_path_state here), the iteration
+// group in group.cu, and the test hooks that run the d*.cuh routines on host-given queries in test_hooks.cu.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
@@ -9,7 +9,6 @@
 #include <cstdlib>
 #include <cstring>
 #include <ctime>
-#include <deque>
 
 #include <dlfcn.h>
 
@@ -27,157 +26,8 @@ static const char* kFlavor = "parity";
 static const char* kFlavor = "fast";
 #endif
 
-namespace {
+namespace etxb_internal __attribute__((visibility("hidden"))) {
 
-// 128-bit content hash of a byte range, chained through `seed`: four independent 64-bit multiply-rotate lanes over 32-byte stripes (the
-// round of xxHash64), a zero-padded tail, and two differently mixed 64-bit digests of the lanes and the length.  It detects edits, not
-// adversaries.
-constexpr uint64_t kHashP1 = 0x9E3779B185EBCA87ull, kHashP2 = 0xC2B2AE3D27D4EB4Full, kHashP3 = 0x165667B19E3779F9ull, kHashP4 = 0x85EBCA77C2B2AE63ull;
-inline uint64_t rotl64(uint64_t x, int r) { return (x << r) | (x >> (64 - r)); }
-inline uint64_t hash_round(uint64_t acc, uint64_t w) { return rotl64(acc + w * kHashP2, 31) * kHashP1; }
-inline uint64_t hash_mix(uint64_t h) {
-  h ^= h >> 33;
-  h *= kHashP2;
-  h ^= h >> 29;
-  h *= kHashP3;
-  return h ^ (h >> 32);
-}
-Hash128 hash128(const void* data, size_t bytes, Hash128 seed) {
-  const uint8_t* p = static_cast<const uint8_t*>(data);
-  uint64_t v[4] = {seed.lo + kHashP1 + kHashP2, seed.hi + kHashP2, seed.lo ^ kHashP3, seed.hi - kHashP1};
-  size_t i = 0;
-  for (; i + 32 <= bytes; i += 32) {
-    uint64_t w[4];
-    memcpy(w, p + i, 32);
-    for (int k = 0; k < 4; ++k) v[k] = hash_round(v[k], w[k]);
-  }
-  uint64_t tail[4] = {0, 0, 0, 0};
-  if (bytes > i) memcpy(tail, p + i, bytes - i);
-  for (int k = 0; k < 4; ++k) v[k] = hash_round(v[k], tail[k]);
-  const uint64_t a = rotl64(v[0], 1) + rotl64(v[1], 7) + rotl64(v[2], 12) + rotl64(v[3], 18);
-  const uint64_t b = (v[0] * kHashP4) ^ rotl64(v[1], 29) ^ (v[2] * kHashP3) ^ rotl64(v[3], 43);
-  return {hash_mix(a ^ (uint64_t(bytes) * kHashP4)), hash_mix(b + uint64_t(bytes) * kHashP1)};
-}
-}  // namespace
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Iterations in flight (etxb_group): L contexts on one device, one host thread each, pulling iteration indices from per-lane
-// queues (WorkPlan).  VCM iterations are independent (vcm_cpu.cxx:95-113: the index only sets the merge radius and the sampler seeds), and
-// the bounce loop of one iteration ends in a long latency-bound tail (a few thousand paths, ~50 bounces); with several iterations in
-// flight that tail overlaps the full-width head of another iteration.  The film is the mean of the lanes' films weighted by the
-// iterations each lane finished — the same set of iterations, hence the same estimate, as one context running them in sequence.
-// ---------------------------------------------------------------------------------------------------------------------
-extern "C" {  // the film-combine kernels keep unmangled names in the module
-constexpr uint32_t kMaxLanes = 9;  // 8 whole-iteration lanes + the camera-split lane of the replica mode
-struct FilmLanes {
-  const float4* camera[kMaxLanes];
-  const float4* light[kMaxLanes];
-  float weight[kMaxLanes];        // camera layer
-  float weight_light[kMaxLanes];  // light layer (differs from `weight` only for a camera-split lane that is not part 0)
-  float weight_count[kMaxLanes];  // raw mode: what the lane adds to .w
-  uint32_t lanes, layer, pixels;
-  uint32_t raw;  // 1: no clamp, alpha = sum of the weights (a partial sum that another stage finishes)
-};
-__global__ void __launch_bounds__(256) k_film_combine(FilmLanes f, float4* out) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= f.pixels) return;
-  float x = 0.0f, y = 0.0f, z = 0.0f;
-  for (uint32_t l = 0; l < f.lanes; ++l) {
-    float4 c = (f.layer != ETXB_FILM_LIGHT) ? f.camera[l][i] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-    float4 g = (f.layer != ETXB_FILM_CAMERA) ? f.light[l][i] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-    x += f.weight[l] * c.x + f.weight_light[l] * g.x;
-    y += f.weight[l] * c.y + f.weight_light[l] * g.y;
-    z += f.weight[l] * c.z + f.weight_light[l] * g.z;
-  }
-  if (f.raw) {
-    float w = 0.0f;
-    for (uint32_t l = 0; l < f.lanes; ++l) w += f.weight_count[l];
-    out[i] = make_float4(x, y, z, w);
-    return;
-  }
-  if (f.layer == ETXB_FILM_RESULT) {  // Film::layer(Result): max(0, camera + light) (film.cxx:381-418)
-    x = fmaxf(0.0f, x);
-    y = fmaxf(0.0f, y);
-    z = fmaxf(0.0f, z);
-  }
-  out[i] = make_float4(x, y, z, 1.0f);
-}
-// rank 0 of a replica run: the reduced sum of (iterations x mean film) over the ranks -> the mean over all iterations (.w carries the count)
-__global__ void __launch_bounds__(256) k_film_finish_mean(const float4* sum, float4* out, uint32_t pixels, uint32_t clamp) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= pixels) return;
-  float4 v = sum[i];
-  float inv = (v.w > 0.0f) ? 1.0f / v.w : 0.0f;
-  float x = v.x * inv, y = v.y * inv, z = v.z * inv;
-  if (clamp) {
-    x = fmaxf(0.0f, x);
-    y = fmaxf(0.0f, y);
-    z = fmaxf(0.0f, z);
-  }
-  out[i] = make_float4(x, y, z, 1.0f);
-}
-}  // extern "C"
-
-// Which lane renders which iteration of an etxb_group.  etxb_group_enqueue deals the new ordinals into queues (plan_enqueue, the one place
-// that reads the mode); lane l pops queues[lane_queue[l]], whatever the mode.
-//   local     one GPU: every lane reads queue 0, which holds the ordinals in order, so a free lane takes the next one
-//   tiles     etxb_group_comm_init, world >= 2: lane l reads queue l, which holds the ordinals l, l + L, l + 2L, ... on EVERY rank (lane l of every
-//             rank shares a communicator; one shared queue would pair different iterations across ranks)
-//   replicas  etxb_group_comm_init_replicas, world >= 2: replica_plan deals the job's ordinals; whole frames go to queue 0, which every lane but
-//             the split lane reads, and camera-split parts to the split lane's own queue
-// The split lane reads its own queue in every mode, which only the replica mode fills; tile mode and a split lane refuse each other.
-struct WorkItem {
-  uint32_t ordinal;      // of the iteration within the job
-  uint32_t part, parts;  // parts == 1: the whole frame; else the camera pass of part `part` (tile % parts == part), light pass in full
-};
-enum class GroupMode : uint32_t { local = 0, tiles = 1, replicas = 2 };  // the values etxb_debug_group_plan takes
-struct WorkPlan {
-  GroupMode mode = GroupMode::local;
-  uint32_t world = 1, rank = 0;
-  uint32_t enqueued = 0;                     // iterations enqueued since etxb_group_begin: the next ordinal
-  uint32_t split_lane = 0xffffffffu;         // the lane reserved for camera-split iterations (etxb_group_reserve_split_lane), or none
-  uint32_t split_part = 0, split_parts = 0;  // the (part, parts) that lane's film is made of; 0 parts = not used yet
-  std::vector<std::deque<WorkItem>> queues;  // one per lane
-  std::vector<uint32_t> lane_queue;
-};
-
-struct etxb_group {
-  std::vector<etxb_ctx*> lanes;
-  std::vector<std::thread> workers;
-  std::mutex m;
-  std::condition_variable cv_work, cv_idle;
-  uint32_t first_iteration = 0, taken = 0;  // the k-th iteration handed out renders index first + k
-  uint32_t in_flight = 0;
-  WorkPlan plan;
-  bool quit = false;
-  int error = ETXB_OK;
-  std::string error_text;
-  std::chrono::steady_clock::time_point busy_since;
-  double busy_seconds = 0.0;   // wall time with at least one iteration queued or in flight
-  double last_iteration_seconds = 0.0;
-  DevBuf<float4> combined;
-  int device = 0;
-  ncclComm_t reduce_comm = nullptr;  // the frame reduce has its own communicator: the lanes' ones are busy with iterations in flight
-  cudaStream_t stream = nullptr;
-  DevBuf<float4> combined_light, reduced;
-};
-
-namespace {
-
-// NCCL is bound at run time: a single-GPU host needs no libnccl, and a torch host that already loaded its bundled libnccl.so.2 shares it.
-struct NcclApi {
-  void* handle = nullptr;
-  ncclResult_t (*GetUniqueId)(ncclUniqueId*) = nullptr;
-  ncclResult_t (*CommInitRank)(ncclComm_t*, int, ncclUniqueId, int) = nullptr;
-  ncclResult_t (*CommDestroy)(ncclComm_t) = nullptr;
-  ncclResult_t (*AllReduce)(const void*, void*, size_t, ncclDataType_t, ncclRedOp_t, ncclComm_t, cudaStream_t) = nullptr;
-  ncclResult_t (*AllGather)(const void*, void*, size_t, ncclDataType_t, ncclComm_t, cudaStream_t) = nullptr;
-  ncclResult_t (*Reduce)(const void*, void*, size_t, ncclDataType_t, ncclRedOp_t, int, ncclComm_t, cudaStream_t) = nullptr;
-  ncclResult_t (*Broadcast)(const void*, void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
-  ncclResult_t (*GroupStart)() = nullptr;
-  ncclResult_t (*GroupEnd)() = nullptr;
-  const char* (*GetErrorString)(ncclResult_t) = nullptr;
-};
 NcclApi* nccl_api() {
   static NcclApi api;
   static std::once_flag once;
@@ -206,13 +56,6 @@ NcclApi* nccl_api() {
   return api.handle ? &api : nullptr;
 }
 
-#define NCCL_OK(ctx, call)                                                                                                 \
-  do {                                                                                                                     \
-    ncclResult_t res__ = (call);                                                                                           \
-    if (res__ != ncclSuccess) return fail(ctx, ETXB_ERR_CUDA, "%s failed: %s (%s:%d)", #call, nccl_api()->GetErrorString(res__), __FILE__, __LINE__); \
-  } while (0)
-
-// Joins rank `rank` of a `world`-rank communicator on the current device; `id` holds the ncclUniqueId rank 0 made.  Collective.
 int comm_init_rank(etxb_ctx* ctx, ncclComm_t* comm, uint32_t world, uint32_t rank, const void* id) {
   NcclApi* n = nccl_api();
   if (!n) return fail(ctx, ETXB_ERR_NOT_READY, "libnccl.so.2 could not be loaded");
@@ -222,12 +65,15 @@ int comm_init_rank(etxb_ctx* ctx, ncclComm_t* comm, uint32_t world, uint32_t ran
   return ETXB_OK;
 }
 
-// A stream at the device's highest priority, so that its few blocks do not queue behind the lanes' large kernels
 cudaError_t create_priority_stream(cudaStream_t* stream) {
   int prio_low = 0, prio_high = 0;
   if (cudaError_t err = cudaDeviceGetStreamPriorityRange(&prio_low, &prio_high)) return err;
   return cudaStreamCreateWithPriority(stream, cudaStreamNonBlocking, prio_high);
 }
+
+}  // namespace etxb_internal
+
+namespace {
 
 cudaEvent_t next_event(etxb_ctx* ctx) {
   if (ctx->event_cursor == ctx->event_pool.size()) {
@@ -258,13 +104,6 @@ struct LaunchTimer {
     }
   }
 };
-
-bool material_class_supported_host(uint32_t cls) { return cls <= ETXB_MAT_VOID; }
-
-// A Distribution over `size` items holds size + 1 entries (DistributionBuilder allocates the closing {0, 0, 1} entry, distribution_builder.hxx:8-14,
-// 52) while `values.count` says `size` (the reference's loader) or size + 1 (hosts that count the closing entry): both are accepted, and the
-// device always gets the size + 1 entries.
-bool distribution_covers(uint64_t count, uint64_t size) { return (count == size) || (count == size + 1u); }
 
 uint32_t next_pow2(uint64_t v) {
   // next_power_of_two (math.hxx:1001-1010)
@@ -930,569 +769,6 @@ int run_pt_iteration(etxb_ctx* ctx) {
   return finish_iteration(ctx);
 }
 
-// ---- scene upload / update ------------------------------------------------------------------------------------------------------------------
-// etxb_upload_scene and etxb_update_scene run the same stages: validate_scene makes every check and touches nothing on the device,
-// prepare_scene hashes the bulk arrays (prepare_bvh uploads a new geometry and builds its BVH2 on the device), commit_scene commits to the device.  An
-// update keeps the device copies whose content hashes did not change; everything small is derived from the PODs again on every call.
-struct SceneClass {
-  bool stochastic = false;  // has_stochastic_merge
-  bool boundaries = false, subsurface = false, deferred = false, opaque = false, plain = false;
-};
-
-struct ScenePrep {
-  SceneClass cls;
-  SceneHashes hashes;
-  double fingerprint_seconds = 0.0, bvh_seconds = 0.0;
-  uint64_t bytes_hashed = 0;
-  // a new geometry's device copies and BVH2 (prepare_bvh: built once, copied into each context that commits it)
-  DevBuf<DVertex> vertices;
-  DevBuf<DTriangle> triangles;
-  DevBuf<BvhNode> bvh_nodes;
-  DevBuf<float4> bvh_tris;
-  uint32_t max_depth = 0;
-  bool have_bvh = false;
-  DevBuf<WideNode> wide;  // the 4-wide tree collapsed from the first committing context's BVH2
-  uint32_t max_stack = 0;
-  bool have_wide = false;
-};
-
-bool image_has_table(const etxb_image& im) {
-  return (im.y_distribution.values.a != nullptr) && distribution_covers(im.y_distribution.values.count, im.isize[1]) && (im.x_distributions.count == im.isize[1]);
-}
-size_t image_pixel_bytes(const etxb_image& im) { return size_t(im.isize[0]) * im.isize[1] * (im.format == 1u ? 16 : 4); }
-
-int check_scene_args(etxb_ctx* ctx, uint64_t scene_bytes, uint64_t camera_bytes) {
-  if (scene_bytes != sizeof(etxb_scene) || camera_bytes != sizeof(etxb_camera))
-    return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "scene/camera size mismatch: got %llu/%llu, expected %zu/%zu", (unsigned long long)scene_bytes,
-      (unsigned long long)camera_bytes, sizeof(etxb_scene), sizeof(etxb_camera));
-  if (!ctx->xyz_table.ptr) return fail(ctx, ETXB_ERR_NOT_READY, "etxb_upload_color_tables must be called before etxb_upload_scene");
-  return ETXB_OK;
-}
-
-// Every check of the upload but the BVH depth (prepare_bvh), and the scene-class flags.  What the device path does not cover yet fails
-// loudly (no CPU fallback); every index the host builder and the kernels follow is checked: a malformed scene is an error, not an
-// out-of-bounds read.
-int validate_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, SceneClass& c) {
-  if (cam.cls > 1u) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "unknown camera class %u", cam.cls);
-  if (cam.lens_image != ETXB_INVALID_INDEX) {
-    if (cam.lens_image >= s.images.count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "camera lens image index out of range");
-    const auto& lens = static_cast<const etxb_image*>(s.images.a)[cam.lens_image];
-    if (!distribution_covers(lens.y_distribution.values.count, lens.isize[1])) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "camera lens image has no sampling table");
-  }
-  const auto* mats = static_cast<const etxb_material*>(s.materials.a);
-  for (uint64_t i = 0; i < s.materials.count; ++i) {
-    const etxb_material& m = mats[i];
-    if (!material_class_supported_host(m.cls)) return fail(ctx, ETXB_ERR_UNSUPPORTED, "material %llu: class %u is not supported on the device yet", (unsigned long long)i, m.cls);
-    if (m.diffuse_variation > 2u) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "material %llu: unknown diffuse_variation %u", (unsigned long long)i, m.diffuse_variation);
-    if (m.subsurface.cls > 2u) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "material %llu: unknown subsurface class %u", (unsigned long long)i, m.subsurface.cls);
-    if (m.subsurface.cls != 0) {
-      if (s.subsurface_exit_material >= s.materials.count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "material %llu uses subsurface scattering but scene.subsurface_exit_material is not set", (unsigned long long)i);
-      if ((m.subsurface.image_index != ETXB_INVALID_INDEX) && (m.subsurface.image_index >= s.images.count))
-        return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "material %llu: subsurface image index out of range", (unsigned long long)i);
-    }
-    uint32_t imgs[] = {m.reflectance.image_index, m.scattering.image_index, m.emission.image_index, m.roughness.image_index, m.normal_image_index, m.thinfilm.thickness_image};
-    for (uint32_t im : imgs)
-      if ((im != ETXB_INVALID_INDEX) && (im >= s.images.count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "material %llu: image index %u out of range", (unsigned long long)i, im);
-    if (((m.int_medium != ETXB_INVALID_INDEX) && (m.int_medium >= s.mediums.count)) || ((m.ext_medium != ETXB_INVALID_INDEX) && (m.ext_medium >= s.mediums.count)))
-      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "material %llu: medium index out of range", (unsigned long long)i);
-  }
-  c = {};
-  for (uint64_t i = 0; i < s.materials.count; ++i) {
-    const etxb_material& m = mats[i];
-    bool lambert = (m.cls == ETXB_MAT_DIFFUSE) && (m.diffuse_variation == 0);
-    bool smooth = (std::max(m.roughness.value[0], m.roughness.value[1]) <= 1.0e-4f) && (m.roughness.image_index == ETXB_INVALID_INDEX);
-    bool always_delta = (((m.cls == ETXB_MAT_DIELECTRIC) || (m.cls == ETXB_MAT_CONDUCTOR)) && smooth) || (m.cls == ETXB_MAT_THINFILM) || (m.cls == ETXB_MAT_MIRROR) ||
-                        (m.cls == ETXB_MAT_VOID);
-    if (!lambert && !always_delta) c.stochastic = true;
-  }
-  const auto* emitters = static_cast<const etxb_emitter*>(s.emitter_instances.a);
-  for (uint64_t i = 0; i < s.emitter_instances.count; ++i) {
-    if (emitters[i].cls > 2u) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "emitter %llu: unknown class %u", (unsigned long long)i, emitters[i].cls);
-    if (emitters[i].cls == 1u) {
-      const auto& prof = static_cast<const etxb_emitter_profile*>(s.emitter_profiles.a)[emitters[i].profile];
-      if (prof.emission.image_index >= s.images.count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "environment emitter %llu has no image", (unsigned long long)i);
-      const auto& img = static_cast<const etxb_image*>(s.images.a)[prof.emission.image_index];
-      if (!distribution_covers(img.y_distribution.values.count, img.isize[1])) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "environment emitter %llu: image has no sampling table", (unsigned long long)i);
-    }
-  }
-  // media (medium.hxx:8-47)
-  const auto* meds = static_cast<const etxb_medium*>(s.mediums.a);
-  for (uint64_t i = 0; i < s.mediums.count; ++i) {
-    const etxb_medium& md = meds[i];
-    if (md.cls == 1u) {
-      size_t n = size_t(md.dimensions[0]) * md.dimensions[1] * md.dimensions[2];
-      if ((n == 0) || (md.density.count != n)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium %llu: density grid does not match its dimensions", (unsigned long long)i);
-    } else if (md.cls != 0u) {
-      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "medium %llu: unknown class %u", (unsigned long long)i, md.cls);
-    }
-  }
-  for (uint64_t i = 0; i < s.materials.count; ++i) {
-    if (mats[i].cls == ETXB_MAT_BOUNDARY) c.boundaries = true;
-    if (mats[i].subsurface.cls != 0) c.subsurface = true;
-  }
-  if ((cam.medium_index != ETXB_INVALID_INDEX) && (cam.medium_index >= s.mediums.count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "camera medium index out of range");
-  // deferred shadow rays (ShadowBatch, dvcm.cuh) need: no alpha test that can reject, no Boundary surfaces / media (transmittance is 0 or 1),
-  // no BSDF whose evaluation draws from the sampler, no subsurface exits
-  c.plain = !c.boundaries && !c.subsurface && (s.mediums.count == 0) && (cam.medium_index == ETXB_INVALID_INDEX);
-  bool no_alpha = true;
-  const auto* all_images = static_cast<const etxb_image*>(s.images.a);
-  for (uint64_t i = 0; no_alpha && (i < s.materials.count); ++i) {
-    if (mats[i].opacity != 1.0f) no_alpha = false;
-    uint32_t im = mats[i].scattering.image_index;
-    if ((im != ETXB_INVALID_INDEX) && (all_images[im].options & kImageHasAlpha)) no_alpha = false;
-  }
-  c.opaque = c.plain && no_alpha;
-  c.deferred = c.opaque && !c.stochastic;
-  // images: pixels + flattened row/column CDFs (image.hxx:8-50)
-  for (uint64_t i = 0; i < s.images.count; ++i) {
-    const etxb_image& im = all_images[i];
-    if ((im.format != 1u) && (im.format != 2u)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "image %llu: unknown pixel format %u", (unsigned long long)i, im.format);
-    if (size_t(im.isize[0]) * im.isize[1] == 0) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "image %llu is empty", (unsigned long long)i);
-    if (image_has_table(im)) {
-      const auto* rows = static_cast<const etxb_distribution*>(im.x_distributions.a);
-      for (uint32_t y = 0; y < im.isize[1]; ++y)
-        if (!distribution_covers(rows[y].values.count, im.isize[0])) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "image %llu: row %u distribution has %llu entries", (unsigned long long)i, y, (unsigned long long)rows[y].values.count);
-    }
-  }
-  if (s.emitter_instances.count == 0) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "scene has no emitters");
-  const auto* spectra = static_cast<const etxb_spectrum*>(s.spectrums.a);
-  for (uint64_t i = 0; i < s.spectrums.count; ++i) {
-    const etxb_spectrum& sp = spectra[i];
-    if (sp.entry_count != 441) return fail(ctx, ETXB_ERR_UNSUPPORTED, "spectrum %llu has %u entries; the loader's 441-entry 390..830 nm grid is required", (unsigned long long)i, sp.entry_count);
-    for (uint32_t k = 0; k < 441; ++k)
-      if (sp.entries[k].wavelength != float(390 + k)) return fail(ctx, ETXB_ERR_UNSUPPORTED, "spectrum %llu is not on the integer 390..830 nm grid", (unsigned long long)i);
-  }
-  // geometry
-  const auto* tris = static_cast<const etxb_triangle*>(s.triangles.a);
-  for (uint64_t i = 0; i < s.triangles.count; ++i) {
-    const etxb_triangle& t = tris[i];
-    if ((t.i[0] >= s.vertices.count) || (t.i[1] >= s.vertices.count) || (t.i[2] >= s.vertices.count))
-      return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "triangle %llu: vertex index out of range", (unsigned long long)i);
-    if (t.material_index >= s.materials.count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "triangle %llu: material index %u out of range", (unsigned long long)i, t.material_index);
-  }
-  if (s.triangle_to_emitter.count != s.triangles.count)
-    return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "triangle_to_emitter has %llu entries for %llu triangles", (unsigned long long)s.triangle_to_emitter.count, (unsigned long long)s.triangles.count);
-  const auto* t2e = static_cast<const uint32_t*>(s.triangle_to_emitter.a);
-  for (uint64_t i = 0; i < s.triangle_to_emitter.count; ++i)
-    if ((t2e[i] != ETXB_INVALID_INDEX) && (t2e[i] >= s.emitter_instances.count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "triangle %llu: emitter index out of range", (unsigned long long)i);
-  for (uint64_t i = 0; i < s.emitter_instances.count; ++i) {
-    if (emitters[i].profile >= s.emitter_profiles.count) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "emitter %llu: profile index out of range", (unsigned long long)i);
-    if ((emitters[i].cls == 0u) && (emitters[i].triangle_index >= s.triangles.count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "area emitter %llu: triangle index out of range", (unsigned long long)i);
-  }
-  if (!distribution_covers(s.emitters_distribution.values.count, s.emitter_instances.count))
-    return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "emitter distribution has %llu entries for %llu emitters", (unsigned long long)s.emitters_distribution.values.count, (unsigned long long)s.emitter_instances.count);
-  if ((s.pixel_sampler_image != 0xffffffffu) && (s.pixel_sampler_image >= s.images.count)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "pixel sampler image out of range");
-  if (size_t(cam.film_size[0]) * cam.film_size[1] == 0) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "empty film");
-  return ETXB_OK;
-}
-
-// validate_scene + the content hashes of the arrays commit_scene may keep on the device: the vertices and triangles (one geometry
-// hash), each image (pixels, sampling tables, scalar fields) and each density grid (values and dimensions)
-int prepare_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, ScenePrep& p) {
-  if (int rc = validate_scene(ctx, s, cam, p.cls)) return rc;
-  auto t0 = std::chrono::steady_clock::now();
-  SceneHashes& h = p.hashes;
-  auto hash = [&p](const void* data, size_t bytes, Hash128 seed) {
-    p.bytes_hashed += bytes;
-    return hash128(data, bytes, seed);
-  };
-  h.geometry = hash(s.vertices.a, s.vertices.count * sizeof(etxb_vertex), {});
-  h.geometry = hash(s.triangles.a, s.triangles.count * sizeof(etxb_triangle), h.geometry);
-  h.images.assign(s.images.count, {});
-  const auto* imgs = static_cast<const etxb_image*>(s.images.a);
-  for (uint64_t i = 0; i < s.images.count; ++i) {
-    const etxb_image& im = imgs[i];
-    const bool table = image_has_table(im);
-    const float fields[] = {im.fsize[0], im.fsize[1], im.offset[0], im.offset[1], im.scale[0], im.scale[1], im.normalization};
-    const uint32_t ifields[] = {im.isize[0], im.isize[1], im.options, im.format, table ? 1u : 0u};
-    Hash128 x = hash(fields, sizeof(fields), {});
-    x = hash(ifields, sizeof(ifields), x);
-    x = hash(im.pixels.a, image_pixel_bytes(im), x);
-    if (table) {
-      x = hash(im.y_distribution.values.a, (size_t(im.isize[1]) + 1u) * sizeof(etxb_distribution_entry), x);
-      const auto* rows = static_cast<const etxb_distribution*>(im.x_distributions.a);
-      for (uint32_t y = 0; y < im.isize[1]; ++y) x = hash(rows[y].values.a, (size_t(im.isize[0]) + 1u) * sizeof(etxb_distribution_entry), x);
-    }
-    h.images[i] = x;
-  }
-  h.grids.assign(s.mediums.count, {});
-  const auto* meds = static_cast<const etxb_medium*>(s.mediums.a);
-  for (uint64_t i = 0; i < s.mediums.count; ++i) {
-    if (meds[i].cls != 1u) continue;
-    h.grids[i] = hash(meds[i].dimensions, sizeof(meds[i].dimensions), {});
-    h.grids[i] = hash(meds[i].density.a, meds[i].density.count * sizeof(float), h.grids[i]);
-  }
-  h.valid = true;
-  p.fingerprint_seconds = seconds_since(t0);
-  return ETXB_OK;
-}
-
-// a device-to-device copy into `dst`, sized as `src`
-template <class T>
-int copy_device(etxb_ctx* ctx, DevBuf<T>& dst, const DevBuf<T>& src) {
-  CUDA_OK(ctx, dst.alloc(src.count));
-  if (src.count) CUDA_OK(ctx, cudaMemcpyAsync(dst.ptr, src.ptr, src.bytes(), cudaMemcpyDeviceToDevice, ctx->stream));
-  return ETXB_OK;
-}
-
-// A new geometry's vertices and triangles on the device, its BVH2 built there (bvh_build_device.cu: the tree of build_bvh), and the check of
-// its depth against the traversal stack.  Everything goes into the prep's own buffers: a refusal or a CUDA error leaves the committed scene as it was.
-int prepare_bvh(etxb_ctx* ctx, const etxb_scene& s, ScenePrep& p) {
-  if (p.have_bvh) return ETXB_OK;
-  auto t0 = std::chrono::steady_clock::now();
-  const auto* verts = static_cast<const etxb_vertex*>(s.vertices.a);
-  std::vector<DVertex> dverts(s.vertices.count);
-  for (uint64_t i = 0; i < s.vertices.count; ++i) {
-    const etxb_vertex& v = verts[i];
-    dverts[i].pos_u = make_float4(v.pos[0], v.pos[1], v.pos[2], v.tex[0]);
-    dverts[i].nrm_v = make_float4(v.nrm[0], v.nrm[1], v.nrm[2], v.tex[1]);
-    dverts[i].tan = make_float4(v.tan[0], v.tan[1], v.tan[2], 0.0f);
-    dverts[i].btn = make_float4(v.btn[0], v.btn[1], v.btn[2], 0.0f);
-  }
-  if (int rc = upload(ctx, p.vertices, dverts.data(), dverts.size())) return rc;
-  if (int rc = upload(ctx, p.triangles, reinterpret_cast<const DTriangle*>(s.triangles.a), size_t(s.triangles.count))) return rc;
-  const auto b0 = std::chrono::steady_clock::now();
-  DeviceBvhOut out;
-  CUDA_OK(ctx, build_bvh_device(reinterpret_cast<const float*>(p.vertices.ptr), sizeof(DVertex), reinterpret_cast<const uint32_t*>(p.triangles.ptr), sizeof(DTriangle),
-    uint32_t(s.triangles.count), false, ctx->stream, out));
-  adopt(p.bvh_nodes, out.nodes, out.node_count);
-  adopt(p.bvh_tris, reinterpret_cast<float4*>(out.tri_pos), size_t(out.slot_count) * 3u);
-  p.max_depth = out.max_depth;
-  ctx->bvh_build_seconds = seconds_since(b0);
-  ctx->kernel_ms[K_BVH_BUILD] += float(ctx->bvh_build_seconds * 1.0e3);
-  ctx->kernel_count[K_BVH_BUILD] += 1;
-  p.bvh_seconds += seconds_since(t0);
-  p.have_bvh = true;
-  if (p.max_depth >= uint32_t(kBvhStackSize)) return fail(ctx, ETXB_ERR_UNSUPPORTED, "BVH depth %u exceeds the traversal stack (%d)", p.max_depth, kBvhStackSize);
-  return ETXB_OK;
-}
-
-bool geometry_kept(const etxb_ctx* ctx, const ScenePrep& p, bool reuse) { return reuse && ctx->hashes.valid && (ctx->hashes.geometry == p.hashes.geometry); }
-
-// The device side of an upload (reuse = false: every buffer is allocated and copied again) or of an update (reuse = true: what the
-// hashes show unchanged stays, path-state buffers of the same size stay).  Runs after prepare_scene, so only CUDA errors remain: they
-// leave the scene not ready.  Ends with etxb_begin(ctx, 0).
-int commit_scene(etxb_ctx* ctx, const etxb_scene& s, const etxb_camera& cam, ScenePrep& p, bool reuse, etxb_update_info* info) {
-  const bool keep_geometry = geometry_kept(ctx, p, reuse);
-  if (!keep_geometry)
-    if (int rc = prepare_bvh(ctx, s, p)) return rc;
-  const SceneHashes old = std::move(ctx->hashes);
-  ctx->hashes = {};
-  ctx->scene_ready = false;
-  etxb_update_info st = {};
-  ctx->has_stochastic_merge = p.cls.stochastic;
-  ctx->plain_scene = p.cls.plain;
-  ctx->opaque_scene = p.cls.opaque;
-  DeviceScene& d = ctx->dscene;
-  const auto* mats = static_cast<const etxb_material*>(s.materials.a);
-
-  // ---- media: dense density grids go to HBM as they are ---------------------------------------------------------------------------------
-  {
-    const auto* meds = static_cast<const etxb_medium*>(s.mediums.a);
-    std::vector<DMedium> dmeds(s.mediums.count);
-    ctx->medium_density.resize(s.mediums.count);
-    for (uint64_t i = 0; i < s.mediums.count; ++i) {
-      const etxb_medium& md = meds[i];
-      DMedium& dm = dmeds[i];
-      dm = {};
-      dm.bounds_min = {md.bounds_min[0], md.bounds_min[1], md.bounds_min[2]};
-      dm.bounds_max = {md.bounds_max[0], md.bounds_max[1], md.bounds_max[2]};
-      dm.cls = md.cls;
-      dm.enable_explicit_connections = md.enable_explicit_connections;
-      dm.absorption_index = md.absorption_index;
-      dm.scattering_index = md.scattering_index;
-      dm.phase_function_g = md.phase_function_g;
-      dm.max_sigma = md.max_sigma;
-      dm.dim_x = md.dimensions[0];
-      dm.dim_y = md.dimensions[1];
-      dm.dim_z = md.dimensions[2];
-      DevBuf<float>& grid = ctx->medium_density[i];
-      if (md.cls == 1u) {
-        size_t n = size_t(dm.dim_x) * dm.dim_y * dm.dim_z;
-        if (reuse && old.valid && (i < old.grids.size()) && (old.grids[i] == p.hashes.grids[i]) && (grid.count == n)) {
-          st.grids_kept += 1;
-        } else {
-          CUDA_OK(ctx, grid.alloc(n));
-          CUDA_OK(ctx, cudaMemcpyAsync(grid.ptr, md.density.a, n * 4, cudaMemcpyHostToDevice, ctx->stream));
-          st.grids_uploaded += 1;
-        }
-        dm.density = grid.ptr;
-      } else {
-        grid.release();
-      }
-    }
-    if (int rc = upload(ctx, ctx->mediums, dmeds.data(), dmeds.size())) return rc;
-    d.mediums = ctx->mediums.ptr;
-    d.medium_count = uint32_t(dmeds.size());
-    d.has_boundaries = p.cls.boundaries ? 1 : 0;
-    d.has_subsurface = p.cls.subsurface ? 1 : 0;
-    d.subsurface_exit_material = s.subsurface_exit_material;
-    d.deferred_shadow_rays = p.cls.deferred ? 1u : 0u;
-  }
-  // ---- images: pixels + flattened row/column CDFs (image.hxx:8-50) ---------------------------------------------------------------
-  {
-    const auto* imgs = static_cast<const etxb_image*>(s.images.a);
-    std::vector<DImage> dimgs(s.images.count);
-    ctx->image_pixels.resize(s.images.count);
-    ctx->image_dists.resize(s.images.count * 2);
-    for (uint64_t i = 0; i < s.images.count; ++i) {
-      const etxb_image& im = imgs[i];
-      DImage& di = dimgs[i];
-      di = {};
-      const size_t bytes = image_pixel_bytes(im);
-      const bool table = image_has_table(im);
-      DevBuf<uint8_t>& pixels = ctx->image_pixels[i];
-      DevBuf<uint8_t>& x_dist = ctx->image_dists[i * 2];
-      DevBuf<uint8_t>& y_dist = ctx->image_dists[i * 2 + 1];
-      if (reuse && old.valid && (i < old.images.size()) && (old.images[i] == p.hashes.images[i]) && (pixels.count == bytes)) {
-        st.images_kept += 1;
-      } else {
-        CUDA_OK(ctx, pixels.alloc(bytes));
-        CUDA_OK(ctx, cudaMemcpyAsync(pixels.ptr, im.pixels.a, bytes, cudaMemcpyHostToDevice, ctx->stream));
-        x_dist.release();
-        y_dist.release();
-        if (table) {
-          size_t nx = size_t(im.isize[0]) + 1u, ny = size_t(im.isize[1]) + 1u;
-          std::vector<etxb_distribution_entry> flat(nx * im.isize[1]);
-          const auto* rows = static_cast<const etxb_distribution*>(im.x_distributions.a);
-          for (uint32_t y = 0; y < im.isize[1]; ++y) memcpy(flat.data() + size_t(y) * nx, rows[y].values.a, nx * sizeof(etxb_distribution_entry));
-          CUDA_OK(ctx, x_dist.alloc(flat.size() * sizeof(etxb_distribution_entry)));
-          CUDA_OK(ctx, cudaMemcpy(x_dist.ptr, flat.data(), flat.size() * sizeof(etxb_distribution_entry), cudaMemcpyHostToDevice));
-          CUDA_OK(ctx, y_dist.alloc(ny * sizeof(etxb_distribution_entry)));
-          CUDA_OK(ctx, cudaMemcpy(y_dist.ptr, im.y_distribution.values.a, ny * sizeof(etxb_distribution_entry), cudaMemcpyHostToDevice));
-        }
-        st.images_uploaded += 1;
-      }
-      di.pixels_f32 = (im.format == 1u) ? reinterpret_cast<const float4*>(pixels.ptr) : nullptr;
-      di.pixels_u8 = (im.format == 2u) ? reinterpret_cast<const uchar4*>(pixels.ptr) : nullptr;
-      di.fsize_x = im.fsize[0]; di.fsize_y = im.fsize[1];
-      di.offset_x = im.offset[0]; di.offset_y = im.offset[1];
-      di.scale_x = im.scale[0]; di.scale_y = im.scale[1];
-      di.isize_x = im.isize[0]; di.isize_y = im.isize[1];
-      di.normalization = im.normalization;
-      di.options = im.options;
-      di.format = im.format;
-      if (table) {
-        di.x_dist = reinterpret_cast<const etxb_distribution_entry*>(x_dist.ptr);
-        di.y_dist = reinterpret_cast<const etxb_distribution_entry*>(y_dist.ptr);
-        di.has_distribution = 1;
-      }
-    }
-    if (int rc = upload(ctx, ctx->images, dimgs.data(), dimgs.size())) return rc;
-    d.images = ctx->images.ptr;
-    d.image_count = uint32_t(dimgs.size());
-  }
-  const auto* spectra = static_cast<const etxb_spectrum*>(s.spectrums.a);
-  std::vector<DSpectrum> dspec(s.spectrums.count);
-  for (uint64_t i = 0; i < s.spectrums.count; ++i) {
-    for (uint32_t k = 0; k < 441; ++k) dspec[i].power[k] = spectra[i].entries[k].power;
-    memcpy(dspec[i].rgb, spectra[i].integrated, 12);
-  }
-
-  // ---- geometry ------------------------------------------------------------------------------------------------------
-  static_assert(sizeof(DTriangle) == sizeof(etxb_triangle), "triangle layout");
-  if (!keep_geometry) {
-    if (int rc = copy_device(ctx, ctx->vertices, p.vertices)) return rc;
-    if (int rc = copy_device(ctx, ctx->triangles, p.triangles)) return rc;
-  }
-  if (int rc = upload(ctx, ctx->tri_emitter, static_cast<const uint32_t*>(s.triangle_to_emitter.a), size_t(s.triangle_to_emitter.count))) return rc;
-  if (int rc = upload(ctx, ctx->materials, mats, size_t(s.materials.count))) return rc;
-  if (int rc = upload(ctx, ctx->profiles, static_cast<const etxb_emitter_profile*>(s.emitter_profiles.a), size_t(s.emitter_profiles.count))) return rc;
-  if (int rc = upload(ctx, ctx->emitters, static_cast<const etxb_emitter*>(s.emitter_instances.a), size_t(s.emitter_instances.count))) return rc;
-  if (int rc = upload(ctx, ctx->spectra, dspec.data(), dspec.size())) return rc;
-  if (int rc = upload(ctx, ctx->emitter_dist, static_cast<const etxb_distribution_entry*>(s.emitters_distribution.values.a), size_t(s.emitter_instances.count) + 1u))
-    return rc;
-  if (!keep_geometry) {
-    if (int rc = copy_device(ctx, ctx->bvh_nodes, p.bvh_nodes)) return rc;
-    if (int rc = copy_device(ctx, ctx->bvh_tris, p.bvh_tris)) return rc;
-    d.bvh_node_count = uint32_t(p.bvh_nodes.count);
-  }
-  d.vertices = ctx->vertices.ptr;
-  d.triangles = ctx->triangles.ptr;
-  d.tri_emitter = ctx->tri_emitter.ptr;
-  d.materials = ctx->materials.ptr;
-  d.emitter_profiles = ctx->profiles.ptr;
-  d.emitters = ctx->emitters.ptr;
-  d.spectra = ctx->spectra.ptr;
-  d.emitter_dist = ctx->emitter_dist.ptr;
-  d.bvh_nodes = ctx->bvh_nodes.ptr;
-  d.bvh_tris = ctx->bvh_tris.ptr;
-  bool keep_wide = false;
-#if !(defined(ETXB_PARITY) && ETXB_PARITY)
-  // a geometry whose 4-wide tree the traversal stack cannot hold keeps that verdict with it: an update that keeps the geometry does not
-  // collapse the tree again only to reject it
-  if (!keep_geometry) ctx->wide_rejected = false;
-  keep_wide = keep_geometry && ctx->has_stochastic_merge && ((d.wide_nodes != nullptr) || ctx->wide_rejected);
-#endif
-  if (!keep_wide) {
-    d.wide_nodes = nullptr;
-    d.wide_node_count = 0;
-    if (reuse) ctx->wide_nodes.release();
-  }
-#if !(defined(ETXB_PARITY) && ETXB_PARITY)
-  if (ctx->has_stochastic_merge && !keep_wide) {
-    // the sampler streams of such a scene's stochastic stages are the product build's own already: its traversal kernels may meet candidates in
-    // another order, so they walk the 4-wide quantised form of the tree (dwide.cuh); Lambert / delta scenes keep the oracle's candidate order
-    if (!p.have_wide) {
-      // collapsed on the device from the committed BVH2 (new or kept: bvh_build_device.cu, the tree of build_wide_bvh)
-      auto t0 = std::chrono::steady_clock::now();
-      WideNode* wide = nullptr;
-      uint32_t count = 0;
-      CUDA_OK(ctx, build_wide_bvh_device(ctx->bvh_nodes.ptr, d.bvh_node_count, ctx->stream, &wide, &count, &p.max_stack));
-      adopt(p.wide, wide, count);
-      p.have_wide = true;
-      const double seconds = seconds_since(t0);
-      ctx->kernel_ms[K_BVH_WIDE] += float(seconds * 1.0e3);
-      ctx->kernel_count[K_BVH_WIDE] += 1;
-      p.bvh_seconds += seconds;
-    }
-    if (p.max_stack < uint32_t(kWideStackSize)) {
-      if (int rc = copy_device(ctx, ctx->wide_nodes, p.wide)) return rc;
-      d.wide_nodes = ctx->wide_nodes.ptr;
-      d.wide_node_count = uint32_t(p.wide.count);
-    } else {
-      ctx->wide_rejected = true;
-    }
-  }
-#endif
-  d.emitter_count = uint32_t(s.emitter_instances.count);
-  d.triangle_count = uint32_t(s.triangles.count);
-  d.emitter_total_weight = s.emitters_distribution.total_weight;
-  memcpy(d.env_emitters, s.environment_emitters, sizeof(d.env_emitters));
-  d.env_emitter_count = s.environment_emitter_count;
-  d.bounding_sphere_center = {s.bounding_sphere_center[0], s.bounding_sphere_center[1], s.bounding_sphere_center[2]};
-  d.bounding_sphere_radius = s.bounding_sphere_radius;
-  d.min_path_length = s.min_path_length;
-  d.max_path_length = s.max_path_length;
-  d.samples = s.samples;
-  d.random_path_termination = s.random_path_termination;
-  d.spectral = (s.flags & ETXB_SCENE_SPECTRAL) ? 1u : 0u;
-  d.spectrum_count = uint32_t(s.spectrums.count);
-  d.default_dielectric_eta = s.default_dielectric_eta;
-  d.default_conductor_eta = s.default_conductor_eta;
-  d.default_conductor_k = s.default_conductor_k;
-  d.camera = cam;
-  ctx->spectral = d.spectral != 0;
-  ctx->pixel_sampler_image = s.pixel_sampler_image;
-  ctx->pixel_sampler_radius = s.pixel_sampler_radius;
-  ctx->noise_threshold = s.noise_threshold;
-  ctx->radiance_clamp = s.radiance_clamp;
-  ctx->scene_samples = s.samples;
-
-  // ---- film + queues (Film::allocate, film.cxx) ----------------------------------------------------------------------
-  // an update keeps every buffer whose size is what the upload would allocate (DevBuf::ensure)
-  uint32_t allocations = 0;
-  auto sized = [&](auto& b, size_t count) -> cudaError_t {
-    if (reuse) return b.ensure(count, allocations);
-    allocations += 1;
-    return b.alloc(count);
-  };
-  if ((ctx->width != cam.film_size[0]) || (ctx->height != cam.film_size[1])) {  // Denoised starts over at a new film size; the reference no longer fits
-    ctx->film_denoised.release();
-    ctx->reference.release();
-  }
-  ctx->width = cam.film_size[0];
-  ctx->height = cam.film_size[1];
-  ctx->path_count = ctx->width * ctx->height;
-  size_t n = ctx->path_count;
-  if (!reuse) {
-    ctx->film_normals.release();  // sized by the film: re-allocated by the next path-tracer run
-  } else if (ctx->film_normals.ptr && (ctx->film_normals.count != n)) {
-    if (int rc = pt_ensure_film(ctx)) return rc;  // the path tracer's layers and per-pixel history at the new film size
-    allocations += 1;
-  }
-  DevBuf<float4>* per_path_f4[] = {&ctx->ray_o, &ctx->ray_d, &ctx->thr, &ctx->mis, &ctx->hit, &ctx->gathered, &ctx->merged, &ctx->camera_value, &ctx->film_camera,
-    &ctx->film_light, &ctx->film_light_iteration, &ctx->film_out, &ctx->bs_weight_pdf, &ctx->bs_wo_eta};
-  for (auto* b : per_path_f4) CUDA_OK(ctx, sized(*b, n));
-  CUDA_OK(ctx, sized(ctx->bs_props, n));
-  CUDA_OK(ctx, sized(ctx->misc, n));
-  CUDA_OK(ctx, sized(ctx->wavelength, n));
-  DevBuf<uint32_t>* per_path_u32[] = {&ctx->lv_count, &ctx->lp_offset, &ctx->queue_a, &ctx->queue_b, &ctx->sampler_end_light, &ctx->sampler_end_camera, &ctx->merge_key};
-  for (auto* b : per_path_u32) CUDA_OK(ctx, sized(*b, n));
-  CUDA_OK(ctx, sized(ctx->conn_count, 1));
-  CUDA_OK(ctx, sized(ctx->queue_counts, 4));
-  CUDA_OK(ctx, sized(ctx->lv_tmp_count, 1));
-  CUDA_OK(ctx, sized(ctx->overflow, 1));
-  CUDA_OK(ctx, sized(ctx->grid_bbox, 8));
-  CUDA_OK(ctx, sized(ctx->counters, 1));
-  uint64_t cap = ctx->max_light_vertices_cfg ? ctx->max_light_vertices_cfg : uint64_t(n) * 16ull;
-  cap = std::min<uint64_t>(cap, 0x7fffffffull);
-  ctx->lv_capacity = uint32_t(cap);
-  CUDA_OK(ctx, sized(ctx->lv_tmp, cap));
-  CUDA_OK(ctx, sized(ctx->lv_final, cap));
-  CUDA_OK(ctx, sized(ctx->conn_list, cap));
-  if (ctx->has_stochastic_merge) {
-    CUDA_OK(ctx, sized(ctx->conn_list_sorted, cap));
-    CUDA_OK(ctx, sized(ctx->queue_sorted, n));
-    CUDA_OK(ctx, sized(ctx->queue_keys, n));
-    CUDA_OK(ctx, sized(ctx->queue_keys_sorted, n));
-  } else {
-    ctx->conn_list_sorted.release();
-    ctx->queue_sorted.release();
-    ctx->queue_keys.release();
-    ctx->queue_keys_sorted.release();
-  }
-#if defined(ETXB_PARITY) && ETXB_PARITY
-  ctx->conn_rec.release();
-#else
-  // the connection stage's per-path camera vertex records (make_params: connect_stage = has_stochastic_merge)
-  if (ctx->has_stochastic_merge) {
-    CUDA_OK(ctx, sized(ctx->conn_rec, n * (ctx->spectral ? kConnRecRows<true> : kConnRecRows<false>)));
-  } else {
-    ctx->conn_rec.release();
-  }
-#endif
-  CUDA_OK(ctx, sized(ctx->trace_cursor, 1));
-  const bool atomic_candidate = ctx->opaque_scene && ctx->plain_scene && ctx->has_stochastic_merge;
-  if (ctx->dscene.deferred_shadow_rays || atomic_candidate) {
-    // atomic mode: a camera bounce queues its vertex connections (<= cap, the pair list's capacity) plus one emitter segment per path
-    const uint64_t shadow_cap = std::min<uint64_t>(cap + (atomic_candidate ? n : 0), 0x7fffffffull);
-    CUDA_OK(ctx, sized(ctx->shadow_span, n));
-    CUDA_OK(ctx, sized(ctx->shadow_p0, shadow_cap));
-    CUDA_OK(ctx, sized(ctx->shadow_p1, shadow_cap));
-    CUDA_OK(ctx, sized(ctx->shadow_value, shadow_cap));
-    CUDA_OK(ctx, sized(ctx->shadow_result, shadow_cap));
-    CUDA_OK(ctx, sized(ctx->shadow_count, 2));
-  } else {
-    ctx->shadow_span.release();
-    ctx->shadow_p0.release();
-    ctx->shadow_p1.release();
-    ctx->shadow_value.release();
-    ctx->shadow_result.release();
-  }
-  // the sort buffers also hold the gather queue and the path queues (up to one entry per path), whatever the configured pool capacity
-  const uint64_t sort_cap = std::max<uint64_t>(cap, n);
-  DevBuf<uint32_t>* per_vertex_u32[] = {&ctx->keys_in, &ctx->keys_out, &ctx->vals_in, &ctx->vals_out};
-  for (auto* b : per_vertex_u32) CUDA_OK(ctx, sized(*b, sort_cap));
-  DevBuf<float4>* per_vertex_f4[] = {&ctx->g_pos, &ctx->g_nrm, &ctx->g_win, &ctx->g_thr};
-  for (auto* b : per_vertex_f4) CUDA_OK(ctx, sized(*b, cap));
-  CUDA_OK(ctx, sized(ctx->cell_range, next_pow2(cap)));
-  // one scratch buffer for every CUB call of an iteration: the 32-bit pair sorts (photon grid, gather queue, path queues), the pair-list
-  // sort with its 64-bit (path, light vertex) values, and the scan over the per-path vertex counts
-  size_t temp_sort = 0, temp_sort64 = 0, temp_scan = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, temp_sort, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, int(sort_cap));
-  cub::DeviceRadixSort::SortPairs(nullptr, temp_sort64, (uint32_t*)nullptr, (uint32_t*)nullptr, (unsigned long long*)nullptr, (unsigned long long*)nullptr, int(sort_cap), 0, 16);
-  cub::DeviceScan::ExclusiveSum(nullptr, temp_scan, (uint32_t*)nullptr, (uint32_t*)nullptr, int(n));
-  CUDA_OK(ctx, sized(ctx->cub_temp, std::max(std::max(temp_sort, temp_sort64), temp_scan) + 256));
-  CUDA_OK(ctx, cudaMemsetAsync(ctx->overflow.ptr, 0, 4, ctx->stream));
-  CUDA_OK(ctx, cudaMemsetAsync(ctx->counters.ptr, 0, sizeof(DeviceCounters), ctx->stream));
-  CUDA_OK(ctx, cudaMemsetAsync(ctx->sampler_end_light.ptr, 0, n * 4, ctx->stream));
-  CUDA_OK(ctx, cudaMemsetAsync(ctx->sampler_end_camera.ptr, 0, n * 4, ctx->stream));
-  CUDA_OK(ctx, cudaMemsetAsync(ctx->lv_count.ptr, 0, n * 4, ctx->stream));
-  CUDA_OK(ctx, cudaMemsetAsync(ctx->lp_offset.ptr, 0, n * 4, ctx->stream));
-  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-  ctx->hashes = p.hashes;
-  ctx->scene_ready = true;
-  if (info) {
-    st.kept = (keep_geometry ? ETXB_KEPT_GEOMETRY : 0u) | ((keep_wide && (d.wide_nodes != nullptr)) ? ETXB_KEPT_WIDE_TREE : 0u) | (allocations == 0 ? ETXB_KEPT_PATH_STATE : 0u);
-    st.fingerprint_seconds = p.fingerprint_seconds;
-    st.bytes_hashed = p.bytes_hashed;
-    st.bvh_seconds = p.bvh_seconds;
-    *info = st;
-  }
-  return etxb_begin(ctx, 0);
-}
-
 // The three passes of a VCM iteration, each instantiated for the context's scene class.  The light pass starts the iteration's clock,
 // the camera pass stops it (finish_iteration).
 int light_pass(etxb_ctx* ctx) {
@@ -1514,7 +790,104 @@ int camera_pass(etxb_ctx* ctx) {
   return finish_iteration(ctx);
 }
 
-// one whole iteration on the calling thread; returns when it has finished (the bounce loops read queue sizes back)
+// Buffers that only some scene classes use, each with the count the scene asks for: sized by `size(buffer, count)` when `needed`, released
+// otherwise.  Stops at the first error.
+template <class Size, class... T>
+cudaError_t size_if_needed(bool needed, Size&& size, std::pair<DevBuf<T>*, size_t>... bufs) {
+  cudaError_t err = cudaSuccess;
+  if (needed) {
+    ((err = (err == cudaSuccess) ? size(*bufs.first, bufs.second) : err), ...);
+  } else {
+    (bufs.first->release(), ...);
+  }
+  return err;
+}
+
+}  // namespace
+
+namespace etxb_internal __attribute__((visibility("hidden"))) {
+
+// Film + queues (Film::allocate, film.cxx).  An update keeps every buffer whose size is what the upload would allocate (DevBuf::ensure).
+int commit_path_state(etxb_ctx* ctx, const etxb_camera& cam, bool reuse, uint32_t* allocations) {
+  auto sized = [&](auto& b, size_t count) -> cudaError_t {
+    if (reuse) return b.ensure(count, *allocations);
+    *allocations += 1;
+    return b.alloc(count);
+  };
+  if ((ctx->width != cam.film_size[0]) || (ctx->height != cam.film_size[1])) {  // Denoised starts over at a new film size; the reference no longer fits
+    ctx->film_denoised.release();
+    ctx->reference.release();
+  }
+  ctx->width = cam.film_size[0];
+  ctx->height = cam.film_size[1];
+  ctx->path_count = ctx->width * ctx->height;
+  size_t n = ctx->path_count;
+  if (!reuse) {
+    ctx->film_normals.release();  // sized by the film: re-allocated by the next path-tracer run
+  } else if (ctx->film_normals.ptr && (ctx->film_normals.count != n)) {
+    if (int rc = pt_ensure_film(ctx)) return rc;  // the path tracer's layers and per-pixel history at the new film size
+    *allocations += 1;
+  }
+  DevBuf<float4>* per_path_f4[] = {&ctx->ray_o, &ctx->ray_d, &ctx->thr, &ctx->mis, &ctx->hit, &ctx->gathered, &ctx->merged, &ctx->camera_value, &ctx->film_camera,
+    &ctx->film_light, &ctx->film_light_iteration, &ctx->film_out, &ctx->bs_weight_pdf, &ctx->bs_wo_eta};
+  for (auto* b : per_path_f4) CUDA_OK(ctx, sized(*b, n));
+  CUDA_OK(ctx, sized(ctx->bs_props, n));
+  CUDA_OK(ctx, sized(ctx->misc, n));
+  CUDA_OK(ctx, sized(ctx->wavelength, n));
+  DevBuf<uint32_t>* per_path_u32[] = {&ctx->lv_count, &ctx->lp_offset, &ctx->queue_a, &ctx->queue_b, &ctx->sampler_end_light, &ctx->sampler_end_camera, &ctx->merge_key};
+  for (auto* b : per_path_u32) CUDA_OK(ctx, sized(*b, n));
+  CUDA_OK(ctx, sized(ctx->conn_count, 1));
+  CUDA_OK(ctx, sized(ctx->queue_counts, 4));
+  CUDA_OK(ctx, sized(ctx->lv_tmp_count, 1));
+  CUDA_OK(ctx, sized(ctx->overflow, 1));
+  CUDA_OK(ctx, sized(ctx->grid_bbox, 8));
+  CUDA_OK(ctx, sized(ctx->counters, 1));
+  uint64_t cap = ctx->max_light_vertices_cfg ? ctx->max_light_vertices_cfg : uint64_t(n) * 16ull;
+  cap = std::min<uint64_t>(cap, 0x7fffffffull);
+  ctx->lv_capacity = uint32_t(cap);
+  CUDA_OK(ctx, sized(ctx->lv_tmp, cap));
+  CUDA_OK(ctx, sized(ctx->lv_final, cap));
+  CUDA_OK(ctx, sized(ctx->conn_list, cap));
+  // the material sorts of path queues and connection lists (scenes with stochastic BSDFs)
+  CUDA_OK(ctx, size_if_needed(ctx->has_stochastic_merge, sized, std::pair{&ctx->conn_list_sorted, cap}, std::pair{&ctx->queue_sorted, n}, std::pair{&ctx->queue_keys, n},
+                              std::pair{&ctx->queue_keys_sorted, n}));
+#if defined(ETXB_PARITY) && ETXB_PARITY
+  ctx->conn_rec.release();
+#else
+  // the connection stage's per-path camera vertex records (make_params: connect_stage = has_stochastic_merge)
+  CUDA_OK(ctx, size_if_needed(ctx->has_stochastic_merge, sized, std::pair{&ctx->conn_rec, n * (ctx->spectral ? kConnRecRows<true> : kConnRecRows<false>)}));
+#endif
+  CUDA_OK(ctx, sized(ctx->trace_cursor, 1));
+  // the shadow segments of deferred shadow rays and of the atomic mode: a camera bounce queues its vertex connections (<= cap, the pair list's
+  // capacity) plus, in atomic mode, one emitter segment per path
+  const bool atomic_candidate = ctx->opaque_scene && ctx->plain_scene && ctx->has_stochastic_merge;
+  const uint64_t shadow_cap = std::min<uint64_t>(cap + (atomic_candidate ? n : 0), 0x7fffffffull);
+  CUDA_OK(ctx, size_if_needed(ctx->dscene.deferred_shadow_rays || atomic_candidate, sized, std::pair{&ctx->shadow_span, n}, std::pair{&ctx->shadow_p0, shadow_cap},
+                              std::pair{&ctx->shadow_p1, shadow_cap}, std::pair{&ctx->shadow_value, shadow_cap}, std::pair{&ctx->shadow_result, shadow_cap},
+                              std::pair{&ctx->shadow_count, size_t(2)}));
+  // the sort buffers also hold the gather queue and the path queues (up to one entry per path), whatever the configured pool capacity
+  const uint64_t sort_cap = std::max<uint64_t>(cap, n);
+  DevBuf<uint32_t>* per_vertex_u32[] = {&ctx->keys_in, &ctx->keys_out, &ctx->vals_in, &ctx->vals_out};
+  for (auto* b : per_vertex_u32) CUDA_OK(ctx, sized(*b, sort_cap));
+  DevBuf<float4>* per_vertex_f4[] = {&ctx->g_pos, &ctx->g_nrm, &ctx->g_win, &ctx->g_thr};
+  for (auto* b : per_vertex_f4) CUDA_OK(ctx, sized(*b, cap));
+  CUDA_OK(ctx, sized(ctx->cell_range, next_pow2(cap)));
+  // one scratch buffer for every CUB call of an iteration: the 32-bit pair sorts (photon grid, gather queue, path queues), the pair-list
+  // sort with its 64-bit (path, light vertex) values, and the scan over the per-path vertex counts
+  size_t temp_sort = 0, temp_sort64 = 0, temp_scan = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, temp_sort, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, int(sort_cap));
+  cub::DeviceRadixSort::SortPairs(nullptr, temp_sort64, (uint32_t*)nullptr, (uint32_t*)nullptr, (unsigned long long*)nullptr, (unsigned long long*)nullptr, int(sort_cap), 0, 16);
+  cub::DeviceScan::ExclusiveSum(nullptr, temp_scan, (uint32_t*)nullptr, (uint32_t*)nullptr, int(n));
+  CUDA_OK(ctx, sized(ctx->cub_temp, std::max(std::max(temp_sort, temp_sort64), temp_scan) + 256));
+  CUDA_OK(ctx, cudaMemsetAsync(ctx->overflow.ptr, 0, 4, ctx->stream));
+  CUDA_OK(ctx, cudaMemsetAsync(ctx->counters.ptr, 0, sizeof(DeviceCounters), ctx->stream));
+  CUDA_OK(ctx, cudaMemsetAsync(ctx->sampler_end_light.ptr, 0, n * 4, ctx->stream));
+  CUDA_OK(ctx, cudaMemsetAsync(ctx->sampler_end_camera.ptr, 0, n * 4, ctx->stream));
+  CUDA_OK(ctx, cudaMemsetAsync(ctx->lv_count.ptr, 0, n * 4, ctx->stream));
+  CUDA_OK(ctx, cudaMemsetAsync(ctx->lp_offset.ptr, 0, n * 4, ctx->stream));
+  return ETXB_OK;
+}
+
 int run_iteration_blocking(etxb_ctx* ctx) {
   if (ctx->integrator == ETXB_INTEGRATOR_PT) {
     cudaSetDevice(ctx->device);
@@ -1530,6 +903,32 @@ int run_iteration_blocking(etxb_ctx* ctx) {
   if (int rc = grid_build(ctx, records, count)) return rc;
   return camera_pass(ctx);
 }
+
+int ctx_drain(etxb_ctx* ctx) {
+  std::unique_lock<std::mutex> lock(ctx->worker_m);
+  ctx->worker_idle.wait(lock, [&] { return (ctx->worker_queued == 0) && !ctx->worker_busy; });
+  int rc = ctx->worker_error;
+  ctx->worker_error = ETXB_OK;
+  return rc;
+}
+
+const float4* film_layer_finish(uint32_t layer, float4* raw, float4* light, uint32_t width, uint32_t height, float4* out, cudaStream_t stream) {
+  const uint32_t n = width * height;
+  if (layer == ETXB_FILM_RESULT) {
+    FilmBuffers film = {raw, light, nullptr, width, height};
+    k_film_resolve<<<blocks_for(n, 256), 256, 0, stream>>>(film, out);
+    return out;
+  }
+  if (layer == ETXB_FILM_NORMALS) {  // the VCM integrator leaves them empty; shown as n * 0.5 + 0.5
+    k_film_layer_normals<<<blocks_for(n, 256), 256, 0, stream>>>(raw, out, n);
+    return out;
+  }
+  return raw;
+}
+
+}  // namespace etxb_internal
+
+namespace {
 
 void ctx_worker(etxb_ctx* ctx) {
   std::unique_lock<std::mutex> lock(ctx->worker_m);
@@ -1550,64 +949,54 @@ void ctx_worker(etxb_ctx* ctx) {
   }
 }
 
-// blocks until every queued iteration has finished; returns (and clears) the first error one of them hit
-int ctx_drain(etxb_ctx* ctx) {
-  std::unique_lock<std::mutex> lock(ctx->worker_m);
-  ctx->worker_idle.wait(lock, [&] { return (ctx->worker_queued == 0) && !ctx->worker_busy; });
-  int rc = ctx->worker_error;
-  ctx->worker_error = ETXB_OK;
-  return rc;
-}
-
-// Film::layer (film.cxx:381-418): the device buffer that holds `layer` as float4 (computed into film_out where the layer is derived)
-int film_layer_source(etxb_ctx* ctx, uint32_t layer, const float4** out_src) {
-  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
-  cudaSetDevice(ctx->device);
-  const float4* src = nullptr;
+// Film::layer (film.cxx:381-418), step 1: the context's per-pixel buffer that `layer` is made from (the camera image for Result)
+int film_layer_raw(etxb_ctx* ctx, uint32_t layer, float4** out) {
   switch (layer) {
-    case ETXB_FILM_RESULT: {
-      FilmBuffers film = {ctx->film_camera.ptr, ctx->film_light.ptr, ctx->film_light_iteration.ptr, ctx->width, ctx->height};
-      k_film_resolve<<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(film, ctx->film_out.ptr);
-      ctx->kernel_launches += 1;
-      src = ctx->film_out.ptr;
-      break;
-    }
+    case ETXB_FILM_RESULT:
     case ETXB_FILM_CAMERA:
-      src = ctx->film_camera.ptr;
-      break;
+      *out = ctx->film_camera.ptr;
+      return ETXB_OK;
     case ETXB_FILM_LIGHT:
-      src = ctx->film_light.ptr;
-      break;
+      *out = ctx->film_light.ptr;
+      return ETXB_OK;
     case ETXB_FILM_LIGHT_ITERATION:
-      src = ctx->film_light_iteration.ptr;
-      break;
+      *out = ctx->film_light_iteration.ptr;
+      return ETXB_OK;
     case ETXB_FILM_CAMERA_ADAPTIVE:
       if (int rc = film_ensure_adaptive(ctx)) return rc;
-      src = ctx->film_adaptive.ptr;
-      break;
+      *out = ctx->film_adaptive.ptr;
+      return ETXB_OK;
     case ETXB_FILM_DENOISED:
       if (ctx->film_denoised.count != ctx->path_count) {
         CUDA_OK(ctx, ctx->film_denoised.alloc(ctx->path_count));
         CUDA_OK(ctx, cudaMemsetAsync(ctx->film_denoised.ptr, 0, ctx->film_denoised.bytes(), ctx->stream));
       }
-      src = ctx->film_denoised.ptr;
-      break;
+      *out = ctx->film_denoised.ptr;
+      return ETXB_OK;
     case ETXB_FILM_NORMALS:
-    case ETXB_FILM_ALBEDO: {
+    case ETXB_FILM_ALBEDO:
       if (int rc = pt_ensure_film(ctx)) return rc;
-      if (layer == ETXB_FILM_NORMALS) {
-        k_film_layer_normals<<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(ctx->film_normals.ptr, ctx->film_out.ptr, ctx->path_count);
-        ctx->kernel_launches += 1;
-        src = ctx->film_out.ptr;
-      } else {
-        src = ctx->film_albedo.ptr;
-      }
-      break;
-    }
+      *out = (layer == ETXB_FILM_NORMALS) ? ctx->film_normals.ptr : ctx->film_albedo.ptr;
+      return ETXB_OK;
     default:
       return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "unknown film layer %u", layer);
   }
-  *out_src = src;
+}
+
+// step 2 on the context's stream, into its film_out, with the context's light image: `raw` is step 1's buffer or its sum over the ranks
+const float4* film_layer_read_out(etxb_ctx* ctx, uint32_t layer, float4* raw) {
+  const float4* src = film_layer_finish(layer, raw, ctx->film_light.ptr, ctx->width, ctx->height, ctx->film_out.ptr, ctx->stream);
+  if (src != raw) ctx->kernel_launches += 1;
+  return src;
+}
+
+// the device buffer that holds `layer` as float4 (computed into film_out where the layer is derived)
+int film_layer_source(etxb_ctx* ctx, uint32_t layer, const float4** out_src) {
+  if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
+  cudaSetDevice(ctx->device);
+  float4* raw = nullptr;
+  if (int rc = film_layer_raw(ctx, layer, &raw)) return rc;
+  *out_src = film_layer_read_out(ctx, layer, raw);
   return ETXB_OK;
 }
 
@@ -1745,141 +1134,6 @@ int debug_merge(etxb_ctx* ctx, uint32_t record_count, const etxb_merge_query* d_
   return launch_merge<SP>(ctx, p, ctx->queue_a.ptr, ctx->queue_counts.ptr, count);
 }
 
-// What one rank takes of `iterations` more iterations of a replica-mode job (ordinals base .. base + iterations - 1).  Whole frames are dealt
-// round-robin (ordinal j on rank j % world).  What is left when the count is not a multiple of the ranks would leave some ranks a whole iteration
-// behind the others (20 iterations on 8 ranks: 3, 3, 3, 3, 2, 2, 2, 2): with a split lane those R iterations are split instead, each over
-// P = world / R ranks by camera tile — every part traces the whole light pass itself (same photon map, no exchange) and the camera pass of its
-// tiles; the parts meet in the frame reduce.  A split lane's film is made of ONE (part, parts) geometry: a later round that would need another
-// parts count is dealt as whole frames (with the count fixed, a rank's part is always rank % parts).  Returns the parts of this round's split
-// (0: none).
-uint32_t replica_plan(uint32_t world, uint32_t rank, uint32_t base, uint32_t iterations, bool split_lane, uint32_t have_parts, std::vector<WorkItem>& out) {
-  uint32_t whole = iterations, rest = 0, parts = 1;
-  if ((iterations >= world) && split_lane) {
-    rest = iterations % world;
-    parts = rest ? (world / rest) : 1u;
-    if ((parts >= 2u) && ((have_parts == 0u) || (have_parts == parts))) {
-      whole = iterations - rest;
-    } else {
-      rest = 0;
-    }
-  }
-  for (uint32_t j = base; j < base + whole; ++j)
-    if ((j % world) == rank) out.push_back({j, 0u, 1u});
-  for (uint32_t r = 0; r < rest; ++r) {
-    if ((rank / parts) == r) out.push_back({base + whole + r, rank % parts, parts});
-  }
-  return rest ? parts : 0u;
-}
-
-// The planner: deals the ordinals enqueued .. enqueued + iterations - 1 into the queues and routes every lane to its queue (see WorkPlan).
-void plan_enqueue(WorkPlan& p, uint32_t iterations) {
-  const uint32_t lanes = uint32_t(p.queues.size());
-  const bool tiles = p.mode == GroupMode::tiles;
-  for (uint32_t l = 0; l < lanes; ++l) p.lane_queue[l] = (tiles || (l == p.split_lane)) ? l : 0u;
-  if (p.mode == GroupMode::replicas) {
-    std::vector<WorkItem> items;
-    uint32_t parts_used = replica_plan(p.world, p.rank, p.enqueued, iterations, p.split_lane != 0xffffffffu, p.split_parts, items);
-    for (const WorkItem& it : items) {
-      if (it.parts > 1u) p.split_part = it.part;
-      p.queues[(it.parts > 1u) ? p.split_lane : 0u].push_back(it);
-    }
-    if (parts_used) p.split_parts = parts_used;  // every rank records the split geometry, also those that got no part of this round
-  } else {
-    for (uint32_t k = p.enqueued; k < p.enqueued + iterations; ++k) p.queues[tiles ? (k % lanes) : 0u].push_back({k, 0u, 1u});
-  }
-  p.enqueued += iterations;
-}
-void plan_clear(WorkPlan& p) {
-  for (auto& q : p.queues) q.clear();
-  p.enqueued = 0;
-}
-
-bool group_has_work(const etxb_group* grp, uint32_t lane) { return !grp->plan.queues[grp->plan.lane_queue[lane]].empty(); }
-bool group_idle(const etxb_group* grp) {
-  if (grp->in_flight > 0) return false;
-  for (const auto& q : grp->plan.queues)
-    if (!q.empty()) return false;
-  return true;
-}
-
-void group_worker(etxb_group* grp, uint32_t lane) {
-  cudaSetDevice(grp->device);
-  etxb_ctx* ctx = grp->lanes[lane];
-  std::unique_lock<std::mutex> lock(grp->m);
-  for (;;) {
-    grp->cv_work.wait(lock, [&] { return grp->quit || group_has_work(grp, lane); });
-    if (grp->quit) return;
-    auto& queue = grp->plan.queues[grp->plan.lane_queue[lane]];
-    const WorkItem item = queue.front();
-    queue.pop_front();
-    grp->taken = std::max(grp->taken, item.ordinal + 1u);
-    uint32_t iteration = grp->first_iteration + item.ordinal;
-    grp->in_flight += 1;
-    lock.unlock();
-    if (item.parts > 1u) {
-      // this lane renders the camera pass of its part only; the light pass (and so the photon map) in full
-      ctx->rank = item.part;
-      ctx->world = item.parts;
-      ctx->light_full = true;
-    }
-    int rc = etxb_set_next_iteration(ctx, iteration);
-    if (rc == ETXB_OK) rc = run_iteration_blocking(ctx);  // returns when the iteration has finished (the bounce loops read queue sizes back)
-    lock.lock();
-    grp->in_flight -= 1;
-    grp->last_iteration_seconds = ctx->last_iteration_time;
-    if ((rc != ETXB_OK) && (grp->error == ETXB_OK)) {
-      grp->error = rc;
-      grp->error_text = etxb_last_error(ctx);
-      plan_clear(grp->plan);
-    }
-    if (group_idle(grp)) {
-      grp->busy_seconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - grp->busy_since).count();
-      grp->cv_idle.notify_all();
-    }
-  }
-}
-
-// A call the group refuses in its present state: the reason goes to etxb_group_last_error and to lane 0's etxb_last_error
-int group_refuse(etxb_group* grp, const char* why, int code = ETXB_ERR_INVALID_ARGUMENT) {
-  fail(grp->lanes[0], code, "%s", why);
-  std::lock_guard<std::mutex> lock(grp->m);
-  grp->error_text = why;
-  return code;
-}
-
-int group_combine_into(etxb_group* grp, uint32_t layer, DevBuf<float4>& target, uint32_t* completed, bool raw = false) {
-  etxb_ctx* first = grp->lanes[0];
-  if (!first->scene_ready) return fail(first, ETXB_ERR_NOT_READY, "no scene uploaded");
-  size_t n = first->path_count;
-  cudaSetDevice(grp->device);
-  if (target.count < n) CUDA_OK(first, target.alloc(n));
-  FilmLanes f = {};
-  f.lanes = uint32_t(grp->lanes.size());
-  f.layer = layer;
-  f.pixels = uint32_t(n);
-  uint32_t total = 0;
-  for (auto* c : grp->lanes) total += c->completed;
-  for (uint32_t l = 0; l < f.lanes; ++l) {
-    f.camera[l] = grp->lanes[l]->film_camera.ptr;
-    f.light[l] = grp->lanes[l]->film_light.ptr;
-    f.weight[l] = raw ? float(grp->lanes[l]->completed) : (total ? float(double(grp->lanes[l]->completed) / double(total)) : 0.0f);
-    f.weight_light[l] = f.weight[l];
-    f.weight_count[l] = f.weight[l];
-    if (raw && (l == grp->plan.split_lane) && (grp->plan.split_part != 0u)) {
-      // a camera-split lane that is not part 0: its camera tiles count, its (complete, redundant) light image and its iteration count do not
-      f.weight_light[l] = 0.0f;
-      f.weight_count[l] = 0.0f;
-    }
-  }
-  f.raw = raw ? 1u : 0u;
-  // lanes that are still rendering keep updating their films (a preview, like reading the reference's film while it runs); after
-  // etxb_group_wait every lane has synchronised its stream and the result is exact
-  k_film_combine<<<blocks_for(f.pixels, 256), 256, 0, grp->stream>>>(f, target.ptr);
-  CUDA_OK(first, cudaStreamSynchronize(grp->stream));
-  if (completed) *completed = total;
-  return ETXB_OK;
-}
-
 }  // namespace
 
 const char* etxb_build_flavor(void) { return kFlavor; }
@@ -1982,36 +1236,6 @@ int etxb_upload_blue_noise(etxb_ctx* ctx, const uint8_t* sobol_256x256, const ui
   ctx->dscene.has_blue_noise = 1;
   CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
   return ETXB_OK;
-}
-
-int etxb_upload_scene(etxb_ctx* ctx, const void* scene_blob, uint64_t scene_bytes, const void* camera_blob, uint64_t camera_bytes) {
-  if (!ctx || !scene_blob || !camera_blob) return ETXB_ERR_INVALID_ARGUMENT;
-  if (int rc = check_scene_args(ctx, scene_bytes, camera_bytes)) return rc;
-  ctx_drain(ctx);
-  cudaSetDevice(ctx->device);
-  ctx->scene_ready = false;
-  const etxb_scene& s = *static_cast<const etxb_scene*>(scene_blob);
-  const etxb_camera& cam = *static_cast<const etxb_camera*>(camera_blob);
-  ScenePrep p;
-  if (int rc = prepare_scene(ctx, s, cam, p)) return rc;
-  return commit_scene(ctx, s, cam, p, false, nullptr);
-}
-
-int etxb_update_scene(etxb_ctx* ctx, const void* scene_blob, uint64_t scene_bytes, const void* camera_blob, uint64_t camera_bytes, etxb_update_info* info) {
-  const auto t0 = std::chrono::steady_clock::now();
-  if (info) memset(info, 0, sizeof(*info));
-  if (!ctx || !scene_blob || !camera_blob) return ETXB_ERR_INVALID_ARGUMENT;
-  if (int rc = check_scene_args(ctx, scene_bytes, camera_bytes)) return rc;
-  if (ctx->comm != nullptr) return fail(ctx, ETXB_ERR_UNSUPPORTED, "etxb_update_scene: a context with a communicator takes a new scene through etxb_upload_scene");
-  ctx_drain(ctx);
-  cudaSetDevice(ctx->device);
-  const etxb_scene& s = *static_cast<const etxb_scene*>(scene_blob);
-  const etxb_camera& cam = *static_cast<const etxb_camera*>(camera_blob);
-  ScenePrep p;
-  if (int rc = prepare_scene(ctx, s, cam, p)) return rc;
-  int rc = commit_scene(ctx, s, cam, p, ctx->scene_ready, info);
-  if (info) info->total_seconds = seconds_since(t0);
-  return rc;
 }
 
 void etxb_options_default(etxb_vcm_options* opt) {
@@ -2222,41 +1446,19 @@ int etxb_comm_reduce_film(etxb_ctx* ctx, uint32_t layer, float* dst_rgba, uint64
   if (!ctx->scene_ready) return fail(ctx, ETXB_ERR_NOT_READY, "no scene uploaded");
   if (ctx->comm == nullptr) return etxb_read_film(ctx, layer, dst_rgba, dst_bytes);
   if (int rc = ctx_drain(ctx)) return rc;
-  NcclApi* n = nccl_api();
   cudaSetDevice(ctx->device);
   const size_t px = ctx->path_count;
   if (ctx->film_reduced.count < px) CUDA_OK(ctx, ctx->film_reduced.alloc(px));
-  // the tiled layers: each rank holds its own tiles and zeros elsewhere (k_pt_accumulate and k_film_adaptive_vcm write owned pixels only)
-  const float4* tiles = ctx->film_camera.ptr;
-  if ((layer == ETXB_FILM_NORMALS) || (layer == ETXB_FILM_ALBEDO)) {
-    if (int rc = pt_ensure_film(ctx)) return rc;
-    tiles = (layer == ETXB_FILM_NORMALS) ? ctx->film_normals.ptr : ctx->film_albedo.ptr;
-  } else if (layer == ETXB_FILM_CAMERA_ADAPTIVE) {
-    if (int rc = film_ensure_adaptive(ctx)) return rc;
-    tiles = ctx->film_adaptive.ptr;
+  if (layer != ETXB_FILM_LIGHT) {
+    // the tiled layers: each rank holds its own tiles and zeros elsewhere (k_pt_accumulate and k_film_adaptive_vcm write owned pixels only)
+    float4* tiles = nullptr;
+    if (int rc = film_layer_raw(ctx, layer, &tiles)) return rc;
+    NCCL_OK(ctx, nccl_api()->Reduce(tiles, ctx->film_reduced.ptr, px * 4u, ncclFloat, ncclSum, 0, ctx->comm, ctx->stream));
   }
-  if (layer != ETXB_FILM_LIGHT)
-    NCCL_OK(ctx, n->Reduce(tiles, ctx->film_reduced.ptr, px * 4u, ncclFloat, ncclSum, 0, ctx->comm, ctx->stream));
-  if (ctx->rank != 0u) {
-    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+  return end_rank0_reduce(ctx, ctx->stream, ctx->rank, dst_rgba, dst_bytes, px, [&](const float4** src) -> int {
+    *src = (layer == ETXB_FILM_LIGHT) ? ctx->film_light.ptr : film_layer_read_out(ctx, layer, ctx->film_reduced.ptr);
     return ETXB_OK;
-  }
-  if (!dst_rgba || (dst_bytes < px * 16u)) return fail(ctx, ETXB_ERR_INVALID_ARGUMENT, "film buffer too small");
-  const float4* src = (layer == ETXB_FILM_LIGHT) ? ctx->film_light.ptr : ctx->film_reduced.ptr;
-  if (layer == ETXB_FILM_NORMALS) {  // etxb_read_film's read-out (Film::layer: n * 0.5 + 0.5)
-    k_film_layer_normals<<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(ctx->film_reduced.ptr, ctx->film_out.ptr, ctx->path_count);
-    ctx->kernel_launches += 1;
-    src = ctx->film_out.ptr;
-  }
-  if (layer == ETXB_FILM_RESULT) {
-    FilmBuffers film = {ctx->film_reduced.ptr, ctx->film_light.ptr, ctx->film_light_iteration.ptr, ctx->width, ctx->height};
-    k_film_resolve<<<blocks_for(ctx->path_count, 256), 256, 0, ctx->stream>>>(film, ctx->film_out.ptr);
-    ctx->kernel_launches += 1;
-    src = ctx->film_out.ptr;
-  }
-  CUDA_OK(ctx, cudaMemcpyAsync(dst_rgba, src, px * 16u, cudaMemcpyDeviceToHost, ctx->stream));
-  CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-  return ETXB_OK;
+  });
 }
 
 int etxb_poll(etxb_ctx* ctx, etxb_status* status) {
@@ -2754,311 +1956,5 @@ int etxb_debug_merge(etxb_ctx* ctx, const void* records, uint32_t record_count, 
   grid->merge_queries = after.merge_queries - before.merge_queries;
   grid->merge_candidates = after.merge_candidates - before.merge_candidates;
   grid->merge_accepts = after.merge_accepts - before.merge_accepts;
-  return ETXB_OK;
-}
-
-// ---- iterations in flight (etxb_group) ----------------------------------------------------------------------------------------------------
-int etxb_group_create(etxb_group** out, const etxb_device_config* cfg, uint32_t lanes) {
-  if (!out || (lanes == 0) || (lanes > kMaxLanes)) return ETXB_ERR_INVALID_ARGUMENT;
-  *out = nullptr;
-  auto* grp = new etxb_group();
-  grp->device = cfg ? cfg->device_index : 0;
-  for (uint32_t l = 0; l < lanes; ++l) {
-    etxb_ctx* ctx = nullptr;
-    int rc = etxb_create(&ctx, cfg);
-    if (rc != ETXB_OK) {
-      for (auto* c : grp->lanes) etxb_destroy(c);
-      delete grp;
-      return rc;
-    }
-    ctx->group_lane = true;
-    grp->lanes.push_back(ctx);
-  }
-  grp->plan.queues.resize(lanes);
-  grp->plan.lane_queue.assign(lanes, 0u);
-  cudaSetDevice(grp->device);
-  create_priority_stream(&grp->stream);  // the frame combine / reduce
-  for (uint32_t l = 0; l < lanes; ++l) grp->workers.emplace_back(group_worker, grp, l);
-  *out = grp;
-  return ETXB_OK;
-}
-
-void etxb_group_destroy(etxb_group* grp) {
-  if (!grp) return;
-  {
-    std::lock_guard<std::mutex> lock(grp->m);
-    grp->quit = true;
-  }
-  grp->cv_work.notify_all();
-  for (auto& w : grp->workers) w.join();
-  cudaSetDevice(grp->device);
-  if (grp->reduce_comm != nullptr) {
-    if (NcclApi* n = nccl_api()) n->CommDestroy(grp->reduce_comm);
-  }
-  if (grp->stream) cudaStreamDestroy(grp->stream);
-  for (auto* c : grp->lanes) etxb_destroy(c);
-  delete grp;
-}
-
-uint32_t etxb_group_lanes(const etxb_group* grp) { return grp ? uint32_t(grp->lanes.size()) : 0u; }
-etxb_ctx* etxb_group_lane(etxb_group* grp, uint32_t lane) { return (grp && (lane < grp->lanes.size())) ? grp->lanes[lane] : nullptr; }
-const char* etxb_group_last_error(const etxb_group* grp) { return grp ? grp->error_text.c_str() : "null group"; }
-
-int etxb_group_wait(etxb_group* grp) {
-  if (!grp) return ETXB_ERR_INVALID_ARGUMENT;
-  std::unique_lock<std::mutex> lock(grp->m);
-  grp->cv_idle.wait(lock, [&] { return group_idle(grp); });
-  return grp->error;
-}
-
-int etxb_group_begin(etxb_group* grp, uint32_t first_iteration) {
-  if (!grp) return ETXB_ERR_INVALID_ARGUMENT;
-  if (int rc = etxb_group_wait(grp)) return rc;
-  for (auto* c : grp->lanes)
-    if (int rc = etxb_begin(c, first_iteration)) return rc;
-  std::lock_guard<std::mutex> lock(grp->m);
-  grp->first_iteration = first_iteration;
-  grp->taken = 0;
-  plan_clear(grp->plan);
-  grp->plan.split_part = grp->plan.split_parts = 0;
-  grp->busy_seconds = 0.0;
-  grp->error = ETXB_OK;
-  grp->error_text.clear();
-  return ETXB_OK;
-}
-
-int etxb_group_set_film_pixel_size(etxb_group* grp, uint32_t size) {
-  if (!grp) return ETXB_ERR_INVALID_ARGUMENT;
-  if ((size > 1u) && ((grp->plan.mode != GroupMode::local) || (grp->reduce_comm != nullptr)))
-    return group_refuse(grp, "etxb_group_set_film_pixel_size: a group with communicators renders film pixels in tiles or parts; the coarse preview renders on one GPU", ETXB_ERR_UNSUPPORTED);
-  if (int rc = etxb_group_wait(grp)) return rc;
-  for (auto* c : grp->lanes) {
-    if (int rc = etxb_set_film_pixel_size(c, size)) {
-      std::lock_guard<std::mutex> lock(grp->m);
-      grp->error_text = etxb_last_error(c);
-      return rc;
-    }
-  }
-  return ETXB_OK;
-}
-
-int etxb_group_update_scene(etxb_group* grp, const void* scene_blob, uint64_t scene_bytes, const void* camera_blob, uint64_t camera_bytes, etxb_update_info* info) {
-  const auto t0 = std::chrono::steady_clock::now();
-  if (info) memset(info, 0, sizeof(*info));
-  if (!grp || !scene_blob || !camera_blob) return ETXB_ERR_INVALID_ARGUMENT;
-  etxb_ctx* first = grp->lanes[0];
-  auto refuse = [&](int rc) {
-    std::lock_guard<std::mutex> lock(grp->m);
-    grp->error_text = etxb_last_error(first);
-    return rc;
-  };
-  bool comm = grp->plan.mode != GroupMode::local;
-  for (auto* c : grp->lanes) comm = comm || (c->comm != nullptr);
-  if (comm) return refuse(fail(first, ETXB_ERR_UNSUPPORTED, "etxb_group_update_scene: a group with communicators takes a new scene through etxb_upload_scene on each lane"));
-  if (int rc = check_scene_args(first, scene_bytes, camera_bytes)) return refuse(rc);
-  if (int rc = etxb_group_wait(grp)) return rc;
-  const etxb_scene& s = *static_cast<const etxb_scene*>(scene_blob);
-  const etxb_camera& cam = *static_cast<const etxb_camera*>(camera_blob);
-  cudaSetDevice(grp->device);
-  // hashed and validated once; a new geometry's BVH is built once, and its depth checked, before any lane changes
-  ScenePrep p;
-  if (int rc = prepare_scene(first, s, cam, p)) return refuse(rc);
-  for (auto* c : grp->lanes)
-    if (!geometry_kept(c, p, c->scene_ready))
-      if (int rc = prepare_bvh(first, s, p)) return refuse(rc);
-  uint32_t kept = ~0u;
-  for (size_t l = 0; l < grp->lanes.size(); ++l) {
-    etxb_ctx* c = grp->lanes[l];
-    etxb_update_info lane = {};
-    ctx_drain(c);
-    if (int rc = commit_scene(c, s, cam, p, c->scene_ready, &lane)) {
-      std::lock_guard<std::mutex> lock(grp->m);
-      grp->error_text = etxb_last_error(c);
-      return rc;
-    }
-    kept &= lane.kept;
-    if (info && (l == 0)) *info = lane;
-  }
-  if (info) {
-    info->kept = kept;  // what every lane kept; the image and grid counts are lane 0's
-    info->total_seconds = seconds_since(t0);
-  }
-  return etxb_group_begin(grp, 0);
-}
-
-int etxb_group_enqueue(etxb_group* grp, uint32_t iterations) {
-  if (!grp) return ETXB_ERR_INVALID_ARGUMENT;
-  {
-    std::lock_guard<std::mutex> lock(grp->m);
-    if (grp->error != ETXB_OK) return grp->error;
-    if (iterations == 0) return ETXB_OK;
-    if (group_idle(grp)) grp->busy_since = std::chrono::steady_clock::now();
-    plan_enqueue(grp->plan, iterations);
-  }
-  grp->cv_work.notify_all();
-  return ETXB_OK;
-}
-
-int etxb_group_poll(etxb_group* grp, etxb_status* status) {
-  if (!grp || !status) return ETXB_ERR_INVALID_ARGUMENT;
-  memset(status, 0, sizeof(*status));
-  std::lock_guard<std::mutex> lock(grp->m);
-  for (size_t l = 0; l < grp->lanes.size(); ++l) {
-    etxb_ctx* c = grp->lanes[l];
-    // a camera-split iteration is finished by several ranks: it counts where part 0 ran
-    if (!((l == grp->plan.split_lane) && (grp->plan.split_part != 0u))) status->completed_iterations += c->completed;
-    status->light_vertices = std::max(status->light_vertices, c->last_light_vertices);
-    status->overflow |= c->overflow_flag;
-  }
-  status->current_iteration = grp->first_iteration + grp->taken;
-  status->iteration_in_flight = group_idle(grp) ? 0u : 1u;
-  status->last_iteration_time = grp->last_iteration_seconds;
-  status->total_time = grp->busy_seconds;
-  if (status->iteration_in_flight) status->total_time += std::chrono::duration<double>(std::chrono::steady_clock::now() - grp->busy_since).count();
-  return ETXB_OK;
-}
-
-// Pixel tiles over several processes, `lanes` iterations in flight on each: ids = (lanes + 1) NCCL unique ids of 128 bytes, the same on every
-// rank (lane l of every rank forms communicator l; the last one carries the frame reduce).  Collective.  Refused, before any NCCL call and so
-// alike on every rank, on a group that already has a communicator or, for world >= 2, a split lane.
-int etxb_group_comm_init(etxb_group* grp, uint32_t world, uint32_t rank, const void* ids, uint32_t id_count) {
-  if (!grp || !ids || (world == 0u) || (rank >= world) || (id_count != grp->lanes.size() + 1u)) return ETXB_ERR_INVALID_ARGUMENT;
-  if (int rc = etxb_group_wait(grp)) return rc;
-  if (grp->reduce_comm != nullptr) return group_refuse(grp, "etxb_group_comm_init: the group already has a communicator");
-  if ((world > 1u) && (grp->plan.split_lane != 0xffffffffu)) return group_refuse(grp, "etxb_group_comm_init: pixel tiles and a split lane exclude each other");
-  for (auto* c : grp->lanes) {
-    if (c->target_pixel_size > 1u) return group_refuse(grp, "etxb_group_comm_init: the coarse preview (film pixel size above 1) renders on one GPU", ETXB_ERR_UNSUPPORTED);
-    if ((world > 1u) && (c->integrator == ETXB_INTEGRATOR_PT))
-      return group_refuse(grp, "etxb_group_comm_init: the path tracer does not run on a group in pixel-tile mode: each lane would keep its own per-pixel history", ETXB_ERR_UNSUPPORTED);
-  }
-  const uint8_t* bytes = static_cast<const uint8_t*>(ids);
-  for (size_t l = 0; l < grp->lanes.size(); ++l) {
-    if (int rc = etxb_comm_init(grp->lanes[l], world, rank, bytes + l * sizeof(ncclUniqueId), sizeof(ncclUniqueId))) {
-      grp->error_text = etxb_last_error(grp->lanes[l]);
-      return rc;
-    }
-  }
-  cudaSetDevice(grp->device);
-  if (int rc = comm_init_rank(grp->lanes[0], &grp->reduce_comm, world, rank, bytes + grp->lanes.size() * sizeof(ncclUniqueId))) return rc;
-  std::lock_guard<std::mutex> lock(grp->m);
-  grp->plan.mode = (world > 1u) ? GroupMode::tiles : GroupMode::local;
-  grp->plan.world = world;
-  grp->plan.rank = rank;
-  grp->plan.enqueued = 0;
-  return ETXB_OK;
-}
-
-// Test hook (no device needed): the queues of a `lanes`-lane group in `mode` (0 local, 1 tiles, 2 replicas) on rank `rank` of `world`, with its
-// last lane reserved for camera-split iterations if `split_lane`, after etxb_group_enqueue(enqueues[0]), ..., (enqueues[count - 1]) — quads
-// (queue, ordinal, part, parts) into out, queue by queue in the order the lanes pop them; returns their number.
-int etxb_debug_group_plan(uint32_t mode, uint32_t lanes, uint32_t world, uint32_t rank, int split_lane, const uint32_t* enqueues, uint32_t count,
-                          uint32_t* out_quads, uint32_t capacity) {
-  if ((mode > uint32_t(GroupMode::replicas)) || (lanes == 0u) || (lanes > kMaxLanes) || (world == 0u) || (rank >= world) || (!enqueues && count) || !out_quads)
-    return ETXB_ERR_INVALID_ARGUMENT;
-  if (split_lane && ((lanes < 2u) || (GroupMode(mode) == GroupMode::tiles))) return ETXB_ERR_INVALID_ARGUMENT;
-  WorkPlan p;
-  p.mode = GroupMode(mode);
-  p.world = world;
-  p.rank = rank;
-  p.queues.resize(lanes);
-  p.lane_queue.assign(lanes, 0u);
-  if (split_lane) p.split_lane = lanes - 1u;
-  for (uint32_t i = 0; i < count; ++i) plan_enqueue(p, enqueues[i]);
-  uint32_t n = 0;
-  for (uint32_t q = 0; q < lanes; ++q)
-    for (const WorkItem& it : p.queues[q]) {
-      if (n >= capacity) return int(n);
-      uint32_t* o = out_quads + 4u * n++;
-      o[0] = q, o[1] = it.ordinal, o[2] = it.part, o[3] = it.parts;
-    }
-  return int(n);
-}
-
-// Replica mode: reserves the group's LAST lane for camera-split iterations (see replica_plan); it takes no whole-frame iterations.  Call before
-// etxb_group_comm_init_replicas; needs at least two lanes, and is refused on a group in tile mode.
-int etxb_group_reserve_split_lane(etxb_group* grp) {
-  if (!grp || (grp->lanes.size() < 2u)) return ETXB_ERR_INVALID_ARGUMENT;
-  if (int rc = etxb_group_wait(grp)) return rc;
-  if (grp->plan.mode == GroupMode::tiles) return group_refuse(grp, "etxb_group_reserve_split_lane: pixel tiles and a split lane exclude each other");
-  std::lock_guard<std::mutex> lock(grp->m);
-  grp->plan.split_lane = uint32_t(grp->lanes.size()) - 1u;
-  return ETXB_OK;
-}
-
-// The other way to split a K-iteration render over the ranks: whole-frame iterations, the job's j-th iteration on rank j % world (each rank's
-// lanes take that rank's share in order).  No collective inside an iteration; one ncclReduce of the (count-weighted) films per frame.  id = one
-// NCCL unique id.  Collective.  Refused, before any NCCL call, on a group that already has a communicator.
-int etxb_group_comm_init_replicas(etxb_group* grp, uint32_t world, uint32_t rank, const void* id, uint64_t bytes) {
-  if (!grp || !id || (bytes < sizeof(ncclUniqueId)) || (world == 0u) || (rank >= world)) return ETXB_ERR_INVALID_ARGUMENT;
-  if (int rc = etxb_group_wait(grp)) return rc;
-  if (grp->reduce_comm != nullptr) return group_refuse(grp, "etxb_group_comm_init_replicas: the group already has a communicator");
-  for (auto* c : grp->lanes)
-    if (c->target_pixel_size > 1u) return group_refuse(grp, "etxb_group_comm_init_replicas: the coarse preview (film pixel size above 1) renders on one GPU", ETXB_ERR_UNSUPPORTED);
-  cudaSetDevice(grp->device);
-  if (int rc = comm_init_rank(grp->lanes[0], &grp->reduce_comm, world, rank, id)) return rc;
-  std::lock_guard<std::mutex> lock(grp->m);
-  grp->plan.mode = (world > 1u) ? GroupMode::replicas : GroupMode::local;
-  grp->plan.world = world;
-  grp->plan.rank = rank;
-  grp->plan.enqueued = 0;
-  return ETXB_OK;
-}
-
-// Collective over the ranks of a sharded group: the lanes' films are combined locally (mean weighted by the iterations each lane finished —
-// the same weights on every rank, the lane -> iteration map is fixed), the camera tiles are summed on rank 0, Result = max(0, camera + light).
-int etxb_group_comm_reduce_film(etxb_group* grp, uint32_t layer, float* dst_rgba, uint64_t dst_bytes) {
-  if (!grp || (layer > ETXB_FILM_LIGHT)) return ETXB_ERR_INVALID_ARGUMENT;
-  if (grp->plan.mode == GroupMode::local) return etxb_group_read_film(grp, layer, dst_rgba, dst_bytes);
-  NcclApi* n = nccl_api();
-  etxb_ctx* first = grp->lanes[0];
-  const size_t px = first->path_count;
-  cudaSetDevice(grp->device);
-  if (grp->plan.mode == GroupMode::replicas) {
-    // every rank: sum over its lanes of (iterations finished x mean film), .w = iterations; rank 0 divides the reduced sum by the reduced count
-    if (int rc = group_combine_into(grp, layer, grp->combined, nullptr, true)) return rc;
-    if (grp->reduced.count < px) CUDA_OK(first, grp->reduced.alloc(px));
-    NCCL_OK(first, n->Reduce(grp->combined.ptr, grp->reduced.ptr, px * 4u, ncclFloat, ncclSum, 0, grp->reduce_comm, grp->stream));
-    if (grp->plan.rank != 0u) {
-      CUDA_OK(first, cudaStreamSynchronize(grp->stream));
-      return ETXB_OK;
-    }
-    if (!dst_rgba || (dst_bytes < px * 16u)) return fail(first, ETXB_ERR_INVALID_ARGUMENT, "film buffer too small");
-    k_film_finish_mean<<<blocks_for(uint32_t(px), 256), 256, 0, grp->stream>>>(grp->reduced.ptr, grp->combined.ptr, uint32_t(px), (layer == ETXB_FILM_RESULT) ? 1u : 0u);
-    CUDA_OK(first, cudaMemcpyAsync(dst_rgba, grp->combined.ptr, px * 16u, cudaMemcpyDeviceToHost, grp->stream));
-    CUDA_OK(first, cudaStreamSynchronize(grp->stream));
-    return ETXB_OK;
-  }
-  if (layer != ETXB_FILM_LIGHT) {
-    if (int rc = group_combine_into(grp, ETXB_FILM_CAMERA, grp->combined, nullptr)) return rc;
-    if (grp->reduced.count < px) CUDA_OK(first, grp->reduced.alloc(px));
-    NCCL_OK(first, n->Reduce(grp->combined.ptr, grp->reduced.ptr, px * 4u, ncclFloat, ncclSum, 0, grp->reduce_comm, grp->stream));
-  }
-  if (grp->plan.rank != 0u) {
-    CUDA_OK(first, cudaStreamSynchronize(grp->stream));
-    return ETXB_OK;
-  }
-  if (!dst_rgba || (dst_bytes < px * 16u)) return fail(first, ETXB_ERR_INVALID_ARGUMENT, "film buffer too small");
-  const float4* src = grp->reduced.ptr;
-  if (layer != ETXB_FILM_CAMERA) {
-    if (int rc = group_combine_into(grp, ETXB_FILM_LIGHT, grp->combined_light, nullptr)) return rc;
-    src = grp->combined_light.ptr;
-  }
-  if (layer == ETXB_FILM_RESULT) {
-    FilmBuffers film = {grp->reduced.ptr, grp->combined_light.ptr, nullptr, first->width, first->height};
-    k_film_resolve<<<blocks_for(uint32_t(px), 256), 256, 0, grp->stream>>>(film, grp->combined.ptr);
-    src = grp->combined.ptr;
-  }
-  CUDA_OK(first, cudaMemcpyAsync(dst_rgba, src, px * 16u, cudaMemcpyDeviceToHost, grp->stream));
-  CUDA_OK(first, cudaStreamSynchronize(grp->stream));
-  return ETXB_OK;
-}
-
-int etxb_group_read_film(etxb_group* grp, uint32_t layer, float* dst_rgba, uint64_t dst_bytes) {
-  if (!grp || !dst_rgba || (layer > ETXB_FILM_LIGHT)) return ETXB_ERR_INVALID_ARGUMENT;
-  if (int rc = group_combine_into(grp, layer, grp->combined, nullptr)) return rc;
-  etxb_ctx* first = grp->lanes[0];
-  const uint64_t bytes = uint64_t(first->path_count) * 16u;
-  if (dst_bytes < bytes) return fail(first, ETXB_ERR_INVALID_ARGUMENT, "film buffer too small");
-  CUDA_OK(first, cudaMemcpy(dst_rgba, grp->combined.ptr, bytes, cudaMemcpyDeviceToHost));
   return ETXB_OK;
 }

@@ -190,7 +190,7 @@ def _material_case(kind, spectral, queries_n):
 
 
 def _always_delta(m):
-    """module.cu validate_scene: a material no vertex of the camera pass merges at (smooth conductor or dielectric, thin film, mirror, void)"""
+    """scene_upload.cu validate_scene: a material no vertex of the camera pass merges at (smooth conductor or dielectric, thin film, mirror, void)"""
     smooth = max(float(m["roughness"]["value"][0]), float(m["roughness"]["value"][1])) <= 1e-4 and int(m["roughness"]["image_index"]) == S.INVALID
     return (int(m["cls"]) in (S.MAT_DIELECTRIC, S.MAT_CONDUCTOR) and smooth) or int(m["cls"]) in (S.MAT_THINFILM, S.MAT_MIRROR, S.MAT_VOID)
 

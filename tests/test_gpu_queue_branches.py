@@ -35,7 +35,7 @@ def _connect_only():
 
 
 def _stochastic(sd):
-    """the scene has a surface the generic gather and the connection stage handle (module.cu validate_scene: not Lambert, not always delta)"""
+    """the scene has a surface the generic gather and the connection stage handle (scene_upload.cu validate_scene: not Lambert, not always delta)"""
     for m in sd.a_materials:
         lambert = int(m["cls"]) == S.MAT_DIFFUSE and int(m["diffuse_variation"]) == 0
         smooth = max(float(m["roughness"]["value"][0]), float(m["roughness"]["value"][1])) <= 1e-4 and int(m["roughness"]["image_index"]) == S.INVALID

@@ -157,7 +157,7 @@ def _group_plan(lib, mode, lanes, world, rank, split, enqueues):
 
 
 def test_work_plan_deals_every_iteration_exactly_once():
-    """etxb_group_enqueue's work plan (module.cu plan_enqueue, through the device-free test hook etxb_debug_group_plan).
+    """etxb_group_enqueue's work plan (group.cu plan_enqueue, through the device-free test hook etxb_debug_group_plan).
     Replica mode: whole frames round-robin; with a split lane the n % world left-over iterations are split over world / (n % world) ranks each by
     camera tile.  Whatever (world, n): every ordinal is rendered exactly once — by one rank as a whole frame, or by `parts` ranks holding the
     parts 0 .. parts - 1 — and no rank carries more than ceil(n / world) units of work.  Whole frames wait in queue 0, split parts in the split
